@@ -38,11 +38,12 @@ def peaks():
             d = json.load(f)
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 / FP16
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -167,6 +168,26 @@ def run_reference(args):
     print(json.dumps(line), flush=True)
 
 
+def dump_outputs(out_dir, ws, gathered=None):
+    """What a caller of the timed step receives, from its last step: per utterance the token ids (padding beyond the
+    count set to -1), the token count, the score sum / count and the status flag — with N > 1 GPUs taken from the
+    gathered buffer, i.e. every rank's utterances in rank order — and per frame the greedy id and its probability (this
+    rank's frames: they are not gathered).  float64 (ids and counts are exact), one .npy per array."""
+    os.makedirs(out_dir, exist_ok=True)
+    B, Tt = ws["tokens"].shape
+    n = B * Tt + 4 * B                                # one rank's out_pack: tokens | ntok | pcount | status | psum
+    packs = (gathered if gathered is not None else ws["out_pack"]).cpu().numpy().reshape(-1, n)
+    tokens = packs[:, :B * Tt].reshape(-1, Tt).astype(np.float64)
+    ntok = packs[:, B * Tt:B * Tt + B].reshape(-1)
+    tokens[np.arange(Tt)[None, :] >= ntok[:, None]] = -1
+    arrays = {"tokens": tokens, "ntok": ntok, "pcount": packs[:, B * Tt + B:B * Tt + 2 * B].reshape(-1),
+              "status": packs[:, B * Tt + 2 * B:B * Tt + 3 * B].reshape(-1),
+              "psum": np.ascontiguousarray(packs[:, B * Tt + 3 * B:]).view(np.float32).reshape(-1),
+              "frame_ids": ws["ids"].cpu().numpy(), "frame_maxp": ws["maxp"].cpu().numpy()}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float64))
+
+
 # ------------------------------------------------------------------------------------------------
 def main():
     ap = argparse.ArgumentParser()
@@ -177,6 +198,8 @@ def main():
     ap.add_argument("--ref-sample", type=int, default=4, help="utterances per step of the reference CPU arm")
     ap.add_argument("--cpu-baseline-utts", type=int, default=6)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 0)
     if args.impl == "reference":
@@ -201,7 +224,7 @@ def main():
     numa = None
     if world > 1 and os.environ.get("MASR_BENCH_AFFINITY", "1") != "0":
         # one process per GPU: keep this rank's staging threads and its pinned buffers on the CPUs / NUMA node next to ITS GPU
-        # (8 ranks x (4 stager threads + 20 MB pinned memcpy per step) otherwise contend across sockets: e2e efficiency 0.91 at N=8 in r01)
+        # (8 ranks x (4 stager threads + 20 MB pinned memcpy per step) otherwise contend across sockets)
         try:
             import pynvml
             pynvml.nvmlInit()
@@ -249,7 +272,7 @@ def main():
     lengths = [UTT_SAMPLES] * BATCH_PER_GPU
     offs = torch.tensor(np.arange(BATCH_PER_GPU + 1, dtype=np.int64) * UTT_SAMPLES, device=dev)
     wave_dev = torch.from_numpy(np.concatenate(waves)).to(dev)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 50 MB L2
 
     T = 248
     gather_state = {}
@@ -330,11 +353,13 @@ def main():
         flush.zero_()                         # L2 flush between timed iterations (outside the event bracket)
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        device_step()
+        ws_last = device_step()
         e1.record()
         evs.append((e0, e1))
     barrier()
     wall = time.perf_counter() - wall0
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        dump_outputs(args.dump_outputs, ws_last, gather_state[("gbuf", ws_last["out_pack"].numel())] if world > 1 else None)
     launches = (eng.launches - launches0) // max(1, args.steps)
     dev_ms = sum(a.elapsed_time(b) for a, b in evs) / args.steps
     t = torch.tensor([dev_ms], device=dev, dtype=torch.float64)
@@ -463,13 +488,7 @@ def main():
         flops = 2.0 * M * 256 * 2048                 # per launch (w_1 and w_2 have the same FLOPs)
         achieved = flops / (ffn_ms * 1e-3) / 1e12
         traffic = None
-        tp = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-        if os.path.exists(tp):
-            try:
-                traffic = json.load(open(tp)).get("ffn_gemm_dram_bytes_per_launch")
-            except Exception:
-                traffic = None
-        kname = ("tc_gemm_kernel (FFN w_1/w_2; tcgen05 kind::f16, FP16x2 split = 3 MMAs per K-step, fp32-grade)"
+        kname = ("tc_gemm_kernel (FFN w_1/w_2; wgmma f16, FP16x2 split = 3 MMAs per K-step, fp32-grade)"
                  if eng.gemm_path == "tc" else "sgemm_tn_kernel<128,128> (FFN w_1/w_2, fp32 FMA pipe)")
         roof = {"kernel": kname, "bound": "tensor", "achieved": achieved,
                 "peak": pk["bf16_tflops_sustained"], "unit": "TFLOP/s", "frac": achieved / pk["bf16_tflops_sustained"],
@@ -502,7 +521,7 @@ def main():
     if rank == 0:
         line = {"metric": "audio_seconds_per_second", "value": value, "unit": "audio-s/s", "n_gpus": world,
                 "steps": args.steps, "warmup": args.warmup, "ms_per_step": dev_ms, "higher_is_better": True,
-                "scaling": "weak", "vs_baseline": None, "dtype": "f32 (GEMMs: fp16x2-split operands on tcgen05, fp32 accumulate; fp32-grade results)" if eng.gemm_path == "tc" else "f32",
+                "scaling": "weak", "vs_baseline": None, "dtype": "f32 (GEMMs: fp16x2-split operands on wgmma, fp32 accumulate; fp32-grade results)" if eng.gemm_path == "tc" else "f32",
                 "data": "synthetic",
                 "config": {"workload": WORKLOAD, "cuda_graph": bool(eng.use_graphs), "global_batch": BATCH_PER_GPU * world, "parallelism": f"dp{world} (utterance shard)",
                            "l2": "flushed between timed steps (256 MiB memset outside the event bracket)",
@@ -529,7 +548,7 @@ def main():
         sys.stderr.flush()
         if graph_gather:
             # CUDA graphs that captured NCCL kernels still reference the communicator; destroy_process_group() then waits
-            # forever (seen at N=2, r02).  Everything is measured and printed: leave without tearing NCCL down.
+            # forever.  Everything is measured and printed: leave without tearing NCCL down.
             os._exit(0)
         dist.destroy_process_group()
 

@@ -1,4 +1,4 @@
-/* masr_b200 — C ABI of the B200-native MASR inference hot path.
+/* masr_b200 — C ABI of the H100-native MASR inference hot path.
  *
  * The reference (yeyupiaoling/MASR) is pure Python and has NO FFI of its own: its hot path is
  * `MASRPredictor.predict / predict_stream` (masr/predict.py:167,237) -> `AudioFeaturizer.featurize`
@@ -16,7 +16,7 @@
  *   - `stream` is a cudaStream_t passed as void*; all work is enqueued asynchronously on it;
  *   - float32 everywhere ("f32" suffix), row-major, leading dimensions (`ld*`) in elements;
  *   - returns MASR_OK (0) or an error code; `masr_last_error()` has the message (thread-local);
- *   - there is no CPU fallback: without an sm_100 device the calls fail.
+ *   - there is no CPU fallback: without an sm_90 device the calls fail.
  */
 #ifndef MASR_B200_H_
 #define MASR_B200_H_
@@ -102,7 +102,7 @@ int masr_gemm_f32(const float* A, int64_t lda, const float* W, const float* bias
                   int64_t ldr, float* C, int64_t ldc, int M, int N, int K, int epilogue, float alpha,
                   void* stream);
 
-/* Tensor-core (tcgen05/TMEM/TMA) variant of masr_gemm_f32 with fp32-grade results: operands are fp16
+/* Tensor-core (wgmma/TMA) variant of masr_gemm_f32 with fp32-grade results: operands are fp16
  * (h, l) pairs, h = fp16(x), l = fp16((x - h) * 2^11) (masr_split_f16); C ~= Ah.Wh^T + 2^-11 (Ah.Wl^T + Al.Wh^T)
  * accumulated in fp32.  Output: fp32 C and/or the (Ch, Cl) pair the next GEMM consumes (either may be NULL,
  * not both).  K % 64 == 0, lda % 8 == 0, ldc % 8 == 0 (ldc % 4 when only fp32 is written); W is [N, K] dense. */
@@ -225,7 +225,7 @@ int masr_relpos_attention_tc(const float* Q, int64_t ldq, int64_t q_bstride, con
                              int64_t o_bstride, const int* q_lens, const int* k_lens, int B, int H, int d_k, int max_q,
                              void* stream);
 
-/* masr_relpos_attention_tc on the 5th-generation tensor cores (tcgen05.mma, S and O accumulators in TMEM, K / linear_pos(pe) / V
+/* masr_relpos_attention_tc on the Hopper tensor cores (wgmma, S and O accumulators in registers, K / linear_pos(pe) / V
  * tiles by TMA, V consumed as an MN-major operand, softmax between the two products inside the kernel): one CTA per
  * (utterance, head), for utterances of up to 256 frames — max_q <= 256 and every k_lens[b] <= 256 (the batched whole-utterance
  * path of 10 s audio: T = 248).  Same arguments plus `table_rows` (rows of the P table), same results (fp32-grade). */

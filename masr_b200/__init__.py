@@ -1,4 +1,4 @@
-"""masr_b200 — a B200-native (sm_100a) implementation of MASR's inference hot path
+"""masr_b200 — a H100-native (sm_90a) implementation of MASR's inference hot path
 (fbank -> Conformer-family encoder -> CTC greedy / prefix beam) behind the reference's
 ``MASRPredictor.predict / predict_stream`` interface.  See DESIGN.md."""
 

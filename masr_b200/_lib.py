@@ -92,7 +92,7 @@ def load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise MasrB200Error(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). masr_b200 has no CPU or PyTorch fallback.")
+            "(nvcc, sm_90a). masr_b200 has no CPU or PyTorch fallback.")
     lib = C.CDLL(LIB_PATH)
     lib.masr_last_error.restype = C.c_char_p
     lib.masr_last_error.argtypes = []

@@ -1,4 +1,4 @@
-"""In-tree build of libmasr_b200.so with nvcc for sm_100a (no torch dependency in the library)."""
+"""In-tree build of libmasr_b200.so with nvcc for sm_90a (no torch dependency in the library)."""
 from __future__ import annotations
 
 import glob
@@ -9,7 +9,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libmasr_b200.so")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-shared",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 
 

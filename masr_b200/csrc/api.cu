@@ -27,8 +27,8 @@ extern "C" const char* masr_last_error(void) { return masr::g_err; }
 
 extern "C" int masr_abi_version(void) { return MASR_ABI_VERSION; }
 
-// Fails loudly (non-zero + message) unless the current device is a Blackwell sm_100 part: the
-// library carries sm_100a SASS only and has no fallback path.
+// Fails loudly (non-zero + message) unless the current device is a Hopper sm_90 part: the
+// library carries sm_90a SASS only and has no fallback path.
 extern "C" int masr_check_device(void) {
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
@@ -36,8 +36,8 @@ extern "C" int masr_check_device(void) {
     cudaDeviceProp prop;
     e = cudaGetDeviceProperties(&prop, dev);
     if (e != cudaSuccess) { masr::set_last_error("cudaGetDeviceProperties: %s", cudaGetErrorString(e)); return (int)e; }
-    if (prop.major != 10) {
-        masr::set_last_error("masr_b200 needs an sm_100 (B200) device, found sm_%d%d (%s)", prop.major, prop.minor, prop.name);
+    if (prop.major != 9 || prop.minor != 0) {
+        masr::set_last_error("masr_b200 needs an sm_90 (H100) device, found sm_%d%d (%s)", prop.major, prop.minor, prop.name);
         return MASR_ERR_UNSUPPORTED_DEVICE;
     }
     return MASR_OK;

@@ -141,7 +141,7 @@ __global__ void __launch_bounds__(256) relpos_attention_kernel(AttnParams p) {
                 float ps = warp_sum(p0 + p1);
                 Ss[row * SS + lane] = p0;
                 Ss[row * SS + lane + 32] = p1;
-                __syncwarp();                   // every lane has read row_m[row] (racecheck r02: read/write hazard inside the owning warp)
+                __syncwarp();                   // every lane has read row_m[row] (read/write hazard inside the owning warp otherwise)
                 if (lane == 0) {
                     float alpha = expf(m_old - m_new);
                     row_a[row] = alpha;

@@ -12,8 +12,8 @@
 // the probabilities and the output accumulators never leave registers (the S accumulator fragment of two 8-key
 // blocks is exactly the A fragment of the P.V MMA).
 //
-// This is the legacy HMMA path (a 5 % FLOP share but 14 % of the step: 162 registers and 88 KB of shared memory per CTA
-// leave 8 warps per SM, ncu: 11 % warps active, latency-bound); a tcgen05 version is future work.
+// This is the mma.sync path (162 registers and 88 KB of shared memory per CTA leave 8 warps per SM: latency-bound); the
+// wgmma kernel (attention_tc5.cu) covers utterances of up to 256 frames.
 #include <cuda_fp16.h>
 #include <math.h>
 

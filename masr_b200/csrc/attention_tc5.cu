@@ -1,21 +1,22 @@
-// Relative-position attention core on the 5th-generation tensor cores (tcgen05.mma, accumulators in TMEM, operands staged by
-// TMA / written in the UMMA shared-memory layout), for utterances of up to 256 encoder frames — the batched whole-utterance
-// path of the headline config (T = 248).  Same contract and results (fp32-grade, FP16x2 operand split) as
-// relpos_attention_mma_kernel (attention_mma.cu, legacy mma.sync), which stays the kernel for longer utterances.
+// Relative-position attention core on the Hopper tensor cores (wgmma.mma_async, accumulators in registers, K / linear_pos(pe)
+// / V tiles by TMA), for utterances of up to 256 encoder frames — the batched whole-utterance path of the headline config
+// (T = 248).  Same contract and results (fp32-grade, FP16x2 operand split) as relpos_attention_mma_kernel (attention_mma.cu,
+// mma.sync), which stays the kernel for longer utterances.
 //
 //   S      = [q+u | q+v] . [k | p]^T / sqrt(d_k)          (128-wide contraction; no rel_shift, attention.py:245-247)
 //   out    = softmax_j(S[:, j < klen]) . v                 (attention.py:107-118)
-//   x.y   ~= xh.yh + 2^-11 (xh.yl + xl.yh)                 (two fp32 TMEM accumulators, as in tc_gemm.cu)
+//   x.y   ~= xh.yh + 2^-11 (xh.yl + xl.yh)                 (two fp32 accumulators, as in tc_gemm.cu)
 //
-// One CTA per (utterance, head); the utterance's queries are processed as one or two 128-row tiles.  Per tile:
-//   1. TMA: K and linear_pos(pe) rows 0..255 of this head (fp16 (h,l) pairs, written by the qkv GEMM epilogue / at load time)
-//      -> B operand [256 keys x (64 | 64)] in region R1; meanwhile all warps build A = [q+u | q+v] (fp32 add, then split) for
-//      the tile's 128 rows in region R2, directly in the 128-byte-swizzled K-major UMMA layout;
-//   2. 24 tcgen05.mma (M=128, N=256, K=16): S main -> TMEM columns [0,256), S correction -> [256,512);
-//   3. 8 softmax warps (TMEM lane quarter x column half): pass 1 row maximum, pass 2 p = 2^(s - max) (keys >= klen -> 0), row
-//      sums, and p as fp16 (h,l) pairs written into R1 as the A operand of the second product (un-normalised, flash-style);
+// One CTA per (utterance, head), two warpgroups of 64 query rows each; the utterance's queries are processed as one or two
+// 128-row tiles.  K | P (h, l) are loaded once per CTA.  Per tile:
+//   1. all threads build A = [q+u | q+v] (fp32 add, then split) for the tile's 128 rows in region R2, directly in the
+//      128-byte-swizzled K-major layout;
+//   2. per 64-key block: 12 wgmma m64n64k16 (S main, S correction) -> s = (main + 2^-11 corr) * scale kept in registers
+//      (the whole 64 x 256 row block of S: 128 registers per thread);
+//   3. row maximum and p = 2^(s - max) (keys >= klen -> 0) in registers, row sums by quad shuffles; p is split into fp16
+//      (h, l) register fragments that are directly the A operand of the second product (un-normalised, flash-style);
 //      meanwhile TMA loads V [256 keys x 64] into R2 — consumed as an MN-major B operand, so no transpose is needed;
-//   4. 48 tcgen05.mma (M=128, N=64, K=16): O main -> TMEM [0,64), O correction -> [64,128);
+//   4. 48 wgmma m64n64k16 with A from registers: O main, O correction;
 //   5. epilogue: O / rowsum -> fp32 and/or the fp16 (h,l) pair the output projection consumes; rows >= qlen are zeros.
 // Replaces attention.py:230-251,107-118 like the other attention kernels.
 #include <cuda.h>
@@ -32,10 +33,10 @@ namespace at5 {
 constexpr int AT_D = 64;                       // d_k
 constexpr int AT_KEYS = 256;                   // keys per CTA (one tile)
 constexpr int AT_ROWS = 128;                   // query rows per tile
-constexpr int AT_THREADS = 384;                // warp 0: TMA + MMA issue; warps 4..11: softmax / epilogue; all: Q staging
-constexpr int AT_R1 = 128 * 1024;              // K|P (h,l): 4 x 32 KB   /  P-matrix (h,l): 2 x 4 x 16 KB
+constexpr int AT_THREADS = 256;                // two warpgroups, 64 query rows each
+constexpr int AT_R1 = 128 * 1024;              // K|P (h,l): 4 x 32 KB
 constexpr int AT_R2 = 64 * 1024;               // Qcat (h,l): 4 x 16 KB  /  V (h,l): 2 x 32 KB
-constexpr size_t kAttnTc5Smem = AT_R1 + AT_R2 + 1024 /*align*/ + 2 * 2 * 128 * 4 /*row max / sum exchange*/ + 256;
+constexpr size_t kAttnTc5Smem = AT_R1 + AT_R2 + 1024 /*align*/ + 256;
 constexpr float kLoS = 2048.0f, kLoSInv = 1.0f / 2048.0f;
 
 __device__ __forceinline__ uint32_t s_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -61,55 +62,44 @@ __device__ __forceinline__ void tma_2d(const CUtensorMap* map, uint64_t* bar, vo
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         ::"r"(s_u32(dst)), "l"(map), "r"(s_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void mma_f16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t acc) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(acc) : "memory");
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+template <int R>
+__device__ __forceinline__ void rfence(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(s_u32(bar)) : "memory");
+
+#define AT_D32 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, " \
+               "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}"
+#define AT_O32(d) "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), \
+    "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), \
+    "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), \
+    "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+// D[64x64] (+)= A . B, A K-major in shared memory, B K-major in shared memory
+__device__ __forceinline__ void mma_ss(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " AT_D32 ", %32, %33, p, 1, 1, 0, 0;\n\t}"
+                 : AT_O32(d) : "l"(da), "l"(db), "r"(scale_d));
 }
-__device__ __forceinline__ void tm_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tm_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred = 0;
-    asm volatile(
-        "{\n\t"
-        ".reg .b32 %%rx;\n\t"
-        ".reg .pred %%px;\n\t"
-        "elect.sync %%rx|%%px, %1;\n\t"
-        "@%%px mov.s32 %0, 1;\n\t"
-        "}"
-        : "+r"(pred)
-        : "r"(0xFFFFFFFFu));
-    return pred != 0;
+// D[64x64] (+)= A . B, A from registers (the m64k16 fragment), B MN-major in shared memory
+__device__ __forceinline__ void mma_rs_tb(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " AT_D32 ", {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}"
+                 : AT_O32(d) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
 }
 // 128-byte-swizzled operand tile, rows of 64 halves (128 B), 8-row groups 1024 B apart.  Valid both for a K-major operand
-// (rows = M/N index, the 128 B = 64 contraction elements) and for an MN-major one (rows = contraction index, the 128 B = 64
-// M/N elements; SBO = distance between 8-row groups): start address >> 4 | LBO = 1 (unused) | SBO = 1024 B | version 1 | SWIZZLE_128B.
+// (rows = M/N index, the 128 B = 64 contraction elements) and for an MN-major one with 64 M/N elements (rows = contraction
+// index; the 8-row group stride is then the only stride used, given as both LBO and SBO): start address >> 4 |
+// LBO = 1024 B | SBO = 1024 B | layout SWIZZLE_128B (1 @ bit 62).
 __device__ __forceinline__ uint64_t desc_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(1024 >> 4) << 16;
     d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
 // byte offset of the 16-byte chunk `c16` (0..7) of row `r` inside a [rows x 64 halves] swizzled tile
@@ -130,6 +120,12 @@ __device__ __forceinline__ void split8(const float (&v)[8], uint32_t (&h)[4], ui
         h[j] = h2_bits(hh); l[j] = h2_bits(ll);
     }
 }
+__device__ __forceinline__ void split2(float a, float b, uint32_t& h, uint32_t& l) {
+    const __half2 hh = __floats2half2_rn(a, b);
+    const float2 hf = __half22float2(hh);
+    h = h2_bits(hh);
+    l = h2_bits(__floats2half2_rn((a - hf.x) * kLoS, (b - hf.y) * kLoS));
+}
 
 struct AttnTc5Params {
     const float* Q; int64_t ldq, q_bstride;
@@ -145,29 +141,21 @@ struct AttnTc5Maps { CUtensorMap kh, kl, vh, vl, ph, pl; };
 __global__ void __launch_bounds__(AT_THREADS, 1) relpos_attention_tc5_kernel(const __grid_constant__ AttnTc5Maps maps, AttnTc5Params p) {
     extern __shared__ uint8_t at_smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(at_smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* R1 = smem;                         // K|P tiles: [kb][hl] x 32 KB   /  P-matrix tiles: [hl][kb4] x 16 KB
+    uint8_t* R1 = smem;                         // K|P tiles: [kb][hl] x 32 KB
     uint8_t* R2 = smem + AT_R1;                 // Qcat tiles: [kb][hl] x 16 KB  /  V tiles: [hl] x 32 KB
-    float* xch = reinterpret_cast<float*>(R2 + AT_R2);          // [2 column halves][128 rows] max, then [2][128] sums
-    uint64_t* bars = reinterpret_cast<uint64_t*>(xch + 2 * 2 * 128);   // kv, s, v, o
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(R2 + AT_R2);   // kp, v
 
     const int h = blockIdx.x, b = blockIdx.y;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int wg = warp >> 2, wi = warp & 3;
     if (tid == 0) {
-        for (int i = 0; i < 4; ++i) mb_init(&bars[i], 1);
+        for (int i = 0; i < 2; ++i) mb_init(&bars[i], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.kh) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.ph) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.vh) : "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(tmem_slot)), "r"(512u));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    fence_before();
     __syncthreads();
-    fence_after();
-    const uint32_t tmem = *tmem_slot;
     pdl_wait();                                 // programmatic dependent launch: the qkv GEMM has completed
     pdl_launch_dependents();
 
@@ -175,40 +163,38 @@ __global__ void __launch_bounds__(AT_THREADS, 1) relpos_attention_tc5_kernel(con
     const int64_t krow0 = (int64_t)b * p.k_bstride;
     const int ntile = (qlen > 0 && klen > 0) ? (qlen + AT_ROWS - 1) / AT_ROWS : 0;
 
+    if (ntile > 0 && tid == 0) {                // K | P: once per CTA
+        mb_expect_tx(&bars[0], 4 * 32768);
+        tma_2d(&maps.kh, &bars[0], R1 + 0 * 32768, h * AT_D, (int)krow0);       // kb 0 (keys), h
+        tma_2d(&maps.kl, &bars[0], R1 + 1 * 32768, h * AT_D, (int)krow0);       // kb 0, l
+        tma_2d(&maps.ph, &bars[0], R1 + 2 * 32768, h * AT_D, 0);                // kb 1 (positions), h
+        tma_2d(&maps.pl, &bars[0], R1 + 3 * 32768, h * AT_D, 0);                // kb 1, l
+    }
     for (int mt = 0; mt < ntile; ++mt) {
-        const uint32_t par = mt & 1;
         const int r0 = mt * AT_ROWS;
-        // ---- 1. K | P via TMA into R1; [q+u | q+v] built by all threads into R2 ----
-        if (warp == 0 && elect_one()) {
-            mb_expect_tx(&bars[0], 4 * 32768);
-            tma_2d(&maps.kh, &bars[0], R1 + 0 * 32768, h * AT_D, (int)krow0);       // kb 0 (keys), h
-            tma_2d(&maps.kl, &bars[0], R1 + 1 * 32768, h * AT_D, (int)krow0);       // kb 0, l
-            tma_2d(&maps.ph, &bars[0], R1 + 2 * 32768, h * AT_D, 0);                // kb 1 (positions), h
-            tma_2d(&maps.pl, &bars[0], R1 + 3 * 32768, h * AT_D, 0);                // kb 1, l
-        }
+        // ---- 1. [q+u | q+v] built by all threads into R2 ----
         {
-            // every thread owns one 16-byte column chunk (c16 = tid & 7: 384 % 8 == 0) of rows tid/8, +48, +96 (the last only for
-            // tid < 256): the positional biases are loaded once, the three rows' query loads are issued together (the r02 capture
-            // showed the dependent load -> add chain of a one-row-at-a-time loop as the kernel's largest stall)
+            // every thread owns one 16-byte column chunk (c16 = tid & 7) of rows tid/8 + 32 it: the positional biases are
+            // loaded once, the four rows' query loads are issued together
             const float* qsrc = p.Q + ((int64_t)b * p.q_bstride + r0) * p.ldq + h * AT_D;
             const uint32_t base = s_u32(R2);
             const int c16 = tid & 7;
             const float4 u0 = ldg_f4(p.pos_u + h * AT_D + c16 * 8), u1 = ldg_f4(p.pos_u + h * AT_D + c16 * 8 + 4);
             const float4 v0 = ldg_f4(p.pos_v + h * AT_D + c16 * 8), v1 = ldg_f4(p.pos_v + h * AT_D + c16 * 8 + 4);
-            float4 qa[3], qb[3];
+            constexpr int IT = AT_ROWS / (AT_THREADS / 8);
+            float4 qa[IT], qb[IT];
 #pragma unroll
-            for (int it = 0; it < 3; ++it) {
+            for (int it = 0; it < IT; ++it) {
                 const int r = (tid >> 3) + it * (AT_THREADS / 8);
                 qa[it] = make_float4(0.f, 0.f, 0.f, 0.f); qb[it] = qa[it];
-                if (r < AT_ROWS && r0 + r < qlen) {
+                if (r0 + r < qlen) {
                     qa[it] = ldg_f4(qsrc + (int64_t)r * p.ldq + c16 * 8);
                     qb[it] = ldg_f4(qsrc + (int64_t)r * p.ldq + c16 * 8 + 4);
                 }
             }
 #pragma unroll
-            for (int it = 0; it < 3; ++it) {
+            for (int it = 0; it < IT; ++it) {
                 const int r = (tid >> 3) + it * (AT_THREADS / 8);
-                if (r >= AT_ROWS) break;
                 const bool ok = r0 + r < qlen;
                 const float4 a0 = qa[it], a1 = qb[it];
                 float qu[8], qv[8];
@@ -232,150 +218,123 @@ __global__ void __launch_bounds__(AT_THREADS, 1) relpos_attention_tc5_kernel(con
         }
         fence_async_smem();                     // the generic-proxy stores above must be visible to the tensor core
         __syncthreads();
-        // ---- 2. S = Qcat . Kcat^T : main -> TMEM [0,256), correction -> [256,512) ----
-        if (warp == 0 && elect_one()) {
-            mb_wait(&bars[0], par);
-            fence_after();
-            constexpr uint32_t idesc = (1u << 4) | ((uint32_t)(AT_KEYS >> 3) << 17) | ((uint32_t)(AT_ROWS >> 4) << 24);
+        // ---- 2. S = Qcat . Kcat^T per 64-key block; this warpgroup's 64 rows, all 256 keys, in registers ----
+        mb_wait(&bars[0], 0);
+        // fragment of m64n64: this thread holds rows 16 wi + lane / 4 (+ 8) and columns 8 i + 2 (lane % 4) (+ 1), i = 0..7
+        float s[4][32];
+#pragma unroll
+        for (int nb = 0; nb < 4; ++nb) {
+            float a[32], c[32];
+            rfence(a); rfence(c);
+            wg_fence();
 #pragma unroll
             for (int kb = 0; kb < 2; ++kb) {
-                const uint64_t dAh = desc_sw128(s_u32(R2 + (2 * kb + 0) * 16384)), dAl = desc_sw128(s_u32(R2 + (2 * kb + 1) * 16384));
-                const uint64_t dBh = desc_sw128(s_u32(R1 + (2 * kb + 0) * 32768)), dBl = desc_sw128(s_u32(R1 + (2 * kb + 1) * 32768));
+                const uint32_t qa_ = s_u32(R2 + (2 * kb) * 16384) + wg * 8192;      // this warpgroup's 64 query rows
+                const uint64_t dAh = desc_sw128(qa_), dAl = desc_sw128(qa_ + 16384);
+                const uint32_t kb_ = s_u32(R1 + (2 * kb) * 32768) + nb * 8192;      // keys [64 nb, 64 nb + 64)
+                const uint64_t dBh = desc_sw128(kb_), dBl = desc_sw128(kb_ + 32768);
 #pragma unroll
                 for (int ks = 0; ks < 4; ++ks) {
                     const uint64_t adv = (uint64_t)(ks * 2);                          // 16 halves = 32 B = 2 x 16-byte units
-                    mma_f16(tmem + 0, dAh + adv, dBh + adv, idesc, (kb | ks) ? 1u : 0u);
-                    mma_f16(tmem + 256, dAh + adv, dBl + adv, idesc, (kb | ks) ? 1u : 0u);
-                    mma_f16(tmem + 256, dAl + adv, dBh + adv, idesc, 1u);
+                    mma_ss(a, dAh + adv, dBh + adv, (kb | ks) ? 1u : 0u);
+                    mma_ss(c, dAh + adv, dBl + adv, (kb | ks) ? 1u : 0u);
+                    mma_ss(c, dAl + adv, dBh + adv, 1u);
                 }
             }
-            mma_commit(&bars[1]);
-            // ---- V via TMA into R2 as soon as the S products have consumed Qcat ----
-            mb_wait(&bars[1], par);
-            mb_expect_tx(&bars[2], 2 * 32768);
-            tma_2d(&maps.vh, &bars[2], R2 + 0 * 32768, h * AT_D, (int)krow0);
-            tma_2d(&maps.vl, &bars[2], R2 + 1 * 32768, h * AT_D, (int)krow0);
+            wg_commit();
+            wg_wait0();
+            rfence(a); rfence(c);
+#pragma unroll
+            for (int j = 0; j < 32; ++j) s[nb][j] = fmaf(c[j], kLoSInv, a[j]) * p.scale;
         }
-        // ---- 3. softmax: 8 warps = TMEM lane quarter (warp & 3) x column half ((warp - 4) >> 2) ----
-        float inv_sum = 0.f;
-        if (warp >= 4) {
-            const int q = warp & 3, ch = (warp - 4) >> 2;
-            const int row = q * 32 + lane;
-            const uint32_t tl = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(ch * 128);
-            mb_wait(&bars[1], par);
-            fence_after();
-            float mx = -INFINITY;
-#pragma unroll 1
-            for (int cc = 0; cc < 4; ++cc) {
-                uint32_t a[32], c[32];
-                tm_ld32(tl + cc * 32, a);
-                tm_ld32(tl + 256 + cc * 32, c);
-                tm_ld_wait();
-                const int col0 = ch * 128 + cc * 32;
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const float s = fmaf(__uint_as_float(c[j]), kLoSInv, __uint_as_float(a[j])) * p.scale;
-                    mx = fmaxf(mx, col0 + j < klen ? s : -INFINITY);
-                }
-            }
-            xch[ch * 128 + row] = mx;
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-            mx = fmaxf(xch[row], xch[128 + row]);                                    // (klen >= 1: finite)
-            float sum = 0.f;
-            const uint32_t pbase = s_u32(R1);
-#pragma unroll 1
-            for (int cc = 0; cc < 4; ++cc) {
-                uint32_t a[32], c[32];
-                tm_ld32(tl + cc * 32, a);
-                tm_ld32(tl + 256 + cc * 32, c);
-                tm_ld_wait();
-                const int col0 = ch * 128 + cc * 32;
-                const int kb = col0 >> 6, c16b = (col0 & 63) >> 3;                   // 64-key K-block and first 16-byte chunk in it
-#pragma unroll
-                for (int g8 = 0; g8 < 4; ++g8) {
-                    float pv[8];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const int jj = g8 * 8 + j;
-                        const float s = fmaf(__uint_as_float(c[jj]), kLoSInv, __uint_as_float(a[jj])) * p.scale;
-                        pv[j] = col0 + jj < klen ? ex2_approx(s - mx) : 0.f;
-                        sum += pv[j];
-                    }
-                    uint32_t hh[4], ll[4];
-                    split8(pv, hh, ll);
-                    const uint32_t off = sw128_off(row, c16b + g8);
-                    sts128(pbase + (0 * 4 + kb) * 16384 + off, hh[0], hh[1], hh[2], hh[3]);
-                    sts128(pbase + (1 * 4 + kb) * 16384 + off, ll[0], ll[1], ll[2], ll[3]);
-                }
-            }
-            xch[256 + ch * 128 + row] = sum;
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-            inv_sum = 1.0f / (xch[256 + row] + xch[256 + 128 + row]);
-            fence_before();
+        __syncthreads();                        // both warpgroups are done reading Qcat (R2)
+        // ---- V via TMA into R2 ----
+        if (tid == 0) {
+            mb_expect_tx(&bars[1], 2 * 32768);
+            tma_2d(&maps.vh, &bars[1], R2 + 0 * 32768, h * AT_D, (int)krow0);
+            tma_2d(&maps.vl, &bars[1], R2 + 1 * 32768, h * AT_D, (int)krow0);
         }
-        fence_async_smem();
-        __syncthreads();                        // P-matrix complete in R1; S has been read out of TMEM
-        // ---- 4. O = P . V : main -> TMEM [0,64), correction -> [64,128) ----
-        if (warp == 0 && elect_one()) {
-            mb_wait(&bars[2], par);
-            fence_after();
-            constexpr uint32_t idesc = (1u << 4) | (1u << 16) /* B is MN-major */ | ((uint32_t)(AT_D >> 3) << 17) | ((uint32_t)(AT_ROWS >> 4) << 24);
-            const uint64_t dVh = desc_sw128(s_u32(R2)), dVl = desc_sw128(s_u32(R2 + 32768));
+        // ---- 3. softmax in registers: rows (lane / 4) and (lane / 4 + 8) of the warp's 16; a row's columns live in 4 lanes ----
+        float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-            for (int kb = 0; kb < 4; ++kb) {
-                const uint64_t dPh = desc_sw128(s_u32(R1 + (0 * 4 + kb) * 16384)), dPl = desc_sw128(s_u32(R1 + (1 * 4 + kb) * 16384));
+        for (int nb = 0; nb < 4; ++nb)
 #pragma unroll
-                for (int ks = 0; ks < 4; ++ks) {
-                    const uint64_t adva = (uint64_t)(ks * 2);                         // A (K-major): 16 halves = 32 B
-                    const uint64_t advb = (uint64_t)((kb * 64 + ks * 16) * 128 >> 4); // B (MN-major): 16 key rows of 128 B
-                    mma_f16(tmem + 0, dPh + adva, dVh + advb, idesc, (kb | ks) ? 1u : 0u);
-                    mma_f16(tmem + 64, dPh + adva, dVl + advb, idesc, (kb | ks) ? 1u : 0u);
-                    mma_f16(tmem + 64, dPl + adva, dVh + advb, idesc, 1u);
+            for (int i = 0; i < 8; ++i)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int col = nb * 64 + 8 * i + 2 * (lane & 3) + (e & 1);
+                    if (col < klen) mx[e >> 1] = fmaxf(mx[e >> 1], s[nb][4 * i + e]);
                 }
-            }
-            mma_commit(&bars[3]);
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+            mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));      // (klen >= 1: finite)
         }
+        float sum[2] = {0.f, 0.f};
+        uint32_t ph[16][4], pl[16][4];          // A fragments of P (h, l) for the 16 key steps of 16
+#pragma unroll
+        for (int nb = 0; nb < 4; ++nb)
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                float pv[4];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int col = nb * 64 + 8 * i + 2 * (lane & 3) + (e & 1);
+                    pv[e] = col < klen ? ex2_approx(s[nb][4 * i + e] - mx[e >> 1]) : 0.f;
+                    sum[e >> 1] += pv[e];
+                }
+                // accumulator columns 16 j .. 16 j + 15 (i = 2 j, 2 j + 1) are the A fragment of key step j:
+                // a0 = (row, k 0..7), a1 = (row + 8, k 0..7), a2 = (row, k 8..15), a3 = (row + 8, k 8..15)
+                const int j = nb * 4 + (i >> 1), hi = (i & 1) * 2;
+                split2(pv[0], pv[1], ph[j][hi], pl[j][hi]);
+                split2(pv[2], pv[3], ph[j][hi + 1], pl[j][hi + 1]);
+            }
+        float inv_sum[2];
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            sum[r] += __shfl_xor_sync(0xffffffffu, sum[r], 1);
+            sum[r] += __shfl_xor_sync(0xffffffffu, sum[r], 2);
+            inv_sum[r] = 1.0f / sum[r];
+        }
+        // ---- 4. O = P . V : main, correction ----
+        mb_wait(&bars[1], mt & 1);
+        float o[32], oc[32];
+        rfence(o); rfence(oc);
+        wg_fence();
+        {
+            const uint32_t vh = s_u32(R2), vl = vh + 32768;
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+                const uint64_t advb = (uint64_t)((j * 16) * 128 >> 4);                // B (MN-major): 16 key rows of 128 B
+                mma_rs_tb(o, ph[j], desc_sw128(vh) + advb, j ? 1u : 0u);
+                mma_rs_tb(oc, ph[j], desc_sw128(vl) + advb, j ? 1u : 0u);
+                mma_rs_tb(oc, pl[j], desc_sw128(vh) + advb, 1u);
+            }
+        }
+        wg_commit();
+        wg_wait0();
+        rfence(o); rfence(oc);
         // ---- 5. epilogue: O / rowsum -> global (rows >= qlen: zeros) ----
-        if (warp >= 4) {
-            const int q = warp & 3, cg = (warp - 4) >> 2;                            // 32 output columns per warp
-            const int row = q * 32 + lane;
-            mb_wait(&bars[3], par);
-            fence_after();
-            uint32_t a[32], c[32];
-            const uint32_t tl = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(cg * 32);
-            tm_ld32(tl, a);
-            tm_ld32(tl + 64, c);
-            tm_ld_wait();
-            fence_before();
-            const int grow = r0 + row;
-            if (grow < p.max_q) {
-                const bool valid = grow < qlen;
-                const int64_t off = ((int64_t)b * p.o_bstride + grow) * p.ldo + h * AT_D + cg * 32;
-                float o[32];
 #pragma unroll
-                for (int j = 0; j < 32; ++j)
-                    o[j] = valid ? fmaf(__uint_as_float(c[j]), kLoSInv, __uint_as_float(a[j])) * inv_sum : 0.f;
-                if (p.O) {
+        for (int r = 0; r < 2; ++r) {
+            const int grow = r0 + wg * 64 + wi * 16 + (lane >> 2) + 8 * r;
+            if (grow >= p.max_q) continue;
+            const bool valid = grow < qlen;
+            const int64_t off = ((int64_t)b * p.o_bstride + grow) * p.ldo + h * AT_D + 2 * (lane & 3);
 #pragma unroll
-                    for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(p.O + off + j) = make_float4(o[j], o[j + 1], o[j + 2], o[j + 3]);
-                }
+            for (int i = 0; i < 8; ++i) {
+                const float x0 = valid ? fmaf(oc[4 * i + 2 * r], kLoSInv, o[4 * i + 2 * r]) * inv_sum[r] : 0.f;
+                const float x1 = valid ? fmaf(oc[4 * i + 2 * r + 1], kLoSInv, o[4 * i + 2 * r + 1]) * inv_sum[r] : 0.f;
+                if (p.O) *reinterpret_cast<float2*>(p.O + off + 8 * i) = make_float2(x0, x1);
                 if (p.Oh) {
-#pragma unroll
-                    for (int g8 = 0; g8 < 4; ++g8) {
-                        float t8[8];
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) t8[j] = o[g8 * 8 + j];
-                        uint32_t hh[4], ll[4];
-                        split8(t8, hh, ll);
-                        *reinterpret_cast<uint4*>(p.Oh + off + g8 * 8) = make_uint4(hh[0], hh[1], hh[2], hh[3]);
-                        *reinterpret_cast<uint4*>(p.Ol + off + g8 * 8) = make_uint4(ll[0], ll[1], ll[2], ll[3]);
-                    }
+                    uint32_t hh, ll;
+                    split2(x0, x1, hh, ll);
+                    *reinterpret_cast<uint32_t*>(p.Oh + off + 8 * i) = hh;
+                    *reinterpret_cast<uint32_t*>(p.Ol + off + 8 * i) = ll;
                 }
             }
         }
-        fence_before();
-        __syncthreads();                        // TMEM, R1 and R2 are free for the next tile
-        fence_after();
+        __syncthreads();                        // R2 (V) is free for the next tile's Qcat
     }
     // query rows no tile covered (padded rows of a short utterance, empty utterances): deterministic zeros
     {
@@ -390,13 +349,6 @@ __global__ void __launch_bounds__(AT_THREADS, 1) relpos_attention_tc5_kernel(con
                 *reinterpret_cast<uint2*>(p.Ol + off) = make_uint2(0u, 0u);
             }
         }
-    }
-    fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        fence_after();
-        __syncwarp();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u));
     }
 }
 
@@ -436,7 +388,7 @@ int make_map(CUtensorMap* map, const void* ptr, int64_t rows, int64_t cols, int6
 using namespace masr;
 using namespace masr::at5;
 
-// Same arguments and results as masr_relpos_attention_tc, computed on tcgen05 / TMEM / TMA.  Restrictions of this kernel:
+// Same arguments and results as masr_relpos_attention_tc, computed with wgmma / TMA.  Restrictions of this kernel:
 // max_q <= 256, every k_lens[b] <= 256, d_k = 64, table_rows >= 1 rows in the linear_pos(pe) table (rows beyond it read as zero and
 // only meet masked keys).  Callers fall back to masr_relpos_attention_tc otherwise.
 extern "C" int masr_relpos_attention_tc5(const float* Q, int64_t ldq, int64_t q_bstride, const void* Kh, const void* Kl,

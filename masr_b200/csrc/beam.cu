@@ -272,7 +272,7 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
             }
             __syncthreads();
             // the digit where the descending cumulative count reaches `want`: inclusive scan over the 256 bins by 8 warps
-            // (the first version walked the bins serially in thread 0 — a third of the kernel's time in the r02 capture)
+            // (walking the bins serially in thread 0 would serialise a large part of the kernel)
             {
                 int v = 0, incl = 0;
                 if (tid < 256) {

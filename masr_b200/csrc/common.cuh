@@ -1,4 +1,4 @@
-// Shared device/host helpers for the masr_b200 kernels (sm_100a only).
+// Shared device/host helpers for the masr_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -67,7 +67,7 @@ __device__ __forceinline__ float fast_silu(float x) { return x * fast_sigmoid(x)
 
 // ---- programmatic dependent launch (PDL) --------------------------------------------------------------------------
 // The device step is a chain of ~180 short kernels.  Launched with programmaticStreamSerialization, a kernel may start
-// (and run its prologue: barrier init, TMEM allocation, table loads into registers) while its predecessor drains; it
+// (and run its prologue: barrier init, descriptor prefetch, table loads into registers) while its predecessor drains; it
 // blocks in pdl_wait() until the predecessor grid has completed and its memory is visible, BEFORE its first global access.
 // Kernels launched without the attribute see a no-op.  MASR_PDL=0 disables the attribute.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

@@ -64,7 +64,7 @@ __global__ void __launch_bounds__(256) ctc_frame_argmax_kernel(const float* __re
 // One CTA per utterance.  Frames are staged through shared memory in tiles of 256 (coalesced loads); the keep flags
 // (id != blank and id != previous id) are compacted with warp ballots; the score sum stays a left-to-right float32 chain
 // over the non-blank frames, as `greedy_decoder` computes it (ctc_greedy_decoder.py:28-30), run by one thread from shared
-// memory.  (The first version walked global memory from one thread per utterance: 46 us of pure load latency.)
+// memory (one thread per utterance walking global memory is pure load latency).
 __global__ void __launch_bounds__(256) ctc_greedy_collapse_kernel(const int* __restrict__ ids, const float* __restrict__ maxp,
                                                                   int64_t bstride, const int* __restrict__ lens, int blank,
                                                                   int prev_id_in, int* __restrict__ tokens, int64_t tok_stride,

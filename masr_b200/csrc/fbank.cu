@@ -150,9 +150,8 @@ __global__ void wave_gain_kernel(const int64_t* __restrict__ offs, const double*
 // ---- fbank ----------------------------------------------------------------------------------------
 // One warp per frame.  The 512-point real FFT runs as a 256-point complex FFT factored 8 x 8 x 4 (decimation in
 // frequency): each lane keeps 8 complex points in registers and does the radix-8 / radix-4 butterflies there, so the data
-// crosses shared memory twice (two transposes) instead of once per radix-2 stage — the first version (8 radix-2 stages in
-// shared memory, twiddles and window through L1) ran at 91 % L1/shared-pipe utilisation and 0.04 of the HBM roofline
-// (ncu, profiles/r01_step_kernels_summary.md).  Stage twiddles live in registers, window / post-twiddles / mel weights in
+// crosses shared memory twice (two transposes) instead of once per radix-2 stage (8 radix-2 stages in shared memory,
+// twiddles and window through L1, make the L1/shared pipe the bound).  Stage twiddles live in registers, window / post-twiddles / mel weights in
 // shared memory (loaded once per CTA).
 constexpr int kWarpsPerBlock = 4;
 constexpr int kFramesPerWarp = 4;

@@ -214,9 +214,9 @@ __global__ void __launch_bounds__(256) sgemm_tn_kernel(GemmParams p) {
 template <int AMODE>
 static int launch_gemm(const GemmParams& p, cudaStream_t st) {
     // Large problems: 128x128 tiles.  Small / skinny ones: 64x64 tiles so the grid still covers the
-    // 148 SMs (guide: Guideline 11).
+    // 132 SMs (guide: Guideline 11).
     long tiles128 = (long)((p.M + 127) / 128) * ((p.N + 127) / 128);
-    if (tiles128 >= 148) {
+    if (tiles128 >= 132) {
         dim3 grid((p.N + 127) / 128, (p.M + 127) / 128);
         sgemm_tn_kernel<128, 128, AMODE><<<grid, 256, 0, st>>>(p);
     } else {

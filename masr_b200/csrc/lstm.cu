@@ -71,7 +71,7 @@ __global__ void __launch_bounds__(LSTM_UNITS * 32) lstm_step_kernel(
 
 // ---- persistent form: the whole sequence of one layer / direction in ONE launch --------------------------------------------
 // The per-step kernel above re-reads W_hh (16 MB at H = 1024) from L2 on every step through a handful of warps and was pure
-// load latency (~70 us per step, 1240 launches per utterance batch).  Here every CTA keeps ITS slice of W_hh — the four gate
+// load latency (one launch per step).  Here every CTA keeps ITS slice of W_hh — the four gate
 // rows of LS_UNITS hidden units — resident in shared memory for all T steps (32 x H floats = 128 KB at H = 1024), streams
 // h_{t-1} ([H][32] per batch chunk, written by all CTAs in the previous step) through a double-buffered shared-memory window,
 // and the steps are separated by a grid-wide barrier (one atomic counter; the grid has at most one CTA per SM, all
@@ -85,18 +85,21 @@ __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
     asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
     return v;
 }
-// packed fp32 FMA (Blackwell fma.rn.f32x2): two independent round-to-nearest FMAs per issue slot
+// a pair of fp32 values in one 64-bit register: two independent round-to-nearest FMAs per call
 __device__ __forceinline__ uint64_t pack2(float a, float b) {
     uint64_t r;
     asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
     return r;
 }
+__device__ __forceinline__ void unpack2(uint64_t v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
 __device__ __forceinline__ void ffma2(uint64_t& d, uint64_t a, uint64_t b) {
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(d) : "l"(a), "l"(b));
+    float d0, d1, a0, a1, b0, b1;
+    unpack2(d, d0, d1); unpack2(a, a0, a1); unpack2(b, b0, b1);
+    d = pack2(fmaf(a0, b0, d0), fmaf(a1, b1, d1));
 }
 __device__ __forceinline__ float sum2(uint64_t v) {
     float a, b;
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
+    unpack2(v, a, b);
     return a + b;
 }
 __device__ __forceinline__ void cp_async16_cg(void* dst, const void* src) {

@@ -16,7 +16,7 @@ namespace masr {
 // a lane owns 8 consecutive output channels (72 weights in registers, loaded once per CTA and amortised over
 // CONV1_TR x W1 positions), so the 9 window values of a position are 9 shared-memory broadcasts for 72 FMAs and the
 // results leave as 128-bit stores (one per fp16 half, or two for fp32).  The first version (thread per channel, 16-bit
-// scalar stores, 9 shared loads per output) was instruction-bound at 75 % issue utilisation (ncu, r01).
+// scalar stores, 9 shared loads per output) was instruction-bound.
 constexpr int CONV1_TR = 4;
 
 __global__ void __launch_bounds__(256) conv1_cmvn_relu_kernel(const float* __restrict__ feats,

@@ -1,31 +1,29 @@
-// Tensor-core GEMM with fp32-grade results:  C[M,N] = epilogue(A[M,K] * W[N,K]^T)  on tcgen05 / TMEM,
-// operands staged by TMA, accumulators in tensor memory.
+// Tensor-core GEMM with fp32-grade results:  C[M,N] = epilogue(A[M,K] * W[N,K]^T)  on Hopper wgmma,
+// operands staged by TMA, accumulators in registers.
 //
 // Precision scheme ("FP16x2 split", DESIGN.md §4 precision policy): every fp32 operand x is carried as
 // two fp16 numbers  h = fp16(x),  l = fp16((x - h) * 2^11)  (22 significand bits), and the product is
 //     A.W^T  ~=  Ah.Wh^T  +  2^-11 * (Ah.Wl^T + Al.Wh^T)            (the Al.Wl term is < 2^-22 relative)
-// with both sums accumulated in fp32 in two TMEM accumulators.  3 MMAs per K-step => one third of the
+// with both sums accumulated in fp32 in two register accumulators.  3 MMAs per K-step => one third of the
 // fp16/bf16 tensor peak, but the greedy ids stay bit-exact against the fp32 reference (a single-pass
 // bf16/tf32/fp16 GEMM flips argmaxes, see DESIGN.md).
 //
 // Replaces the same reference call sites as gemm.cu (positionwise.py:37, attention.py:72-74,119,
 // convolution.py:117-118,127, subsampling.py:110, loss/ctc.py:70).
 //
-// Structure (persistent: one CTA per SM walks 128x128 output tiles; 64 + 32*EW threads, EW = 16 epilogue warps by default):
-//   warp 0   TMA producer: 4 boxes per K-block (Ah, Al, Wh, Wl; 64 halves = one 128-byte swizzle row)
-//   warp 1   TMEM allocator + single-thread tcgen05.mma issuer (12 MMAs per K-block); main accumulator ping-pong by
-//            256-wide K chunk, correction accumulator ping-pong by tile (512 TMEM columns), so the MMAs of tile i+1
-//            run while the epilogue drains tile i
-//   warps 2.. epilogue: tcgen05.ld 32x32b -> registers -> fused bias/SiLU/ReLU/GLU/scale/residual -> transposed
-//            through shared memory -> row-contiguous 128-bit stores (fp32 and/or the fp16 (h,l) pair the next GEMM consumes)
-//   smem ring of 3 x 64 KB stages with full/empty mbarriers; tcgen05.commit releases slots and signals the epilogue.
-//   Launched with programmatic dependent launch: the prologue overlaps the producer kernel's tail.
-// PAIR form (the default, DESIGN.md 4b): clusters of 2 CTAs own 256 x 128 tiles through tcgen05.mma.cta_group::2 — each CTA
-// stages its 128 A rows and half of the W tile, the pair's leader issues the MMAs and multicasts the commits (4 x 48 KB stages).
-// Round-2 additions (DESIGN.md 4b): residual epilogues fetch the residual at tile start into the running sum (flags bit 4);
+// Structure (persistent: one CTA per SM walks 128x128 output tiles; 16 consumer warps + 1 producer warp):
+//   warps 0..15  four consumer warpgroups, each owns a 64x64 quarter of the tile: wgmma.mma_async m64n64k16 from the
+//                shared-memory ring (12 MMAs per K-block: main Ah.Wh, correction Ah.Wl + Al.Wh), then the epilogue:
+//                accumulators -> the warpgroup's 16 KB of shared memory -> one thread per (row, 32 columns) -> fused
+//                bias/SiLU/ReLU/GLU/scale/residual -> row-contiguous 128-bit stores (fp32 and/or the fp16 (h,l) pair the
+//                next GEMM consumes)
+//   warp 16      TMA producer: 4 boxes per K-block (Ah, Al, Wh, Wl; 64 halves = one 128-byte swizzle row)
+//   smem ring of 2 x 64 KB stages with full/empty mbarriers; the producer fills the next tile's stages while the
+//   consumers run the epilogue.  Launched with programmatic dependent launch: the prologue overlaps the producer
+//   kernel's tail.
 // EPI_CTC_PARTIAL keeps per (row, 32 columns) softmax partials instead of logits (+ ctc_partial_combine_kernel);
 // the LNC variant (clusters of 2 CTAs) fuses the LayerNorm(s) that follow a residual projection, row statistics over DSMEM
-// (pre-norm LN / LN2 and the Squeezeformer's post-norm + adaptive scale) — measured, not the default.
+// (pre-norm LN / LN2 and the Squeezeformer's post-norm + adaptive scale).
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <math.h>
@@ -38,21 +36,12 @@
 namespace masr {
 
 constexpr int TBM = 128, TBN = 128, TBK = 64;
-constexpr int TSTAGES = 3;
+constexpr int TSTAGES = 2;
 constexpr int TILE_BYTES = TBM * TBK * 2;              // 16 KB: one operand tile
 constexpr int STAGE_BYTES = 4 * TILE_BYTES;            // Ah, Al, Wh, Wl
-// PAIR kernels (cta_group::2, a 256 x 128 tile per pair of CTAs): a CTA stages its own 128 A rows and HALF of the W tile
-// (64 of the 128 output columns; the tensor cores of both SMs read both halves) -> 48 KB per K-block, 4 stages
-template <bool PAIR> struct RingCfg {
-    static constexpr int STAGES = PAIR ? 4 : TSTAGES;
-    static constexpr int W_BYTES = PAIR ? TILE_BYTES / 2 : TILE_BYTES;
-    static constexpr int BYTES = 2 * TILE_BYTES + 2 * W_BYTES;
-};
-constexpr int MAX_STAGES = 4;
-static_assert(RingCfg<true>::STAGES * RingCfg<true>::BYTES == TSTAGES * STAGE_BYTES, "both rings take 192 KB");
-constexpr int EPI_STAGE_TOTAL = 32768;                 // epilogue store staging, split evenly over the epilogue warps
-constexpr int tc_threads(int ew) { return 64 + 32 * ew; }   // TMA warp + MMA warp + EW epilogue warps
-constexpr uint32_t TMEM_COLS = 512;                    // 2 x main (ping-pong) + correction accumulator, 128 fp32 columns each (384 -> 512)
+constexpr int RES_BYTES = TBM * TBN * 4;               // fp32 result tile, 16 KB per consumer warpgroup
+constexpr int EW = 16;                                 // consumer / epilogue warps
+constexpr int TC_THREADS = 32 * EW + 32;               // + the TMA producer warp
 constexpr float kLoScale = 2048.0f, kLoInv = 1.0f / 2048.0f;
 
 // ---- PTX wrappers ---------------------------------------------------------------------------------
@@ -80,13 +69,21 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* ba
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
+// the same box into this CTA's and the cluster peer's shared memory (same offset), complete_tx on each CTA's mbarrier
+__device__ __forceinline__ void tma_load_2d_mc(const CUtensorMap* map, uint64_t* bar, void* smem_dst, int c0, int c1, uint16_t mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+        ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
+    uint32_t a;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(a) : "r"(smem_u32(bar)), "r"(rank));
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(a) : "memory");
+}
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
-// One lane of a converged warp (CUTLASS's elect_one_sync): the compiler then knows the region runs on a single thread and
-// issues the uniform-datapath instructions (UTMALDG, UTCHMMA, UTCBAR) directly.  With `if (lane == 0)` every one of them
-// was wrapped in an ELECT / vote / branch retry sequence (~9 SASS instructions per MMA): the issuing thread needed about as
-// long to issue a K-block's 12 MMAs as the tensor core to execute them, and the pipe idled half of the time (ncu r01).
+// One lane of a converged warp (CUTLASS's elect_one_sync): the compiler then knows the region runs on a single thread
 __device__ __forceinline__ bool elect_one_sync() {
     uint32_t pred = 0, laneid = 0;
     asm volatile(
@@ -101,105 +98,52 @@ __device__ __forceinline__ bool elect_one_sync() {
         : "r"(0xFFFFFFFFu));
     return pred != 0;
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+// ---- wgmma (sm_90a) ---------------------------------------------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of accumulator registers across wgmma issue / wait
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// D[64x64] (+)= A[64x16] . B[64x16]^T, both operands K-major in shared memory; scale_d == 0 overwrites D
+__device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// ---- cta_group::2 forms (PAIR kernels): issued by the leader CTA (cluster rank 0) for both SMs of the pair ----
-__device__ __forceinline__ void umma_f16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrives on the mbarrier at this CTA-relative address in BOTH CTAs of the pair once the MMAs issued so far have retired
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-    return r;
-}
-// TMA into this CTA's shared memory, transaction bytes reported to an mbarrier of the pair's leader (shared::cluster address)
-__device__ __forceinline__ void tma_load_2d_pair(const CUtensorMap* map, uint32_t bar_cluster, void* smem_dst, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(map), "r"(bar_cluster), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair(const CUtensorMap* map, uint32_t bar_cluster, void* smem_dst, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(map), "r"(bar_cluster), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_cluster) {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t"
+        "}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// K-major, 128-byte-swizzled operand tile (rows of 64 halves, 8-row groups 1024 B apart):
-// start address >> 4 | LBO (ignored for swizzled K-major) | SBO = 1024 B | version 1 | SWIZZLE_128B.
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
+// K-major, 128-byte-swizzled operand tile (rows of 64 halves, 8-row groups 1024 B apart), wgmma descriptor:
+// start address >> 4 | LBO (unused for swizzled K-major) = 16 B | SBO = 1024 B | layout SWIZZLE_128B (1 @ bit 62).
+// Tile bases are 1024-byte aligned, so the swizzle phase (base offset) is 0.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
     d |= (uint64_t)1 << 16;
     d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
 
 // fp32 -> (h, l) with l pre-scaled by 2^11
-// packed fp32 arithmetic (Blackwell f32x2: two independent IEEE round-to-nearest operations per issue slot; the results are
-// bit-identical to the scalar forms).  The epilogues of the K <= 256 GEMMs are bound by issue slots and pipe time, not by data.
-#ifdef MASR_TC_SCALAR_EPI      // A/B builds only: the scalar forms
-__device__ __forceinline__ void fma2(float& d0, float& d1, float a0, float a1, float b0, float b1, float c0, float c1) { d0 = fmaf(a0, b0, c0); d1 = fmaf(a1, b1, c1); }
+// two independent IEEE round-to-nearest operations (pairs kept together for the vectorised store paths)
 __device__ __forceinline__ void add2(float& d0, float& d1, float a0, float a1, float b0, float b1) { d0 = a0 + b0; d1 = a1 + b1; }
 __device__ __forceinline__ void sub2(float& d0, float& d1, float a0, float a1, float b0, float b1) { d0 = a0 - b0; d1 = a1 - b1; }
 __device__ __forceinline__ void mul2(float& d0, float& d1, float a0, float a1, float b0, float b1) { d0 = a0 * b0; d1 = a1 * b1; }
-#else
-__device__ __forceinline__ void fma2(float& d0, float& d1, float a0, float a1, float b0, float b1, float c0, float c1) {
-    asm("{\n\t.reg .b64 a, b, c, d;\n\tmov.b64 a, {%2, %3};\n\tmov.b64 b, {%4, %5};\n\tmov.b64 c, {%6, %7};\n\t"
-        "fma.rn.f32x2 d, a, b, c;\n\tmov.b64 {%0, %1}, d;\n\t}"
-        : "=f"(d0), "=f"(d1) : "f"(a0), "f"(a1), "f"(b0), "f"(b1), "f"(c0), "f"(c1));
-}
-__device__ __forceinline__ void add2(float& d0, float& d1, float a0, float a1, float b0, float b1) {
-    asm("{\n\t.reg .b64 a, b, d;\n\tmov.b64 a, {%2, %3};\n\tmov.b64 b, {%4, %5};\n\tadd.rn.f32x2 d, a, b;\n\tmov.b64 {%0, %1}, d;\n\t}"
-        : "=f"(d0), "=f"(d1) : "f"(a0), "f"(a1), "f"(b0), "f"(b1));
-}
-__device__ __forceinline__ void sub2(float& d0, float& d1, float a0, float a1, float b0, float b1) {
-    asm("{\n\t.reg .b64 a, b, d;\n\tmov.b64 a, {%2, %3};\n\tmov.b64 b, {%4, %5};\n\tsub.rn.f32x2 d, a, b;\n\tmov.b64 {%0, %1}, d;\n\t}"
-        : "=f"(d0), "=f"(d1) : "f"(a0), "f"(a1), "f"(b0), "f"(b1));
-}
-__device__ __forceinline__ void mul2(float& d0, float& d1, float a0, float a1, float b0, float b1) {
-    asm("{\n\t.reg .b64 a, b, d;\n\tmov.b64 a, {%2, %3};\n\tmov.b64 b, {%4, %5};\n\tmul.rn.f32x2 d, a, b;\n\tmov.b64 {%0, %1}, d;\n\t}"
-        : "=f"(d0), "=f"(d1) : "f"(a0), "f"(a1), "f"(b0), "f"(b1));
-}
-#endif
 __device__ __forceinline__ void split_f16(float x, __half& h, __half& l) {
     h = __float2half_rn(x);
     l = __float2half_rn((x - __half2float(h)) * kLoScale);
@@ -237,7 +181,6 @@ struct TcParams {
     float* part_m;
     float* part_s;
     int* part_i;
-    float inv_alpha;   // flags bit 4 (residual prefetch): 1 / alpha, exact (alpha is a power of two)
     const float* ada_s;   // EPI_RESIDUAL_POSTLN: optional per-channel scale / bias applied to the LayerNorm output for the pair
     const float* ada_b;
     // LayerNorm prologue (masr_gemm_tc_lnpre_f16x2, K = 256): the A operand is LayerNorm(lnp_x; ln_g, ln_b) — every CTA
@@ -305,9 +248,8 @@ __device__ __forceinline__ void tma_load_4d(const CUtensorMap* map, uint64_t* ba
 }
 
 // ---- epilogue stores ------------------------------------------------------------------------------
-// A TMEM lane is an output row, so each epilogue thread holds 32 consecutive columns of ONE row: storing
-// straight from registers makes every warp store touch 32 different 128-byte lines, 16 bytes each (ncu:
-// the store pipe, not the tensor pipe, bounded the K=256 GEMMs).  Each warp therefore transposes its
+// Each epilogue thread holds 32 consecutive columns of ONE row: storing straight from registers makes every
+// warp store touch 32 different 128-byte lines, 16 bytes each.  Each warp therefore transposes its
 // 32 x 32 block through a private, XOR-swizzled 4 KB shared-memory buffer (conflict-free both ways) and
 // writes it back row-contiguous: every store instruction covers whole lines (4 rows x 128 B for fp32).
 struct EpiCtx {
@@ -317,8 +259,8 @@ struct EpiCtx {
     int nvalid;         // rows of this warp's 32 that exist
 };
 
-// explicit shared-space accesses: through a generic pointer these compiled to LD.E/ST.E (generic), whose
-// latency the 2-warps-per-scheduler epilogue could not hide (ncu: 25 % of its samples waited on them)
+// explicit shared-space accesses: through a generic pointer these compile to generic LD.E/ST.E, whose
+// latency the epilogue warps cannot hide
 __device__ __forceinline__ void sts128(uint32_t a, const uint4& v) {
     asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
@@ -579,7 +521,7 @@ __device__ __forceinline__ void store_chunk(const TcParams& p, const EpiCtx& c, 
     }
     switch (LNC ? (int)MASR_EPI_RESIDUAL : p.epi) {
         case MASR_EPI_BIAS_SILU:
-            // eight independent SFU chains at a time (a one-register serial chain was 5x slower than the MMA loop)
+            // eight independent SFU chains at a time (a one-register serial chain would outlast the MMA loop)
 #pragma unroll
             for (int j = 0; j < 32; j += 8) {
                 float e[8];
@@ -605,10 +547,7 @@ __device__ __forceinline__ void store_chunk(const TcParams& p, const EpiCtx& c, 
             break;
         case MASR_EPI_RESIDUAL: {
             const bool vec_r = (p.ldr & 3) == 0 && (reinterpret_cast<uintptr_t>(p.residual) & 15) == 0;
-            if (p.flags & 16) {                               // the residual seeded the running sum (see the kernel): v = (r/alpha + A.W + bias)
-#pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] *= p.alpha;
-            } else if (BIG && (p.flags & 2) && n + 31 < p.N && vec_r) {
+            if (BIG && (p.flags & 2) && n + 31 < p.N && vec_r) {
                 uint4 rr[8];
                 staged_load(c, rr, reinterpret_cast<const uint8_t*>(p.residual + c.row0 * p.ldr + n), p.ldr * 4);
 #pragma unroll
@@ -670,151 +609,101 @@ __device__ __forceinline__ void store_chunk(const TcParams& p, const EpiCtx& c, 
     emit<32, STG>(p, c, v, n, p.N);
 }
 
-// Accumulation: the tensor core adds into its fp32 TMEM accumulator with truncation, so a long K loop
-// drifts (measured: 1.4e-5 abs at K=2048 vs 2e-6 for an fp32 FMA loop).  The main product therefore
-// accumulates in TMEM for at most CHUNK_KB K-blocks (K=256); the epilogue warps drain each chunk into
-// round-to-nearest fp32 registers while the next chunk runs into the other TMEM buffer (ping-pong).
-// The correction product is 2^-11 smaller, so its drift is irrelevant and it stays in TMEM for the tile.
+// Accumulation: the tensor core adds into its fp32 accumulator with truncation, so a long K loop drifts further
+// from the fp32 result than an FMA loop does.  The main product therefore accumulates in the
+// wgmma accumulator for at most CHUNK_KB K-blocks (K=256) and each chunk is added into a round-to-nearest fp32
+// running sum.  The correction product is 2^-11 smaller, so its drift is irrelevant and it accumulates over the tile.
 //
-// Persistent: grid = min(#tiles, #SMs); every CTA walks tiles blockIdx.x, +gridDim.x, ...  TMEM holds
-// main[2] (ping-pong by chunk) and corr[2] (ping-pong by tile) = 512 columns, so the MMA warp runs tile
-// i+1 while the 8 epilogue warps finish tile i.
-// LNC: the LayerNorm-fused variant (N = 256, launched as clusters of 2 CTAs = the two column tiles of a row block); its
-// per-warp store staging shrinks to 1 KB to make room for the 8 KB statistics exchange buffer.
+// Persistent: grid = min(#tiles, #SMs); every CTA walks tiles blockIdx.x, +gridDim.x, ...
+// LNC: the LayerNorm-fused variant (N = 256, launched as clusters of 2 CTAs = the two column tiles of a row block).
 constexpr int LN_RED_BYTES = 2 * 2 * 4 * 128 * 8;     // red[buffer][source CTA][column group][row] (mean, M2)
-__host__ __device__ constexpr int epi_stage_bytes(int ew, bool lnc) { return lnc ? 1024 * ew : EPI_STAGE_TOTAL; }
+constexpr int EPI_STG = 4096;                         // a warp's 32 x 32 fp32 block of the result tile, reused as its store staging
 
-// PAIR: the cta_group::2 form.  A cluster of 2 CTAs owns a 256 x 128 tile: CTA r stages A rows [128 r, 128 r + 128) and W rows
-// (output columns) [64 r, 64 r + 64) of every K-block in its own shared memory, all transaction bytes land on the LEADER's
-// (rank 0) full barrier, the leader's MMA thread issues M = 256 MMAs that read both CTAs' shared memory and write 128
-// accumulator rows into each CTA's tensor memory, and its commits arrive (multicast) on the empty / accumulator-full barriers
-// of both CTAs.  Each CTA's epilogue warps drain their own TMEM and release the accumulators on the leader's barriers.
-// Per SM and K-block that is 48 KB of TMA writes + 72 KB of operand reads instead of 64 + 96 KB: the 128 x 128 single-CTA
-// mainloop is bound by the 128 B/clk shared-memory port and the L2 -> SM fabric (profiles/r02_gemm_prof_summary.md).
-template <bool CONV, int EW, bool LNC, bool PAIR = false>
-__global__ void __launch_bounds__(tc_threads(EW), 1)
+// byte offset of (row r, column c) inside a warp's 32 x 32 fp32 block: 16-byte chunks XOR-swizzled by row, so that one
+// thread per row reading its 32 values (and staged_store<8>) is conflict-free
+__device__ __forceinline__ uint32_t res_off(int r, int c) { return (uint32_t)(r * 128 + ((((c >> 2) ^ (r & 7))) << 4) + (c & 3) * 4); }
+
+// PAIR: clusters of 2 CTAs own 256 x 128 tiles — CTA r computes rows [128 r, 128 r + 128) and loads W rows (output
+// columns) [64 r, 64 r + 64) of every K-block by TMA multicast into BOTH CTAs' stage, so each W tile crosses L2 -> SM once
+// per pair.  A stage is refilled only when the consumer warps of both CTAs have released it (empty barrier: 2 x 16
+// arrivals, half of them remote).  Same products in the same order as the single-CTA form: bit-identical outputs.
+template <bool CONV, bool LNC, bool PAIR = false>
+__global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ TcMaps maps, TcParams p, int num_tiles, int tiles_n, int tiles_t) {
-    static_assert(!LNC || (EW == 16 && !CONV), "the LayerNorm epilogue needs one 32-column chunk per epilogue warp");
-    static_assert(!(LNC && PAIR), "the LayerNorm-fused kernel pairs CTAs along N, the cta_group::2 kernel along M");
-    using R = RingCfg<PAIR>;
-    constexpr int EPI_BYTES = epi_stage_bytes(EW, LNC);
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* epi_stage = smem + R::STAGES * R::BYTES;                 // EPI_BYTES / EW per warp (see staged_store)
-    uint8_t* ln_red = epi_stage + EPI_BYTES;                          // LNC only
+    uint8_t* res = smem + TSTAGES * STAGE_BYTES;                      // fp32 result tile: [warpgroup][warp block] x 4 KB
+    uint8_t* ln_red = res + RES_BYTES;                                // LNC only
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(ln_red + (LNC ? LN_RED_BYTES : 0));
-    uint64_t* empty_bar = full_bar + MAX_STAGES;
-    uint64_t* main_full = empty_bar + MAX_STAGES;  // [2]
-    uint64_t* main_empty = main_full + 2;          // [2]
-    uint64_t* corr_full = main_empty + 2;          // [2]
-    uint64_t* corr_empty = corr_full + 2;          // [2]
-    uint64_t* ln_bar = corr_empty + 2;             // [2] (LNC)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(ln_bar + 2);
+    uint64_t* empty_bar = full_bar + TSTAGES;
+    uint64_t* ln_bar = empty_bar + TSTAGES;        // [2] (LNC; lnp: [0])
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nkb = p.K / TBK;
-    uint32_t crank = 0;                                               // PAIR: rank in the CTA pair (0 = leader)
+    static_assert(!(LNC && PAIR), "the LayerNorm-fused kernel pairs CTAs along N, the PAIR kernel along M");
+    uint32_t crank = 0;                                               // PAIR: rank in the cluster
     if (PAIR) asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(crank));
     const int tile_first = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
     const int tile_step = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-    // Tile schedule: CTA (pair) u of U walks tiles u, u + U, ... — or, with the LayerNorm prologue, the contiguous range
+    // Tile schedule: CTA u of U walks tiles u, u + U, ... — or, with the LayerNorm prologue, the contiguous range
     // [T u / U, T (u + 1) / U) (column tile fastest), so that it needs the rows of at most two row blocks and can normalise
     // them itself up front.
     const bool lnp = !LNC && !CONV && p.lnp_x != nullptr;
     const int tile_begin = lnp ? (int)((int64_t)num_tiles * tile_first / tile_step) : tile_first;
     const int tile_end = lnp ? (int)((int64_t)num_tiles * (tile_first + 1) / tile_step) : num_tiles;
     const int tile_stride = lnp ? 1 : tile_step;
-    // K <= 256 without a prefetched residual: the "direct" epilogue (TMEM -> registers -> stores, no running sum).
-    // (Tried and dropped, tools/step_ab.py: two groups of 8 epilogue warps taking alternate tiles, 64 columns per warp, to
-    // overlap the FP32 / MUFU / store phases that 16 warps on one tile run in lockstep -> step +1.4 %, not faster.)
-    const bool pre_res_k = (LNC || p.epi == MASR_EPI_RESIDUAL) && (p.flags & 16);
-    const bool direct = nkb <= CHUNK_KB && !pre_res_k;
-    const int acc_release = EW * (PAIR ? 2 : 1);                      // arrivals that hand an accumulator buffer back
 
-    if (warp == 0 && lane == 0) {
+    if (warp == EW && lane == 0) {
         tma_prefetch_desc(&maps.a[0]); tma_prefetch_desc(&maps.a[1]); tma_prefetch_desc(&maps.w[0]); tma_prefetch_desc(&maps.w[1]);
-        for (int s = 0; s < R::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
+        for (int s = 0; s < TSTAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], PAIR ? 2 * EW : EW); }
         for (int s = 0; s < 2; ++s) {
-            // PAIR: the accumulator-empty barriers that count are the leader's; the epilogue warps of both CTAs arrive there
-            mbar_init(&main_full[s], 1); mbar_init(&main_empty[s], acc_release);
-            mbar_init(&corr_full[s], 1); mbar_init(&corr_empty[s], acc_release);
             if (LNC) mbar_init(&ln_bar[s], 2 * EW);                  // one arrival per epilogue warp of both CTAs
             else if (lnp) mbar_init(&ln_bar[s], EW);                 // [0]: this CTA's rows are normalised
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        if (PAIR) {     // collective over the pair: the same warp of both CTAs, the same slot address
-            asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS));
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;");
-        } else {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS));
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-        }
-    }
-    tc_fence_before();
     __syncthreads();
-    // PAIR: nobody may signal a barrier of the other CTA (TMA transaction bytes, commits, accumulator releases) before that
-    // CTA has initialised it
+    // the peer CTA must have initialised its barriers before anybody arrives on them remotely: arrive here, wait (long
+    // since complete) right before the first exchange / after the producer loop
+    if (LNC) asm volatile("barrier.cluster.arrive.release;" ::: "memory");
+    // PAIR: the peer's multicast bytes and releases may only reach barriers that have been initialised
     if (PAIR) {
         asm volatile("barrier.cluster.arrive.release;" ::: "memory");
         asm volatile("barrier.cluster.wait.acquire;" ::: "memory");
     }
-    // the peer CTA must have initialised its barriers before anybody arrives on them remotely: arrive here, wait (long
-    // since complete) right before the first exchange / after the producer and MMA loops
-    if (LNC) asm volatile("barrier.cluster.arrive.release;" ::: "memory");
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    // programmatic dependent launch: everything above (barriers, TMEM allocation, descriptor prefetch) overlapped the
-    // producer kernel's tail; no global memory has been touched yet
+    // programmatic dependent launch: everything above overlapped the producer kernel's tail; no global memory touched yet
     pdl_wait();
     pdl_launch_dependents();
 
-    // tile -> coordinates.  PAIR: `tile` numbers 256-row (CONV: 12 time rows) pair tiles, this CTA owns half `crank` of it;
-    // a half that lies beyond M / T2 loads zeros and stores nothing
     auto decode = [&](int tile, int& n0, int& m0, int& t0, int& b) {
         const int nt = tile % tiles_n;
         const int rest = tile / tiles_n;
         n0 = nt * TBN;
+        // PAIR: `tile` numbers 256-row (CONV: 12 time rows) pair tiles, this CTA owns half `crank` of it; a half beyond
+        // M / T2 loads zeros and stores nothing
         if (CONV) { t0 = ((rest % tiles_t) * (PAIR ? 2 : 1) + (int)crank) * CONV_TR; b = rest / tiles_t; m0 = 0; }
         else { m0 = (rest * (PAIR ? 2 : 1) + (int)crank) * TBM; t0 = 0; b = 0; }
     };
 
-    if (warp == 0) {
+    if (warp == EW) {
+        // ---- TMA producer ----
         if (elect_one_sync()) {
             constexpr uint32_t a_bytes = CONV ? CONV_ROWS * TBK * 2 : TILE_BYTES;
-            constexpr uint32_t tx_bytes = (2 * a_bytes + 2 * R::W_BYTES) * (PAIR ? 2 : 1);   // PAIR: both CTAs' boxes
+            constexpr uint32_t tx_bytes = 2 * a_bytes + 2 * TILE_BYTES;
             uint32_t kg = 0;
-            if (lnp) mbar_wait(&ln_bar[0], 0);      // the epilogue warps have written this CTA's A rows (LayerNorm prologue)
+            if (lnp) mbar_wait(&ln_bar[0], 0);      // the consumer warps have written this CTA's A rows (LayerNorm prologue)
             for (int tile = tile_begin; tile < tile_end; tile += tile_stride) {
                 int n0, m0, t0, b;
                 decode(tile, n0, m0, t0, b);
                 for (int kb = 0; kb < nkb; ++kb, ++kg) {
-                    const uint32_t s = kg % R::STAGES;
-                    mbar_wait(&empty_bar[s], ((kg / R::STAGES) & 1) ^ 1);
-                    uint8_t* st = smem + s * R::BYTES;
+                    const uint32_t s = kg % TSTAGES;
+                    mbar_wait(&empty_bar[s], ((kg / TSTAGES) & 1) ^ 1);
+                    uint8_t* st = smem + s * STAGE_BYTES;
                     if (p.flags & 32) {      // profiling switch (tools/gemm_bound_probe.py): no loads, the MMAs run on stale tiles
-                        if (!PAIR || crank == 0) mbar_arrive(&full_bar[s]);
+                        mbar_arrive(&full_bar[s]);
                         continue;
                     }
-                    if (!PAIR || crank == 0) mbar_expect_tx(&full_bar[s], tx_bytes);
-                    if (PAIR) {
-                        const uint32_t fb = mapa_u32(smem_u32(&full_bar[s]), 0);     // the leader's barrier
-                        const int wrow = n0 + (int)crank * (TBN / 2);
-                        if (CONV) {
-                            const int tap = kb >> 2, cj = kb & 3;
-                            const int kh = tap / 3, kw = tap - kh * 3;
-                            const int plane = (kh & 1) * 2 + (kw & 1);
-                            tma_load_4d_pair(&maps.a[2 * plane], fb, st, cj * TBK, kw >> 1, t0 + (kh >> 1), b);
-                            tma_load_4d_pair(&maps.a[2 * plane + 1], fb, st + TILE_BYTES, cj * TBK, kw >> 1, t0 + (kh >> 1), b);
-                        } else {
-                            tma_load_2d_pair(&maps.a[0], fb, st, kb * TBK, m0);
-                            tma_load_2d_pair(&maps.a[1], fb, st + TILE_BYTES, kb * TBK, m0);
-                        }
-                        tma_load_2d_pair(&maps.w[0], fb, st + 2 * TILE_BYTES, kb * TBK, wrow);      // box: 64 rows
-                        tma_load_2d_pair(&maps.w[1], fb, st + 2 * TILE_BYTES + R::W_BYTES, kb * TBK, wrow);
-                        continue;
-                    }
+                    mbar_expect_tx(&full_bar[s], tx_bytes);
                     if (CONV) {
                         const int tap = kb >> 2, cj = kb & 3;       // K index = tap*256 + cj*64  (C = 256)
                         const int kh = tap / 3, kw = tap - kh * 3;
@@ -825,64 +714,31 @@ tc_gemm_kernel(const __grid_constant__ TcMaps maps, TcParams p, int num_tiles, i
                         tma_load_2d(&maps.a[0], &full_bar[s], st, kb * TBK, m0);
                         tma_load_2d(&maps.a[1], &full_bar[s], st + TILE_BYTES, kb * TBK, m0);
                     }
-                    tma_load_2d(&maps.w[0], &full_bar[s], st + 2 * TILE_BYTES, kb * TBK, n0);
-                    tma_load_2d(&maps.w[1], &full_bar[s], st + 3 * TILE_BYTES, kb * TBK, n0);
+                    if (PAIR) {          // box: 64 rows, this CTA's half of the W tile, to both CTAs
+                        const uint32_t half = crank * (TILE_BYTES / 2);
+                        tma_load_2d_mc(&maps.w[0], &full_bar[s], st + 2 * TILE_BYTES + half, kb * TBK, n0 + (int)crank * (TBN / 2), 3);
+                        tma_load_2d_mc(&maps.w[1], &full_bar[s], st + 3 * TILE_BYTES + half, kb * TBK, n0 + (int)crank * (TBN / 2), 3);
+                    } else {
+                        tma_load_2d(&maps.w[0], &full_bar[s], st + 2 * TILE_BYTES, kb * TBK, n0);
+                        tma_load_2d(&maps.w[1], &full_bar[s], st + 3 * TILE_BYTES, kb * TBK, n0);
+                    }
                 }
             }
         }
-        if (LNC) asm volatile("barrier.cluster.wait.acquire;" ::: "memory");
-    } else if (warp == 1) {
-        if ((!PAIR || crank == 0) && elect_one_sync()) {
-            // instruction descriptor: D=f32 (bit 4), A=B=f16 (0), K-major both, N>>3 @17, M>>4 @24 (PAIR: M = 256 over two CTAs)
-            constexpr uint32_t idesc = (1u << 4) | ((uint32_t)(TBN >> 3) << 17) | ((uint32_t)((PAIR ? 2 * TBM : TBM) >> 4) << 24);
-            auto mma = [](uint32_t d, uint64_t da, uint64_t db, uint32_t acc) {
-                if (PAIR) umma_f16_pair(d, da, db, idesc, acc); else umma_f16(d, da, db, idesc, acc);
-            };
-            auto commit = [](uint64_t* bar) { if (PAIR) umma_commit_pair(bar); else umma_commit(bar); };
-            uint32_t kg = 0, cg = 0, tl = 0;
-            for (int tile = tile_begin; tile < tile_end; tile += tile_stride, ++tl) {
-                mbar_wait(&corr_empty[tl & 1], ((tl >> 1) & 1) ^ 1);    // epilogue has read corr of tile tl-2
-                tc_fence_after();
-                const uint32_t d_corr = tmem_base + 2 * TBN + (tl & 1) * TBN;
-                for (int kb = 0; kb < nkb; ++kb, ++kg) {
-                    const uint32_t s = kg % R::STAGES;
-                    const bool first = (kb % CHUNK_KB) == 0;
-                    const bool last = (kb % CHUNK_KB) == CHUNK_KB - 1 || kb == nkb - 1;
-                    if (first) {
-                        mbar_wait(&main_empty[cg & 1], ((cg >> 1) & 1) ^ 1);  // epilogue drained this buffer (chunk cg-2)
-                        tc_fence_after();
-                    }
-                    const uint32_t d_main = tmem_base + (cg & 1) * TBN;
-                    mbar_wait(&full_bar[s], (kg / R::STAGES) & 1);
-                    tc_fence_after();
-                    const uint32_t sa = smem_u32(smem + s * R::BYTES);
-                    const uint64_t dAh = umma_desc_k_sw128(sa), dAl = umma_desc_k_sw128(sa + TILE_BYTES);
-                    const uint64_t dWh = umma_desc_k_sw128(sa + 2 * TILE_BYTES), dWl = umma_desc_k_sw128(sa + 2 * TILE_BYTES + R::W_BYTES);
-                    if (!(p.flags & 64))     // profiling switch: loads only, no MMAs
-#pragma unroll
-                    for (int ks = 0; ks < TBK / 16; ++ks) {
-                        const uint64_t adv = (uint64_t)(ks * 2);      // 16 halves = 32 B = 2 x 16-byte units
-                        mma(d_main, dAh + adv, dWh + adv, (first && ks == 0) ? 0u : 1u);
-                        mma(d_corr, dAh + adv, dWl + adv, (kb | ks) ? 1u : 0u);
-                        mma(d_corr, dAl + adv, dWh + adv, 1u);
-                    }
-                    commit(&empty_bar[s]);                             // slot reusable once these MMAs retire
-                    if (last) { commit(&main_full[cg & 1]); ++cg; }
-                }
-                commit(&corr_full[tl & 1]);                            // whole tile (incl. corrections) complete
-            }
-        }
+        __syncwarp();
         if (LNC) asm volatile("barrier.cluster.wait.acquire;" ::: "memory");
     } else {
-        // ---- EW epilogue warps: TMEM lane quarter = warp % 4, column group = (warp - 2) / 4 (CW columns each) ----
-        constexpr int CW = TBN / (EW / 4);                             // 64 columns per warp (EW = 8) or 32 (EW = 16)
-        constexpr int NCH = CW / 32;                                   // 32-column chunks per warp
-        constexpr int STG = EPI_BYTES / EW;
-        const int q = warp & 3, cgrp = (warp - 2) >> 2;
-        const uint32_t lane_base = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)cgrp * CW;
+        // ---- 4 consumer warpgroups: wg owns tile rows [64 (wg & 1), +64) x columns [64 (wg >> 1), +64) ----
+        const int wg = warp >> 2, wi = warp & 3;
+        const int wm = wg & 1, wn = wg >> 1;
+        // epilogue: warp wi of the warpgroup takes the 32 x 32 block (row half wi & 1, column half wi >> 1) of its quarter;
+        // q = 32-row group of the tile, cgrp = 32-column group
+        const int q = 2 * wm + (wi & 1), cgrp = 2 * wn + (wi >> 1);
+        uint8_t* wg_res = res + wg * (RES_BYTES / 4);
+        const uint32_t my_block = smem_u32(wg_res) + wi * EPI_STG;
         const int nchunks = (nkb + CHUNK_KB - 1) / CHUNK_KB;
         EpiCtx ctx;
-        ctx.sb = smem_u32(epi_stage) + (warp - 2) * STG;
+        ctx.sb = my_block;
         ctx.lane = lane;
         LnCtx lnx;
         if (LNC) {
@@ -894,10 +750,6 @@ tc_gemm_kernel(const __grid_constant__ TcMaps maps, TcParams p, int num_tiles, i
             asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(lnx.bar_peer) : "r"(lnx.bar), "r"(rank ^ 1u));
             asm volatile("barrier.cluster.wait.acquire;" ::: "memory");
         }
-        // accumulator release: PAIR -> the leader's barrier (a shared::cluster address; the leader's own for rank 0)
-        auto release = [&](uint64_t* bar) {
-            if (PAIR) mbar_arrive_cluster(mapa_u32(smem_u32(bar), 0)); else mbar_arrive(bar);
-        };
         // row mapping: the warp's 32 tile rows are 32 consecutive output rows in both modes
         auto map_rows = [&](int m0, int t0, int b) {
             if (CONV) {
@@ -910,52 +762,14 @@ tc_gemm_kernel(const __grid_constant__ TcMaps maps, TcParams p, int num_tiles, i
                 ctx.nvalid = max(0, min(32, p.M - (m0 + q * 32)));
             }
         };
-        // direct epilogue of one 32-column slice (tile columns [col, col + 32) = output columns [n, n + 32)) of accumulator
-        // buffer `buf`: v = main + 2^-11 * correction + bias in packed fp32 pairs, the bias from warp-uniform 128-bit loads
-        // (one broadcast transaction each, L1 hits after bias_prefetch) instead of 32 shuffles
-        const uint32_t lane_tm = tmem_base + ((uint32_t)(q * 32) << 16);
-        auto bias_prefetch = [&](int nw, int cols) {
-            if (p.bias != nullptr && lane * 32 < cols && nw + lane * 32 < p.N)
-                asm volatile("prefetch.global.L1 [%0];" ::"l"(p.bias + nw + lane * 32));
-        };
-        auto direct_slice = [&](uint32_t col, int n, bool last, uint32_t buf) {
-            uint32_t r[32], rc[32];
-            tmem_ld32(lane_tm + buf * TBN + col, r);
-            tmem_ld32(lane_tm + 2 * TBN + buf * TBN + col, rc);
-            tmem_ld_wait();
-            if (last) {                                           // TMEM released: the rest runs from registers
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) { release(&main_empty[buf]); release(&corr_empty[buf]); }
-            }
-            if (n >= p.N) return;                                  // warp-uniform
-            float v[32];
-            if (p.bias != nullptr && n + 31 < p.N && (reinterpret_cast<uintptr_t>(p.bias + n) & 15) == 0) {
-#pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    const float4 bb = ldg_f4(p.bias + n + j);
-                    fma2(v[j], v[j + 1], __uint_as_float(rc[j]), __uint_as_float(rc[j + 1]), kLoInv, kLoInv, __uint_as_float(r[j]), __uint_as_float(r[j + 1]));
-                    fma2(v[j + 2], v[j + 3], __uint_as_float(rc[j + 2]), __uint_as_float(rc[j + 3]), kLoInv, kLoInv, __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-                    add2(v[j], v[j + 1], v[j], v[j + 1], bb.x, bb.y);
-                    add2(v[j + 2], v[j + 3], v[j + 2], v[j + 3], bb.z, bb.w);
-                }
-            } else {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const float bj = (p.bias != nullptr && n + j < p.N) ? __ldg(p.bias + n + j) : 0.f;
-                    v[j] = fmaf(__uint_as_float(rc[j]), kLoInv, __uint_as_float(r[j])) + bj;
-                }
-            }
-            store_chunk<STG, LNC>(p, ctx, v, n, lnx);
-        };
         if (lnp) {
-            // LayerNorm prologue: the 16 epilogue warps normalise this CTA's 128 rows of every row block its tile range touches
+            // LayerNorm prologue: the 16 consumer warps normalise this CTA's 128 rows of every row block its tile range touches
             // (8 rows per warp and block, 4 rows in flight) into the pair buffer the A loads read.  A block shared with the
             // neighbouring CTA's range is written twice with identical values.
             if (tile_begin < tile_end) {
                 const int b0 = tile_begin / tiles_n, b1 = (tile_end - 1) / tiles_n;
                 for (int blk = b0; blk <= b1; ++blk) {
-                    const int mrow0 = (blk * (PAIR ? 2 : 1) + (int)crank) * TBM + (warp - 2) * (TBM / EW);
+                    const int mrow0 = (blk * (PAIR ? 2 : 1) + (int)crank) * TBM + warp * (TBM / EW);
 #pragma unroll
                     for (int r4 = 0; r4 < TBM / EW; r4 += 4) {
                         float4 xv[4][2];
@@ -984,116 +798,112 @@ tc_gemm_kernel(const __grid_constant__ TcMaps maps, TcParams p, int num_tiles, i
             __syncwarp();
             if (lane == 0) mbar_arrive(&ln_bar[0]);
         }
-        uint32_t cg = 0, tl = 0;
-        for (int tile = tile_begin; tile < tile_end; tile += tile_stride, ++tl) {
+        const uint32_t wg_bar = 1 + wg;              // named barrier of the warpgroup (0 is __syncthreads)
+        uint32_t kg = 0;
+        for (int tile = tile_begin; tile < tile_end; tile += tile_stride) {
             int n0, m0, t0, b;
             decode(tile, n0, m0, t0, b);
-            const int nw = n0 + cgrp * CW;                             // first column of this warp
             map_rows(m0, t0, b);
-            if (direct) {
-                // K <= 256: main and correction accumulators complete together (one chunk per tile: cg == tl); go straight
-                // from TMEM to the stores 32 columns at a time (no 64-register running sum, so the activations keep their ILP)
-                bias_prefetch(nw, CW);
-                mbar_wait(&main_full[tl & 1], (tl >> 1) & 1);
-                mbar_wait(&corr_full[tl & 1], (tl >> 1) & 1);
-                tc_fence_after();
+            const int nw = n0 + cgrp * 32;                             // first column of this warp's epilogue block
+            if (p.bias != nullptr && nw + lane < p.N) asm volatile("prefetch.global.L1 [%0];" ::"l"(p.bias + nw + lane));
+            float acc[32], cor[32];
+            // fragment of m64n64: this thread holds rows 16 wi + lane / 4 (+ 8) and columns 8 i + 2 (lane % 4) (+ 1), i = 0..7;
+            // element (i, hh) lives at frag_addr(i, hh) in the warpgroup's quarter of the result tile
+            auto frag_addr = [&](int i, int hh) {
+                const int R = 16 * wi + (lane >> 2) + 8 * hh, C = 8 * i + 2 * (lane & 3);
+                return smem_u32(wg_res) + ((R >> 5) + 2 * (C >> 5)) * EPI_STG + res_off(R & 31, C & 31);
+            };
+            asm volatile("bar.sync %0, 128;" ::"r"(wg_bar) : "memory");   // every warp is done with the previous tile's block
+            for (int c = 0; c < nchunks; ++c) {
+                const int kb_end = min(nkb, (c + 1) * CHUNK_KB);
+                for (int kb = c * CHUNK_KB; kb < kb_end; ++kb, ++kg) {
+                    const uint32_t s = kg % TSTAGES;
+                    mbar_wait(&full_bar[s], (kg / TSTAGES) & 1);
+                    const uint32_t sa = smem_u32(smem + s * STAGE_BYTES);
+                    const uint32_t sa_m = sa + wm * (TILE_BYTES / 2), sw_n = sa + 2 * TILE_BYTES + wn * (TILE_BYTES / 2);
+                    const uint64_t dAh = gmma_desc_sw128(sa_m), dAl = gmma_desc_sw128(sa_m + TILE_BYTES);
+                    const uint64_t dWh = gmma_desc_sw128(sw_n), dWl = gmma_desc_sw128(sw_n + TILE_BYTES);
+                    if (!(p.flags & 64)) {   // profiling switch: loads only, no MMAs
+                        reg_fence(acc); reg_fence(cor);
+                        wgmma_fence();
 #pragma unroll
-                for (int cc = 0; cc < NCH; ++cc) direct_slice((uint32_t)(cgrp * CW + cc * 32), nw + cc * 32, cc == NCH - 1, tl & 1);
-                ++cg;
-                continue;
-            }
-            // bias of the warp's columns: lane l keeps columns l (and 32+l), broadcast by shuffle below;
-            // fetched before the accumulator wait so its latency is hidden
-            float bias0 = 0.f, bias1 = 0.f;
-            if (p.bias != nullptr) {
-                if (nw + lane < p.N) bias0 = __ldg(p.bias + nw + lane);
-                if (NCH > 1 && nw + 32 + lane < p.N) bias1 = __ldg(p.bias + nw + 32 + lane);
-            }
-            // Residual epilogues (flags bit 4): this thread's residual values are fetched NOW, before the first accumulator
-            // is ready, and seed the running sum as residual / alpha (alpha is a power of two: exact), so the finished row is
-            // alpha * (sum + bias).  ncu r02: loaded after the last MMA, the row-strided residual read (8 x LDG.128 per
-            // thread, 32 lines per instruction) was more than half of the exposed epilogue of the single-tile-per-CTA GEMMs
-            // (w_2: ~11 of 34 us).
-            const bool pre_res = (LNC || p.epi == MASR_EPI_RESIDUAL) && (p.flags & 16);
-            float acc[CW];
-#pragma unroll
-            for (int j = 0; j < CW; ++j) acc[j] = 0.f;
-            if (pre_res && lane < ctx.nvalid) {
-#pragma unroll
-                for (int cc = 0; cc < NCH; ++cc) {
-                    const int n = nw + cc * 32;
-                    const float* r = p.residual + (ctx.row0 + lane) * p.ldr + n;
-                    if (n + 31 < p.N) {                                   // (host checked ldr % 4 == 0 and the 16-byte alignment)
-#pragma unroll
-                        for (int j = 0; j < 32; j += 4) {
-                            const float4 rv = *reinterpret_cast<const float4*>(r + j);
-                            acc[cc * 32 + j] = rv.x * p.inv_alpha; acc[cc * 32 + j + 1] = rv.y * p.inv_alpha;
-                            acc[cc * 32 + j + 2] = rv.z * p.inv_alpha; acc[cc * 32 + j + 3] = rv.w * p.inv_alpha;
+                        for (int ks = 0; ks < TBK / 16; ++ks) {
+                            const uint64_t adv = (uint64_t)(ks * 2);      // 16 halves = 32 B = 2 x 16-byte units
+                            wgmma_m64n64k16_ss(acc, dAh + adv, dWh + adv, (kb == c * CHUNK_KB && ks == 0) ? 0u : 1u);
+                            wgmma_m64n64k16_ss(cor, dAh + adv, dWl + adv, (kb | ks) ? 1u : 0u);
+                            wgmma_m64n64k16_ss(cor, dAl + adv, dWh + adv, 1u);
                         }
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (n + j < p.N) acc[cc * 32 + j] = r[j] * p.inv_alpha;
+                        wgmma_commit();
+                        wgmma_wait<0>();
+                        reg_fence(acc); reg_fence(cor);
+                    }
+                    __syncwarp();
+                    if (lane == 0) {                                   // slot reusable: this warp's MMAs have retired
+                        mbar_arrive(&empty_bar[s]);
+                        if (PAIR) mbar_arrive_remote(&empty_bar[s], crank ^ 1u);   // the peer multicasts into this stage too
                     }
                 }
-            }
-            for (int c = 0; c < nchunks; ++c, ++cg) {
-                mbar_wait(&main_full[cg & 1], (cg >> 1) & 1);
-                tc_fence_after();
+                // K > 256: the running fp32 sum of the chunks is kept, per thread, at its own elements of the result tile
+                const bool last = c == nchunks - 1;
+                if (c > 0 || !last) {
 #pragma unroll
-                for (int cc = 0; cc < NCH; ++cc) {
-                    uint32_t r[32];
-                    tmem_ld32(lane_base + (cg & 1) * TBN + cc * 32, r);
-                    tmem_ld_wait();
+                    for (int i = 0; i < 8; ++i)
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) acc[cc * 32 + j] += __uint_as_float(r[j]);
+                        for (int hh = 0; hh < 2; ++hh) {
+                            float x0 = acc[4 * i + 2 * hh], x1 = acc[4 * i + 2 * hh + 1];
+                            const uint32_t a = frag_addr(i, hh);
+                            if (c > 0) {
+                                float s0, s1;
+                                asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(s0), "=f"(s1) : "r"(a) : "memory");
+                                x0 = s0 + x0; x1 = s1 + x1;
+                            }
+                            if (last) { acc[4 * i + 2 * hh] = x0; acc[4 * i + 2 * hh + 1] = x1; }
+                            else asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(x0), "f"(x1) : "memory");
+                        }
                 }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) release(&main_empty[cg & 1]);
             }
-            mbar_wait(&corr_full[tl & 1], (tl >> 1) & 1);
-            tc_fence_after();
+            // result (without bias) = sum + 2^-11 * correction -> the warpgroup's quarter of the result tile
 #pragma unroll
-            for (int cc = 0; cc < NCH; ++cc) {
-                uint32_t rc[32];
-                tmem_ld32(lane_base + 2 * TBN + (tl & 1) * TBN + cc * 32, rc);
-                tmem_ld_wait();
+            for (int i = 0; i < 8; ++i)
 #pragma unroll
-                for (int j = 0; j < 32; ++j) acc[cc * 32 + j] = fmaf(__uint_as_float(rc[j]), kLoInv, acc[cc * 32 + j]);
+                for (int hh = 0; hh < 2; ++hh) {
+                    const float x0 = fmaf(cor[4 * i + 2 * hh], kLoInv, acc[4 * i + 2 * hh]);
+                    const float x1 = fmaf(cor[4 * i + 2 * hh + 1], kLoInv, acc[4 * i + 2 * hh + 1]);
+                    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(frag_addr(i, hh)), "f"(x0), "f"(x1) : "memory");
+                }
+            asm volatile("bar.sync %0, 128;" ::"r"(wg_bar) : "memory");
+            if (nw >= p.N) continue;                                   // warp-uniform
+            float v[32];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+                const uint4 r4 = lds128(my_block + lane * 128 + ((k ^ (lane & 7)) << 4));
+                v[4 * k] = __uint_as_float(r4.x); v[4 * k + 1] = __uint_as_float(r4.y);
+                v[4 * k + 2] = __uint_as_float(r4.z); v[4 * k + 3] = __uint_as_float(r4.w);
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) release(&corr_empty[tl & 1]);               // TMEM released: the rest runs from registers
+            if (p.bias != nullptr && nw + 31 < p.N && (reinterpret_cast<uintptr_t>(p.bias + nw) & 15) == 0) {
 #pragma unroll
-            for (int cc = 0; cc < NCH; ++cc) {
-                const int n = nw + cc * 32;
-                if (n >= p.N) break;                                   // warp-uniform
-                float v[32];
-                const float bsrc = cc ? bias1 : bias0;
+                for (int j = 0; j < 32; j += 4) {
+                    const float4 bb = ldg_f4(p.bias + nw + j);      // warp-uniform address: one broadcast transaction
+                    v[j] += bb.x; v[j + 1] += bb.y; v[j + 2] += bb.z; v[j + 3] += bb.w;
+                }
+            } else if (p.bias != nullptr) {
 #pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] = acc[cc * 32 + j] + __shfl_sync(0xffffffffu, bsrc, j);
-                store_chunk<STG, LNC>(p, ctx, v, n, lnx);
+                for (int j = 0; j < 32; ++j)
+                    if (nw + j < p.N) v[j] += __ldg(p.bias + nw + j);
             }
+            store_chunk<EPI_STG, LNC>(p, ctx, v, nw, lnx);
         }
     }
-    tc_fence_before();
     __syncthreads();
     if (LNC || PAIR) {      // neither CTA may exit while its peer can still write into its shared memory / arrive on its barriers
         asm volatile("barrier.cluster.arrive.release;" ::: "memory");
         asm volatile("barrier.cluster.wait.acquire;" ::: "memory");
     }
-    if (warp == 1) {
-        tc_fence_after();
-        __syncwarp();
-        if (PAIR) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
-        else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
-    }
 }
 
-constexpr size_t kTcSmem = TSTAGES * STAGE_BYTES + EPI_STAGE_TOTAL + 1024 /*align*/ + 256 /*barriers + tmem slot*/;
-constexpr size_t kTcSmemLn = TSTAGES * STAGE_BYTES + epi_stage_bytes(16, true) + LN_RED_BYTES + 1024 + 256;
-static_assert(kTcSmem <= 232448 && kTcSmemLn <= 232448, "tc_gemm shared memory exceeds the 227 KB per-CTA limit of sm_100");
+constexpr size_t kTcSmem = TSTAGES * STAGE_BYTES + RES_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+constexpr size_t kTcSmemLn = kTcSmem + LN_RED_BYTES;
+static_assert(kTcSmem <= 232448 && kTcSmemLn <= 232448, "tc_gemm shared memory exceeds the 227 KB per-CTA limit of sm_90");
 
 // ---- fp32 -> (h,l) split, elementwise (weights at load time; activations produced by SIMT kernels) ----
 __global__ void __launch_bounds__(256) split_f16_kernel(const float* __restrict__ x, __half* __restrict__ h,
@@ -1169,7 +979,7 @@ static EncodeTiledFn get_encode_fn() {
     return fn;
 }
 
-// [rows, K] fp16 row-major (ld elements), box = 64 (K) x box_rows (128; 64 for the W halves of the PAIR kernels),
+// [rows, K] fp16 row-major (ld elements), box = 64 (K) x box_rows (128),
 // 128-byte swizzle, zero OOB fill
 static int make_map_2d(CUtensorMap* map, const void* ptr, int64_t rows, int64_t K, int64_t ld, int box_rows = TBM) {
     EncodeTiledFn fn = get_encode_fn();
@@ -1202,24 +1012,13 @@ static int make_map_plane(CUtensorMap* map, const void* ptr, int B, int TH, int 
     return MASR_OK;
 }
 
-// Kernel-variant flags, MASR_TC_FLAGS overrides for A/B runs (tools/gemm_bench.py; B200, M = 7936):
-//   bit 0  staged (row-contiguous) epilogue stores      ffn_w1 58.5 -> 42.1 us, qkv 35.5 -> 23.5, ctc head 91 -> 63
-//   bit 1  stage the residual READ as well              did not pay (w_2 31 -> 35 us); off
-//   bit 2  16 epilogue warps x 32 columns instead of 8 x 64   ffn_w1 43.1 -> 35.0 us, step 4.88 -> 4.59 ms
+// Kernel-variant flags, MASR_TC_FLAGS overrides for A/B runs (tools/gemm_bench.py):
+//   bit 0  staged (row-contiguous) epilogue stores
+//   bit 1  stage the residual READ as well (off)
 //   bits 5, 6  profiling only (results are garbage): 32 = skip the TMA loads, 64 = skip the MMAs (tools/gemm_bound_probe.py)
 static int tc_flags() {
     const char* e = getenv("MASR_TC_FLAGS");
-    return e ? atoi(e) : 5;
-}
-
-// flags bit 4: prefetch the residual into the running sum — needs alpha to be a power of two (so that r / alpha and the final
-// scaling are exact) and 16-byte aligned residual rows.  MASR_TC_PRERES=0 disables it.
-static int preres_flag(const float* residual, int64_t ldr, float alpha) {
-    static int enabled = -1;
-    if (enabled < 0) { const char* e = getenv("MASR_TC_PRERES"); enabled = e ? atoi(e) != 0 : 1; }
-    int ex = 0;
-    const float mant = frexpf(alpha, &ex);
-    return (enabled && residual && mant == 0.5f && (ldr & 3) == 0 && (reinterpret_cast<uintptr_t>(residual) & 15) == 0) ? 16 : 0;
+    return e ? atoi(e) : 1;
 }
 
 static int num_sms() {
@@ -1229,7 +1028,7 @@ static int num_sms() {
     if (dev < 0 || dev >= 64) dev = 0;
     if (n[dev] == 0) {
         int v = 0;
-        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
         n[dev] = v;
     }
     return n[dev];
@@ -1240,35 +1039,42 @@ static int ensure_tc_attrs() {
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) dev = 0;
     if (!g_tc_attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(tc_gemm_kernel<false, 8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gemm_kernel<true, 8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gemm_kernel<false, 16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gemm_kernel<true, 16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gemm_kernel<false, 16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmemLn);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gemm_kernel<false, 16, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gemm_kernel<true, 16, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem);
+        cudaError_t e = cudaFuncSetAttribute(tc_gemm_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gemm_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gemm_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmemLn);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gemm_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gemm_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem);
         if (e != cudaSuccess) { set_last_error("tc_gemm smem attr: %s", cudaGetErrorString(e)); return (int)e; }
         g_tc_attr_set[dev] = true;
     }
     return MASR_OK;
 }
 
-// PAIR (cta_group::2) kernels: the default wherever there is more than one row block.  MASR_TC_PAIR=0 keeps the single-CTA
-// kernel (A/B runs: tools/pair_gemm_check.py per GEMM, tools/step_ab.py for the whole step — B200, 32 x 10 s: 3.64 -> 3.54 ms
-// with every GEMM paired; per GEMM the mainloop of a pair tile is ~15 % shorter, the pair's start-up costs ~0.4 us).
-// Needs the 16-epilogue-warp variant (flags bit 2).
-static bool pair_enabled(int flags, int K, int tiles, bool conv) {
-    (void)K; (void)tiles; (void)conv;
-    if (!(flags & 4)) return false;
-    const char* e = getenv("MASR_TC_PAIR");             // read per call: the A/B tools flip it inside one process
-    return e ? atoi(e) != 0 : true;
+// PAIR kernels (clusters of 2 CTAs along M, W multicast) with MASR_TC_PAIR=1, wherever there is more than one row block;
+// read per call, the A/B tools flip it inside one process.  Off by default: H100 (400 W), headline step 17.2 ms paired vs
+// 15.4 ms single-CTA, outputs bit-identical.
+static bool pair_enabled(bool several_row_blocks) {
+    const char* e = getenv("MASR_TC_PAIR");
+    return several_row_blocks && e != nullptr && atoi(e) != 0;
 }
 
-// Launch a PAIR kernel over `num_ptiles` pair tiles: clusters of 2 CTAs, as many pairs as fit on the device at one CTA per SM.
+// Persistent launch over `tiles_m` row blocks (CONV: time-row tiles per utterance, `batch` utterances) x `tiles_n` column
+// tiles: min(#tiles, #SMs) CTAs, or with `pair` min(#pair tiles, #SMs / 2) clusters of 2 CTAs.  The W tensor maps must
+// have 64-row boxes for the pair form.
 template <bool CONV>
-static void launch_pair(const TcMaps& maps, const TcParams& p, int num_ptiles, int tiles_n, int tiles_t, cudaStream_t stream) {
+static void launch_tc(const TcMaps& maps, const TcParams& p, bool pair, int tiles_n, int tiles_m, int batch, cudaStream_t stream) {
+    if (!pair) {
+        const int num_tiles = tiles_n * tiles_m * batch;
+        const int grid = num_tiles < num_sms() ? num_tiles : num_sms();
+        launch_pdl(tc_gemm_kernel<CONV, false>, dim3(grid), dim3(TC_THREADS), kTcSmem, stream, maps, p, num_tiles, tiles_n, tiles_m);
+        return;
+    }
+    const int ptiles_m = (tiles_m + 1) / 2;
+    const int num_ptiles = tiles_n * ptiles_m * batch;
+    const int pairs = num_ptiles < num_sms() / 2 ? num_ptiles : num_sms() / 2;
     cudaLaunchConfig_t cfg = {};
-    cfg.blockDim = dim3(tc_threads(16));
+    cfg.gridDim = dim3(2 * pairs);
+    cfg.blockDim = dim3(TC_THREADS);
     cfg.dynamicSmemBytes = kTcSmem;
     cfg.stream = stream;
     cudaLaunchAttribute attr[2];
@@ -1277,24 +1083,8 @@ static void launch_pair(const TcMaps& maps, const TcParams& p, int num_ptiles, i
     attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    static int max_pairs[64] = {0};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) dev = 0;
-    if (max_pairs[dev] == 0) {
-        int n = 0;
-        cfg.gridDim = dim3(num_sms() & ~1);
-        cfg.numAttrs = 1;
-        if (cudaOccupancyMaxActiveClusters(&n, tc_gemm_kernel<CONV, 16, false, true>, &cfg) != cudaSuccess || n <= 0) {
-            cudaGetLastError();
-            n = num_sms() / 2;
-        }
-        max_pairs[dev] = n < num_sms() / 2 ? n : num_sms() / 2;
-    }
-    const int pairs = num_ptiles < max_pairs[dev] ? num_ptiles : max_pairs[dev];
-    cfg.gridDim = dim3(2 * pairs);
     cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    cudaLaunchKernelEx(&cfg, tc_gemm_kernel<CONV, 16, false, true>, maps, p, num_ptiles, tiles_n, tiles_t);
+    cudaLaunchKernelEx(&cfg, tc_gemm_kernel<CONV, false, true>, maps, p, num_ptiles, tiles_n, ptiles_m);
 }
 
 }  // namespace masr
@@ -1319,21 +1109,13 @@ extern "C" int masr_conv2_tc_f16x2(const void* c1h, const void* c1l, const void*
         if ((rc = make_map_plane(&maps.a[2 * pl], (const __half*)c1h + pl * plane_elems, B, TH, C))) return rc;
         if ((rc = make_map_plane(&maps.a[2 * pl + 1], (const __half*)c1l + pl * plane_elems, B, TH, C))) return rc;
     }
-    const bool pair = pair_enabled(tc_flags(), 9 * C, 0, true) && T2 > CONV_TR;
+    const bool pair = pair_enabled(T2 > CONV_TR);
     if ((rc = make_map_2d(&maps.w[0], Wh, C, 9 * C, 9 * C, pair ? TBN / 2 : TBN))) return rc;
     if ((rc = make_map_2d(&maps.w[1], Wl, C, 9 * C, 9 * C, pair ? TBN / 2 : TBN))) return rc;
     if ((rc = ensure_tc_attrs())) return rc;
     TcParams p{bias, nullptr, out, (__half*)outh, (__half*)outl, 0, C, B * T2 * CONV_W2, C, 9 * C, MASR_EPI_BIAS_RELU, 1.f, T2, tc_flags()};
     const int tiles_n = (C + TBN - 1) / TBN, tiles_t = (T2 + CONV_TR - 1) / CONV_TR;
-    if (pair) {
-        const int ptiles_t = (tiles_t + 1) / 2;
-        launch_pair<true>(maps, p, tiles_n * ptiles_t * B, tiles_n, ptiles_t, (cudaStream_t)stream);
-        return check_launch("tc_gemm_kernel<conv, pair>");
-    }
-    const int num_tiles = tiles_n * tiles_t * B;
-    const int grid = num_tiles < num_sms() ? num_tiles : num_sms();
-    if (p.flags & 4) launch_pdl(tc_gemm_kernel<true, 16, false>, dim3(grid), dim3(tc_threads(16)), kTcSmem, (cudaStream_t)stream, maps, p, num_tiles, tiles_n, tiles_t);
-    else launch_pdl(tc_gemm_kernel<true, 8, false>, dim3(grid), dim3(tc_threads(8)), kTcSmem, (cudaStream_t)stream, maps, p, num_tiles, tiles_n, tiles_t);
+    launch_tc<true>(maps, p, pair, tiles_n, tiles_t, B, (cudaStream_t)stream);
     return check_launch("tc_gemm_kernel<conv>");
 }
 
@@ -1365,21 +1147,13 @@ extern "C" int masr_gemm_tc_f16x2(const void* Ah, const void* Al, int64_t lda, c
     int rc;
     if ((rc = make_map_2d(&maps.a[0], Ah, M, K, lda))) return rc;
     if ((rc = make_map_2d(&maps.a[1], Al, M, K, lda))) return rc;
-    const bool pair = M > TBM && pair_enabled(tc_flags(), K, ((N + TBN - 1) / TBN) * ((M + TBM - 1) / TBM), false);
+    const bool pair = pair_enabled(M > TBM);
     if ((rc = make_map_2d(&maps.w[0], Wh, N, K, K, pair ? TBN / 2 : TBN))) return rc;
     if ((rc = make_map_2d(&maps.w[1], Wl, N, K, K, pair ? TBN / 2 : TBN))) return rc;
     if ((rc = ensure_tc_attrs())) return rc;
     TcParams p{bias, residual, C, (__half*)Ch, (__half*)Cl, ldr, ldc, M, N, K, epilogue, alpha, 0, tc_flags()};
-    if (epilogue == MASR_EPI_RESIDUAL) { p.flags |= preres_flag(residual, ldr, alpha); p.inv_alpha = 1.0f / alpha; }
     const int tiles_n = (N + TBN - 1) / TBN, tiles_m = (M + TBM - 1) / TBM;
-    if (pair) {
-        launch_pair<false>(maps, p, tiles_n * ((tiles_m + 1) / 2), tiles_n, 1, (cudaStream_t)stream);
-        return check_launch("tc_gemm_kernel<pair>");
-    }
-    const int num_tiles = tiles_n * tiles_m;
-    const int grid = num_tiles < num_sms() ? num_tiles : num_sms();
-    if (p.flags & 4) launch_pdl(tc_gemm_kernel<false, 16, false>, dim3(grid), dim3(tc_threads(16)), kTcSmem, (cudaStream_t)stream, maps, p, num_tiles, tiles_n, 1);
-    else launch_pdl(tc_gemm_kernel<false, 8, false>, dim3(grid), dim3(tc_threads(8)), kTcSmem, (cudaStream_t)stream, maps, p, num_tiles, tiles_n, 1);
+    launch_tc<false>(maps, p, pair, tiles_n, tiles_m, 1, (cudaStream_t)stream);
     return check_launch("tc_gemm_kernel");
 }
 
@@ -1388,7 +1162,7 @@ extern "C" int masr_gemm_tc_f16x2(const void* Ah, const void* Al, int64_t lda, c
 //   :153 / :106 -> positionwise.py:37 (norm_ff / norm_ff_macaron -> w_1 + SiLU)
 // Every CTA (pair) takes a contiguous range of tiles, normalises the <= 2 row blocks that range touches into the operand
 // pair buffer (Ah, Al: [M, 256] fp16, written here, same values as masr_layernorm_split_f16) and then runs the GEMM on it.
-// Replaces masr_layernorm_split_f16 + masr_gemm_tc_f16x2: one launch and its ~5 us of fill / drain less per LayerNorm.
+// Replaces masr_layernorm_split_f16 + masr_gemm_tc_f16x2: one launch and its fill / drain less per LayerNorm.
 extern "C" int masr_gemm_tc_lnpre_f16x2(const float* x, int64_t ldx, const float* gamma, const float* beta, float eps, void* Ah,
                                         void* Al, int64_t lda, const void* Wh, const void* Wl, const float* bias, float* C,
                                         void* Ch, void* Cl, int64_t ldc, int M, int N, int K, int epilogue, float alpha,
@@ -1403,27 +1177,20 @@ extern "C" int masr_gemm_tc_lnpre_f16x2(const float* x, int64_t ldx, const float
     MASR_REQUIRE(epilogue >= MASR_EPI_BIAS && epilogue <= MASR_EPI_BIAS_SCALE, "masr_gemm_tc_lnpre_f16x2: bad epilogue %d", epilogue);
     MASR_REQUIRE(epilogue != MASR_EPI_BIAS_GLU || N % 32 == 0, "masr_gemm_tc_lnpre_f16x2: GLU epilogue needs N %% 32 == 0");
     MASR_REQUIRE(ldc % 8 == 0 || (C && !Ch && ldc % 4 == 0), "masr_gemm_tc_lnpre_f16x2: ldc=%lld alignment", (long long)ldc);
-    MASR_REQUIRE(tc_flags() & 4, "masr_gemm_tc_lnpre_f16x2: needs the 16-epilogue-warp kernel (MASR_TC_FLAGS bit 2)");
     TcMaps maps;
     memset(&maps, 0, sizeof(maps));
     int rc;
     const int tiles_n = (N + TBN - 1) / TBN, tiles_m = (M + TBM - 1) / TBM;
-    const bool pair = M > TBM && pair_enabled(tc_flags(), K, tiles_n * tiles_m, false);
     if ((rc = make_map_2d(&maps.a[0], Ah, M, K, lda))) return rc;
     if ((rc = make_map_2d(&maps.a[1], Al, M, K, lda))) return rc;
+    const bool pair = pair_enabled(M > TBM);
     if ((rc = make_map_2d(&maps.w[0], Wh, N, K, K, pair ? TBN / 2 : TBN))) return rc;
     if ((rc = make_map_2d(&maps.w[1], Wl, N, K, K, pair ? TBN / 2 : TBN))) return rc;
     if ((rc = ensure_tc_attrs())) return rc;
     TcParams p{bias, nullptr, C, (__half*)Ch, (__half*)Cl, 0, ldc, M, N, K, epilogue, alpha, 0, tc_flags()};
     p.ln_g = gamma; p.ln_b = beta; p.ln_eps = eps;
     p.lnp_x = x; p.lnp_ldx = ldx; p.lnp_ld = lda; p.lnp_h = (__half*)Ah; p.lnp_l = (__half*)Al;
-    if (pair) {
-        launch_pair<false>(maps, p, tiles_n * ((tiles_m + 1) / 2), tiles_n, 1, (cudaStream_t)stream);
-        return check_launch("tc_gemm_kernel<pair, ln prologue>");
-    }
-    const int num_tiles = tiles_n * tiles_m;
-    const int grid = num_tiles < num_sms() ? num_tiles : num_sms();
-    launch_pdl(tc_gemm_kernel<false, 16, false>, dim3(grid), dim3(tc_threads(16)), kTcSmem, (cudaStream_t)stream, maps, p, num_tiles, tiles_n, 1);
+    launch_tc<false>(maps, p, pair, tiles_n, tiles_m, 1, (cudaStream_t)stream);
     return check_launch("tc_gemm_kernel<ln prologue>");
 }
 
@@ -1444,7 +1211,7 @@ extern "C" int masr_ctc_head_argmax_tc_f16x2(const void* Ah, const void* Al, int
     int rc;
     if ((rc = make_map_2d(&maps.a[0], Ah, M, K, lda))) return rc;
     if ((rc = make_map_2d(&maps.a[1], Al, M, K, lda))) return rc;
-    const bool pair = M > TBM && pair_enabled(4, K, ((V + TBN - 1) / TBN) * ((M + TBM - 1) / TBM), false);
+    const bool pair = pair_enabled(M > TBM);
     if ((rc = make_map_2d(&maps.w[0], Wh, V, K, K, pair ? TBN / 2 : TBN))) return rc;
     if ((rc = make_map_2d(&maps.w[1], Wl, V, K, K, pair ? TBN / 2 : TBN))) return rc;
     if ((rc = ensure_tc_attrs())) return rc;
@@ -1453,10 +1220,7 @@ extern "C" int masr_ctc_head_argmax_tc_f16x2(const void* Ah, const void* Al, int
     p.part_s = p.part_m + (int64_t)groups * M;
     p.part_i = (int*)(p.part_s + (int64_t)groups * M);
     const int tiles_n = (V + TBN - 1) / TBN, tiles_m = (M + TBM - 1) / TBM;
-    const int num_tiles = tiles_n * tiles_m;
-    const int grid = num_tiles < num_sms() ? num_tiles : num_sms();
-    if (pair) launch_pair<false>(maps, p, tiles_n * ((tiles_m + 1) / 2), tiles_n, 1, (cudaStream_t)stream);
-    else launch_pdl(tc_gemm_kernel<false, 16, false>, dim3(grid), dim3(tc_threads(16)), kTcSmem, (cudaStream_t)stream, maps, p, num_tiles, tiles_n, 1);
+    launch_tc<false>(maps, p, pair, tiles_n, tiles_m, 1, (cudaStream_t)stream);
     if ((rc = check_launch("tc_gemm_kernel<ctc>"))) return rc;
     launch_pdl(ctc_partial_combine_kernel, dim3((M + 31) / 32), dim3(128), 0, (cudaStream_t)stream, (const float*)p.part_m,
                (const float*)p.part_s, (const int*)p.part_i, M, groups, ids, maxp);
@@ -1519,14 +1283,13 @@ static int launch_residual_ln(const void* Ah, const void* Al, int64_t lda, const
                epi_override ? epi_override : (gamma2 ? EPI_RESIDUAL_LN2 : EPI_RESIDUAL_LN), alpha, 0, tc_flags() & ~2};
     p.ln_g = gamma1; p.ln_b = beta1; p.ln_g2 = gamma2; p.ln_b2 = beta2; p.y2 = Y2; p.ln_eps = eps;
     p.ada_s = ada_s; p.ada_b = ada_b;
-    p.flags |= preres_flag(residual, ldr, alpha); p.inv_alpha = 1.0f / alpha;
     const int tiles_m = (M + TBM - 1) / TBM;
     const int num_tiles = 2 * tiles_m;
     const int sms = num_sms() & ~1;
     const int grid = num_tiles < sms ? num_tiles : sms;             // even: a cluster = the two column tiles of one row block
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(tc_threads(16));
+    cfg.blockDim = dim3(TC_THREADS);
     cfg.dynamicSmemBytes = kTcSmemLn;
     cfg.stream = (cudaStream_t)stream;
     cudaLaunchAttribute attr[2];
@@ -1536,6 +1299,6 @@ static int launch_residual_ln(const void* Ah, const void* Al, int64_t lda, const
     attr[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    cudaLaunchKernelEx(&cfg, tc_gemm_kernel<false, 16, true>, maps, p, num_tiles, 2, 1);
+    cudaLaunchKernelEx(&cfg, tc_gemm_kernel<false, true>, maps, p, num_tiles, 2, 1);
     return check_launch("tc_gemm_kernel<ln>");
 }

@@ -1,4 +1,4 @@
-"""Device engine: drives the sm_100a kernels of ``libmasr_b200.so`` over packed weights.
+"""Device engine: drives the sm_90a kernels of ``libmasr_b200.so`` over packed weights.
 
 This is the object that replaces the reference's ``InferencePredictor`` + TorchScript module
 (masr/infer_utils/inference_predictor.py:10-102, masr/model_utils/conformer/model.py:152-190) and
@@ -59,22 +59,22 @@ class GreedyResult:
 
 
 class ConformerEngine:
-    """Conformer (configs/conformer.yml) inference on one B200."""
+    """Conformer (configs/conformer.yml) inference on one H100."""
 
     def __init__(self, weights_src, streaming: bool = True, device: str = "cuda", max_len: int = 5000,
                  gemm: str = "tc", use_graphs: bool = True):
-        """``gemm``: "tc" = tcgen05 FP16x2-split tensor-core GEMMs (fp32-grade results, csrc/tc_gemm.cu) for the
+        """``gemm``: "tc" = wgmma FP16x2-split tensor-core GEMMs (fp32-grade results, csrc/tc_gemm.cu) for the
         batched path; "simt" = the fp32 FMA-pipe GEMMs (csrc/gemm.cu).  The single-stream chunk path always uses
         the fp32 kernels (16-row problems are launch-bound, not math-bound)."""
         if gemm not in ("tc", "simt"):
             raise ValueError("gemm must be 'tc' or 'simt'")
         self.gemm_path = gemm
         # fused epilogues of the tensor-core path.  CTC head (softmax partials + argmax in the GEMM epilogue, no [M,V] logits):
-        # on (MASR_FUSE_CTC=0 for A/B runs).  LayerNorm behind the residual projections (cluster of 2 CTAs + DSMEM): measured
-        # r02 NOT faster than the separate LayerNorm launch — with one tile per CTA the longer epilogue is fully exposed
-        # (w_2 34.3 -> 42.6 us vs 6.0 us for the LayerNorm kernel, profiles/r02_ln_fusion.md) — so off unless MASR_FUSE_LN=1.
+        # on (MASR_FUSE_CTC=0 for A/B runs).  LayerNorm behind the residual projections (cluster of 2 CTAs + DSMEM): with one
+        # tile per CTA the longer epilogue is fully exposed instead of overlapping the next tile's mainloop; off unless
+        # MASR_FUSE_LN=1 (not measured faster on the H100).
         self.fuse_ctc = os.environ.get("MASR_FUSE_CTC", "1") != "0"
-        # attention of utterances up to 256 frames on tcgen05 (csrc/attention_tc5.cu); MASR_ATTN=mma keeps the mma.sync kernel
+        # attention of utterances up to 256 frames on wgmma (csrc/attention_tc5.cu); MASR_ATTN=mma keeps the mma.sync kernel
         self.attn_tc5 = os.environ.get("MASR_ATTN", "tc5") != "mma"
         self.fuse = os.environ.get("MASR_FUSE_LN", "0") == "1"
         # LayerNorm as a PROLOGUE of the GEMM that consumes it (masr_gemm_tc_lnpre_f16x2: norm_mha -> qkv, norm_conv -> pw1,
@@ -83,7 +83,7 @@ class ConformerEngine:
         self.use_graphs = bool(use_graphs)     # replay the batched device step as one CUDA graph per (B, Fmax) shape
         self._graphs = {}
         if not torch.cuda.is_available():
-            raise _lib.MasrB200Error("masr_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise _lib.MasrB200Error("masr_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.lib = _lib.load()
         dev = torch.device(device)
         if dev.index is None:
@@ -152,7 +152,7 @@ class ConformerEngine:
         d = self.d
         ph, pl, _ = self._ptab_pair(L)
         if T <= 256 and self.dk == 64 and self.attn_tc5:
-            # tcgen05 / TMEM / TMA kernel, one CTA per (utterance, head): utterances of up to 256 frames (10 s audio: T = 248)
+            # wgmma / TMA kernel, one CTA per (utterance, head): utterances of up to 256 frames (10 s audio: T = 248)
             self._k("attention", "masr_relpos_attention_tc5", _p(qkv), 3 * d, T, qkvp[0].data_ptr() + 2 * d, qkvp[1].data_ptr() + 2 * d,
                     qkvp[0].data_ptr() + 4 * d, qkvp[1].data_ptr() + 4 * d, 3 * d, T, _p(ph), _p(pl), d, ph.shape[0], _p(L.pos_u),
                     _p(L.pos_v), None, _p(outp[0]), _p(outp[1]), d, T, _p(lens), _p(lens), B, self.h, self.dk, T)
@@ -466,7 +466,7 @@ class ConformerEngine:
         return t0[:M], tl, T, ws
 
     def _encode_tc(self, feats, ws, tl, tlens, B, Fmax, F1, T, M):
-        """Same layer program as ``encode`` with every dense contraction on tcgen05 (FP16x2 split): GEMM inputs
+        """Same layer program as ``encode`` with every dense contraction on wgmma (FP16x2 split): GEMM inputs
         travel as fp16 (h,l) pairs written by the producing kernel's epilogue, the residual stream stays fp32."""
         w, d, tw = self.w, self.d, self._tcw
         x, g, qkv = ws["x"], ws["g"], ws["qkv"]
@@ -614,7 +614,7 @@ class ConformerEngine:
     def transcribe_beam_pipelined(self, batches, beam_size: int = 300, cutoff_prob: float = 0.99, cutoff_top_n: int = 40,
                                   use_db_normalization: bool = True, target_db: float = -20.0):
         """Generator over ``batches`` (iterable of lists of float32 waveforms) yielding ``transcribe_beam(batch)`` per batch, in
-        order, one batch late.  The prefix beam search is one CTA per utterance — 32 of 148 SMs busy for milliseconds — so it
+        order, one batch late.  The prefix beam search is one CTA per utterance — 32 of 132 SMs busy for milliseconds — so it
         runs on a SECOND stream, concurrently with the fbank / encoder / top-k kernels of the next batch on the idle SMs
         (two sets of candidate / trie / output buffers).  Same results as the blocking call."""
         dev = self.device
@@ -857,7 +857,7 @@ class ConformerEngine:
                 item = (slot, B, g["T"], tl, g["ws"]["tokens"].shape[1], True)
             pending.append(item)
             # results are handed out PIPE_DEPTH - 1 batches late: the host runs that far ahead of the GPU, which absorbs host
-            # jitter (with a cross-rank collective in every step any rank's hiccup otherwise stalls all ranks: N=8 e2e, r02)
+            # jitter (with a cross-rank collective in every step any rank's hiccup otherwise stalls all ranks)
             while len(pending) >= self.PIPE_DEPTH:
                 yield finish(pending.popleft())
         while pending:

@@ -1,4 +1,4 @@
-"""Batched evaluation over a manifest on the B200 path (SURVEY.md §8 f1): the decode + error-rate half of
+"""Batched evaluation over a manifest on the H100 path (SURVEY.md §8 f1): the decode + error-rate half of
 ``MASRTrainer.evaluate`` (masr/trainer.py:592-651; the loss half belongs to the training stack and is out of scope).
 
     error_rate, n = evaluate(predictor, read_manifest("dataset/manifest.test"), batch_size=32, metrics_type="cer")

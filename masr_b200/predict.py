@@ -1,4 +1,4 @@
-"""Drop-in for ``masr.predict.MASRPredictor`` (masr/predict.py:19-362) on the B200 engine.
+"""Drop-in for ``masr.predict.MASRPredictor`` (masr/predict.py:19-362) on the H100 engine.
 
 Same constructor arguments, same ``predict`` / ``predict_stream`` / ``reset_stream`` signatures,
 same ``{'text': str, 'score': float}`` results, same YAML keys (``use_model``, ``streaming``,

@@ -50,9 +50,9 @@ class _PoolBase:
         self.feats_in = torch.zeros(n_slots, CHUNK_FRAMES, 80, device=dev, dtype=torch.float32)
         self.lens_host = [0] * n_slots
         self.use_graph = bool(use_graph) and eng.use_graphs
-        # LayerNorm folded into the preceding residual projection (cluster kernel, 4 launches per block fewer): measured r02
-        # SLOWER here too (64 streams: 3.77 vs 3.51-3.59 ms per push, 547 vs 710 launches) — the cluster launch + DSMEM exchange
-        # cost more than the ~2 us LayerNorm launch they replace at M = 1024.  Off unless MASR_POOL_FUSE_LN=1 (tests cover both).
+        # LayerNorm folded into the preceding residual projection (cluster kernel, 4 launches per block fewer): at M = 1024 the
+        # cluster launch + DSMEM exchange replace only a short LayerNorm launch.  Off unless MASR_POOL_FUSE_LN=1 (tests cover
+        # both; not measured faster on the H100).
         import os
         self.fuse_ln = os.environ.get("MASR_POOL_FUSE_LN", "0") == "1" and eng.d == 256
         self._graph = None
@@ -580,7 +580,7 @@ class StreamPool:
         """Incremental ``greedy_decoder_chunk`` (ctc_greedy_decoder.py:70-89) for every slot at once: collapse repeats against
         the previous frame, drop blanks, and keep the score as the reference's left-to-right float32 sum — one vectorised
         float32 add per frame column (16 columns), so each slot's sum sees its terms in order with float32 rounding at
-        every step, exactly like the scalar loop it replaces (which cost ~0.85 ms per push of 64 streams)."""
+        every step, exactly like a scalar per-slot loop."""
         S, C = ids_h.shape
         tout = np.asarray(tout, np.int64)
         if not tout.any():

@@ -13,7 +13,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_100a) device; run with `-m gpu` on the B200 box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_90a) device; run with `-m gpu` on an H100")
     config.addinivalue_line("markers", "reference: needs the read-only reference tree at /root/reference (build container only)")
 
 

@@ -19,7 +19,7 @@ def declared_functions():
 @pytest.fixture(scope="module")
 def lib():
     from masr_b200 import build, _lib
-    build.build()                      # nvcc cross-compiles sm_100a without a GPU
+    build.build()                      # nvcc cross-compiles sm_90a without a GPU
     return _lib.load()
 
 
@@ -56,14 +56,14 @@ def test_abi_version_and_error_string(lib):
     assert isinstance(lib.masr_last_error(), bytes)
 
 
-def test_library_has_sm100a_sass_only():
+def test_library_has_sm90a_sass_only():
     import shutil
     import subprocess
     from masr_b200 import _lib
     if shutil.which("cuobjdump") is None:
         pytest.skip("cuobjdump not on PATH")
     out = subprocess.run(["cuobjdump", "-lelf", _lib.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out and "sm_90" not in out and "sm_80" not in out
+    assert "sm_90a" in out and "sm_100" not in out and "sm_80" not in out
 
 
 def test_product_never_imports_the_oracle():
@@ -105,3 +105,13 @@ def test_unsupported_reference_variants_are_rejected_not_mispacked():
     with pytest.raises(UnsupportedConfig, match="use_gru"):
         check_supported({"encoder.rnns.0.rnn.weight_hh_l0": torch.zeros(3 * 16, 16)}, "deepspeech2")
     check_supported({"encoder.rnns.0.rnn.weight_hh_l0": torch.zeros(4 * 16, 16)}, "deepspeech2")
+
+
+def test_engine_without_cuda_raises_the_library_error(monkeypatch):
+    """No CUDA device: the engine refuses with the package's own error type (there is no CPU fallback)."""
+    import torch
+    from masr_b200 import _lib
+    from masr_b200.engine import ConformerEngine
+    monkeypatch.setattr(torch.cuda, "is_available", lambda: False)
+    with pytest.raises(_lib.MasrB200Error, match="needs a CUDA device"):
+        ConformerEngine({})

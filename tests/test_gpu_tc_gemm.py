@@ -1,4 +1,4 @@
-"""GPU (-m gpu): the tcgen05 FP16x2-split GEMM against a float64 reference, and against the fp32 SIMT
+"""GPU (-m gpu): the wgmma FP16x2-split GEMM against a float64 reference, and against the fp32 SIMT
 GEMM it replaces.  The bar is fp32-grade accuracy (DESIGN.md precision policy)."""
 import math
 
@@ -92,7 +92,7 @@ def test_tc_gemm_fp32_grade(rt, M, N, K):
 
 @pytest.mark.parametrize("B,Fm", [(2, 47), (1, 998), (3, 131)])
 def test_conv_subsampling_tc(rt, B, Fm):
-    """conv1 (parity planes, fp16 pairs) + conv2 (tcgen05 implicit GEMM) against F.conv2d."""
+    """conv1 (parity planes, fp16 pairs) + conv2 (wgmma implicit GEMM) against F.conv2d."""
     g = torch.Generator().manual_seed(Fm)
     idim, C = 80, 256
     feats = torch.randn(B, Fm, idim, generator=g) * 3 + 20
@@ -224,7 +224,7 @@ def test_residual_postln_epilogue(rt, M, K, ada):
 @pytest.mark.parametrize("M,N,K,epi", [(7936, 2048, 256, 1), (7936, 256, 2048, 5), (385, 264, 320, 0), (129, 4233, 256, 0),
                                        (2500, 512, 256, 3), (1000, 256, 4864, 4)])
 def test_pair_kernel_bit_identical_to_single_cta(rt, M, N, K, epi, monkeypatch):
-    """The cta_group::2 form (a 256 x 128 tile per pair of CTAs, MMAs issued by the pair's leader, operands in both CTAs'
+    """The pair form (a 256 x 128 tile per cluster of 2 CTAs, each CTA multicasting half of the W tile into both CTAs'
     shared memory) computes the same products in the same accumulation order as the single-CTA kernel: every output —
     fp32, the fp16 (h, l) pair — must be bit-identical, for full tiles, odd row-block counts and ragged column tiles."""
     g = torch.Generator().manual_seed(7 * M + N + K)
@@ -255,7 +255,7 @@ def test_pair_kernel_bit_identical_to_single_cta(rt, M, N, K, epi, monkeypatch):
 def test_layernorm_prologue_gemm_bit_identical_to_separate_launches(rt, M, N, epi, pair, monkeypatch):
     """masr_gemm_tc_lnpre_f16x2 (every CTA normalises the rows of its own contiguous tile range, then multiplies) against
     masr_layernorm_split_f16 + masr_gemm_tc_f16x2: the operand pair it leaves behind and every output must be bit-identical —
-    single-CTA and cta_group::2 kernels, many tiles per CTA, fewer tiles than CTAs, ragged row blocks and column tiles."""
+    single-CTA and pair kernels, many tiles per CTA, fewer tiles than CTAs, ragged row blocks and column tiles."""
     monkeypatch.setenv("MASR_TC_PAIR", pair)
     K = 256
     g = torch.Generator().manual_seed(M * 3 + N + epi)

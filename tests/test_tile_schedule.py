@@ -1,10 +1,10 @@
 """CPU: the tile schedules of tc_gemm_kernel restated (csrc/tc_gemm.cu: strided for the plain kernels, contiguous ranges for the
-LayerNorm-prologue form; a unit = one CTA or one cta_group::2 pair) — every output tile is computed exactly once, and with the
+LayerNorm-prologue form; a unit = one CTA or one 2-CTA cluster of the pair form) — every output tile is computed exactly once, and with the
 LayerNorm prologue every row block a unit loads was normalised by that same unit (no cross-CTA dependency), at most 2-3 blocks each."""
 import pytest
 
 
-def units_and_tiles(M, N, pair, sms=148):
+def units_and_tiles(M, N, pair, sms=132):
     tiles_n = -(-N // 128)
     tiles_m = -(-M // 128)
     num = tiles_n * (-(-tiles_m // 2) if pair else tiles_m)

@@ -52,9 +52,7 @@ def time_graph(run):
 
 
 M = 7936
-# The pair kernel cannot run without loads: the leader would lap the peer CTA's producer on the empty barriers (in the real
-# kernel it cannot consume a stage before the peer's bytes have landed) and the kernel never ends -> skipped by default.
-skip = set(os.environ.get("PROBE_SKIP", "1no_tma,1neither").split(","))
+skip = set(filter(None, os.environ.get("PROBE_SKIP", "").split(",")))
 shapes = set(sys.argv[1:])
 for name, N, K, epi, want_c, want_p, want_r in (("ffn_w2", 256, 2048, 5, True, False, True), ("embed", 256, 4864, 4, True, False, False),
                                                   ("ffn_w1", 2048, 256, 1, False, True, False), ("qkv", 768, 256, 0, True, True, False)):
@@ -73,14 +71,12 @@ for name, N, K, epi, want_c, want_p, want_r in (("ffn_w2", 256, 2048, 5, True, F
         _lib.call("masr_gemm_tc_f16x2", P(Ah), P(Al), K, P(Wh), P(Wl), P(b), P(R), ldc, P(C), P(Ch), P(Cl), ldc, M, N, K, epi, 0.5, s)
 
     row = {"op": name, "N": N, "K": K}
-    for pair in ("0", "1"):
-        os.environ["MASR_TC_PAIR"] = pair
-        for label, flags in (("full", 5), ("no_tma", 37), ("no_mma", 69), ("neither", 101)):
-            if f"{pair}{label}" in skip:
-                continue
-            os.environ["MASR_TC_FLAGS"] = str(flags)
-            print(f"# {name} pair={pair} {label} ...", flush=True)
-            row[f"pair{pair}_{label}_us"] = round(time_graph(run), 2)
-            print(f"#   {row[f'pair{pair}_{label}_us']} us", flush=True)
-    os.environ["MASR_TC_FLAGS"] = "5"
+    for label, flags in (("full", 1), ("no_tma", 33), ("no_mma", 65), ("neither", 97)):
+        if label in skip:
+            continue
+        os.environ["MASR_TC_FLAGS"] = str(flags)
+        print(f"# {name} {label} ...", flush=True)
+        row[f"{label}_us"] = round(time_graph(run), 2)
+        print(f"#   {row[f'{label}_us']} us", flush=True)
+    os.environ["MASR_TC_FLAGS"] = "1"
     print(json.dumps(row), flush=True)

@@ -1,6 +1,5 @@
 """Dev tool (run under ncu): a handful of masr_gemm_tc_f16x2 launches on the FFN shapes of the headline step
-(M = 7936): w_1 once per MASR_TC_FLAGS value in GP_FLAGS (default 5), then w_2.  `ncu --set full -k regex:tc_gemm -c 4 ...`.
-(r01: GP_FLAGS=5,13 compared the plain kernel with the since-removed A-resident variant, profiles/r01_gemm_prof*.)"""
+(M = 7936): w_1 once per MASR_TC_FLAGS value in GP_FLAGS (default 1), then w_2.  `ncu --set full -k regex:tc_gemm -c 4 ...`."""
 import os
 import sys
 
@@ -42,6 +41,6 @@ def run(N, K, epi, want_c, want_p, want_r, flags, reps=2):
     torch.cuda.synchronize()
 
 
-for fl in os.environ.get("GP_FLAGS", "5").split(","):
+for fl in os.environ.get("GP_FLAGS", "1").split(","):
     run(2048, 256, 1, False, True, False, int(fl))
 run(256, 2048, 5, True, False, True, 5)

@@ -1,5 +1,5 @@
 """Dev tool: compact markdown summary of an `ncu --set full` report (one row per captured launch).
-Usage: python tools/ncu_summary.py profiles/x.ncu-rep > profiles/x_summary.md   (needs the ncu CLI; no GPU)"""
+Usage: python tools/ncu_summary.py x.ncu-rep > x_summary.md   (needs the ncu CLI; no GPU)"""
 import csv
 import io
 import subprocess

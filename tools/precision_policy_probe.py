@@ -13,7 +13,7 @@ and the per-frame CTC argmaxes are compared with the float32 oracle on the bench
 is 0 flips (BASELINE.json: bit-exact greedy ids).  Prints a markdown table: policy, MMA cost relative to all-split
 (weighted by the FLOPs of each call site), flipped argmaxes, max |d posterior|.
 
-    python tools/precision_policy_probe.py [n_utterances] > profiles/r02_precision_policy.md
+    python tools/precision_policy_probe.py [n_utterances] > precision_policy.md
 """
 import os
 import sys

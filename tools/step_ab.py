@@ -2,7 +2,7 @@
 variant) under different kernel-selection environments, INTERLEAVED in one process so that box-to-box and thermal drift
 cancel: every round replays each variant's graph `REPS` times (L2 flushed before every replay, CUDA events), `ROUNDS` rounds.
 Also checks that every variant produces the same token ids.  Variants: name=ENV1:VAL1,ENV2:VAL2 ... on the command line, e.g.
-    python tools/step_ab.py base=MASR_TC_PAIR:0,MASR_TC_FLAGS:5 default= pair_all=MASR_TC_PAIR:1
+    python tools/step_ab.py default= pair=MASR_TC_PAIR:1
 Not a bench value."""
 import json
 import os
@@ -26,7 +26,7 @@ for a in sys.argv[1:]:
     name, _, envs = a.partition("=")
     variants.append((name, dict(kv.split(":") for kv in envs.split(",") if kv)))
 if not variants:
-    variants = [("base", {"MASR_TC_PAIR": "0", "MASR_TC_FLAGS": "5"}), ("default", {})]
+    variants = [("default", {}), ("pair", {"MASR_TC_PAIR": "1"})]
 touched = sorted({k for _, e in variants for k in e})
 
 eng = ConformerEngine(synth.conformer_state_dict(0, 4233), streaming=True)

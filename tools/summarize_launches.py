@@ -1,5 +1,5 @@
-"""Dev tool: turn an `ncu --metrics gpu__time_duration.sum --csv` launch list into the markdown table kept under
-profiles/ (kernel, launches, total us, share).  Usage: python tools/summarize_launches.py launches.csv [title]"""
+"""Dev tool: turn an `ncu --metrics gpu__time_duration.sum --csv` launch list into the markdown table
+(kernel, launches, total us, share).  Usage: python tools/summarize_launches.py launches.csv [title]"""
 import collections
 import csv
 import sys
