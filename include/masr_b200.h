@@ -348,6 +348,74 @@ int masr_ctc_prefix_beam_stream(const int* cand_id, const float* cand_logp, cons
                                 int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int resume, int* out_tok,
                                 int64_t tok_stride, int* out_n, float* out_score, void* stream);
 
+/* ---- character n-gram LM fusion (ARPA) ------------------------------------------------------------------
+ * Replaces the external `Scorer(alpha, beta, model_path, vocabulary)` (masr/decoders/swig_wrapper.py:4-18) that
+ * BeamSearchDecoder builds and queries (beam_search_decoder.py:29-32: is_character_based / get_max_order /
+ * get_dict_size; :47 reset_params(alpha, beta) before every decode) for a CHARACTER-based plain-text ARPA LM.
+ * PARITY UNPINNED (library absent): semantics per oracle/lm.py (DESIGN.md §2).
+ *
+ * The loader is the one part of the library that owns memory: a host handle from masr_lm_load_arpa, released with
+ * masr_lm_free.  Its tables are copied out with masr_lm_export into caller buffers (host), which the caller uploads to
+ * device buffers and points a masr_lm_tables at; the device entry points below take that struct (a host pointer to it). */
+typedef struct masr_lm_tables {
+    const uint32_t* keys;     /* device: 4 words per slot (n word ids, 16 bits each, in words 0..2)            */
+    const float* vals;        /* device: 2 floats per slot: ln p, ln backoff                                    */
+    const int* tok2lm;        /* device [V]: model token id -> LM word id, -1 = not an LM word (or <unk>)       */
+    int order;                /* N, 1..6                                                                        */
+    int bos, eos;             /* LM word ids of <s>, </s>                                                       */
+    int vocab;                /* V                                                                              */
+    int64_t off[8];           /* off[n]: first slot of the order-n table (n = 1..order)                         */
+    int64_t mask[8];          /* mask[n]: slots of the order-n table - 1 (a power of two - 1)                   */
+} masr_lm_tables;
+
+/* info_host[32] layout written by masr_lm_info */
+enum {
+    MASR_LM_INFO_ORDER = 0, MASR_LM_INFO_CHAR_BASED = 1, MASR_LM_INFO_DICT_SIZE = 2, MASR_LM_INFO_VOCAB = 3,
+    MASR_LM_INFO_KEY_WORDS = 4, MASR_LM_INFO_VAL_FLOATS = 5, MASR_LM_INFO_BOS = 6, MASR_LM_INFO_EOS = 7,
+    MASR_LM_INFO_READ = 8,    /* + n - 1: n-grams of order n in the file          */
+    MASR_LM_INFO_KEPT = 14,   /* + n - 1: n-grams of order n kept in the tables   */
+    MASR_LM_INFO_SLOTS = 20,  /* + n - 1: slots of the order-n table              */
+    MASR_LM_INFO_TABLE_BYTES = 26,
+};
+
+/* Parse a plain-text ARPA file (path_host, UTF-8) against the model vocabulary vocab_host (V UTF-8 tokens joined by
+ * '\n'): n-grams containing a word that is neither a model token nor <s> / </s> are dropped (no query reaches them),
+ * `<unk>` counts as out of vocabulary.  Rejects a KenLM binary, a missing \data\ section, count or section mismatches,
+ * a missing <s> or </s>, an order above 6 and malformed lines.  *handle_host receives the handle. */
+int masr_lm_load_arpa(const char* path_host, const char* vocab_host, int V, void** handle_host);
+int masr_lm_info(const void* handle_host, int64_t* info_host);
+/* copy the packed tables (sizes from masr_lm_info) into keys_host / vals_host / tok2lm_host and fill layout_host
+ * (everything but the three pointers, which the caller sets to its device copies) */
+int masr_lm_export(const void* handle_host, uint32_t* keys_host, float* vals_host, int* tok2lm_host,
+                   masr_lm_tables* layout_host);
+int masr_lm_free(void* handle_host);
+
+/* Q queries of lnP(word | window): ctx [Q, order-1] and word [Q] are model token ids, or -1 = <s>, -2 = </s>
+ * (the window oldest first); out [Q].  The lookup the beam search uses, exposed for testing the tables. */
+int masr_lm_score_f32(const masr_lm_tables* lm_host, const int* ctx, const int* word, int Q, float* out, void* stream);
+
+/* masr_ctc_topk_f32 that also writes blank_logp[m] = ln softmax(logits[m])[blank] (whether or not blank is a
+ * candidate): the `std::log(prob[blank_id])` term of the LM search's min_cutoff. */
+int masr_ctc_topk_blank_f32(const float* logits, int64_t ldl, int M, int V, int top_n, float cutoff_prob, int blank,
+                            int* cand_id, float* cand_logp, int* cand_cnt, float* blank_logp, void* stream);
+
+/* masr_ctc_prefix_beam with shallow fusion of the LM (alpha, beta as in the config's ctc_beam_search_decoder_conf):
+ * every extension l -> l+c adds alpha * lnP(c | l) + beta, pairs below min_cutoff are skipped, the beam is ranked by the
+ * fused score (out_score) and out_approx = fused score - len * beta - alpha * lnP(<s>.. tokens </s>) (the reference's
+ * approx_ctc).  Same workspace as masr_ctc_prefix_beam. */
+int masr_ctc_prefix_beam_lm(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
+                            int64_t bstride, const int* lens, int B, int beam_size, int blank, const masr_lm_tables* lm_host,
+                            float alpha, float beta, float* pool, int* trie_parent, int* trie_tok, int64_t trie_cap,
+                            int* out_tok, int64_t tok_stride, int* out_n, float* out_score, float* out_approx, void* stream);
+/* streaming form: as masr_ctc_prefix_beam_stream; the state also carries each beam entry's LM window, so its size
+ * comes from masr_ctc_prefix_beam_lm_state_size */
+int masr_ctc_prefix_beam_lm_state_size(int64_t* ints_per_utt, int64_t* floats_per_utt);
+int masr_ctc_prefix_beam_lm_stream(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
+                                   int64_t bstride, const int* lens, int B, int beam_size, int blank,
+                                   const masr_lm_tables* lm_host, float alpha, float beta, float* pool, int* trie_parent,
+                                   int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int resume, int* out_tok,
+                                   int64_t tok_stride, int* out_n, float* out_score, float* out_approx, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

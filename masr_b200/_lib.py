@@ -18,6 +18,17 @@ STATUS_GAIN_EXCEEDED = 1
 
 _vp, _i, _i64, _f = C.c_void_p, C.c_int, C.c_int64, C.c_float
 
+
+class LmTables(C.Structure):
+    """``masr_lm_tables`` of include/masr_b200.h."""
+    _fields_ = [("keys", _vp), ("vals", _vp), ("tok2lm", _vp), ("order", _i), ("bos", _i), ("eos", _i), ("vocab", _i),
+                ("off", _i64 * 8), ("mask", _i64 * 8)]
+
+
+_lmp = C.POINTER(LmTables)
+LM_INFO_ORDER, LM_INFO_CHAR_BASED, LM_INFO_DICT_SIZE, LM_INFO_VOCAB, LM_INFO_KEY_WORDS, LM_INFO_VAL_FLOATS = range(6)
+LM_INFO_READ, LM_INFO_KEPT, LM_INFO_SLOTS, LM_INFO_TABLE_BYTES = 8, 14, 20, 26
+
 # name -> argtypes, exactly the declarations of include/masr_b200.h
 SIGNATURES = {
     "masr_abi_version": [],
@@ -74,6 +85,17 @@ SIGNATURES = {
     "masr_ctc_prefix_beam_state_size": [C.POINTER(_i64), C.POINTER(_i64)],
     "masr_ctc_prefix_beam_stream": [_vp, _vp, _vp, _i64, _vp, _i, _i, _i, _vp, _vp, _vp, _i64, _vp, _vp, _i, _vp, _i64, _vp, _vp, _vp],
     "masr_ctc_greedy_collapse": [_vp, _vp, _i64, _vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp],
+    "masr_lm_load_arpa": [_vp, _vp, _i, C.POINTER(_vp)],
+    "masr_lm_info": [_vp, C.POINTER(_i64)],
+    "masr_lm_export": [_vp, _vp, _vp, _vp, _lmp],
+    "masr_lm_free": [_vp],
+    "masr_lm_score_f32": [_lmp, _vp, _vp, _i, _vp, _vp],
+    "masr_ctc_topk_blank_f32": [_vp, _i64, _i, _i, _i, _f, _i, _vp, _vp, _vp, _vp, _vp],
+    "masr_ctc_prefix_beam_lm": [_vp, _vp, _vp, _vp, _i64, _vp, _i, _i, _i, _lmp, _f, _f, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _vp,
+                                _vp, _vp],
+    "masr_ctc_prefix_beam_lm_state_size": [C.POINTER(_i64), C.POINTER(_i64)],
+    "masr_ctc_prefix_beam_lm_stream": [_vp, _vp, _vp, _vp, _i64, _vp, _i, _i, _i, _lmp, _f, _f, _vp, _vp, _vp, _i64, _vp, _vp, _i,
+                                       _vp, _i64, _vp, _vp, _vp, _vp],
 }
 
 

@@ -15,7 +15,10 @@
 //                          order) and the result equals the CPU restatement.
 #include <math.h>
 
+#include <type_traits>
+
 #include "common.cuh"
+#include "lm.cuh"
 
 namespace masr {
 
@@ -24,9 +27,12 @@ constexpr int BEAM_CAP = 512;     // beam_size cap (reference default 300)
 constexpr int BEAM_THREADS = 512;
 
 // ---------------------------------------------------------------------------------------------------------------
+// BLANK: also write blank_lp[row] = ln softmax[blank] from the same statistics (the LM search's min_cutoff term)
+template <bool BLANK>
 __global__ void __launch_bounds__(256) ctc_topk_kernel(const float* __restrict__ logits, int64_t ldl, int V, int top_n,
                                                        float cutoff_prob, int* __restrict__ cand_id,
-                                                       float* __restrict__ cand_logp, int* __restrict__ cand_cnt) {
+                                                       float* __restrict__ cand_logp, int* __restrict__ cand_cnt, int blank,
+                                                       float* __restrict__ blank_lp) {
     constexpr int PER = 20;                    // 256 * 20 >= 4233 (larger vocabularies take the strided fallback below)
     const int row = blockIdx.x, tid = threadIdx.x;
     const float* x = logits + (int64_t)row * ldl;
@@ -101,6 +107,7 @@ __global__ void __launch_bounds__(256) ctc_topk_kernel(const float* __restrict__
             if (cum >= cutoff_prob) break;
         }
         cand_cnt[row] = n;
+        if constexpr (BLANK) blank_lp[row] = logf(expf(__ldg(x + blank) - mx) / tot);   // == cand_logp when blank is a candidate
     }
 }
 
@@ -166,19 +173,39 @@ struct BeamShared {
     int r_src[BEAM_CAP];
 };
 
+// The LM instantiation: each beam entry carries its LM window (the last N-1 LM word ids, oldest first), so an extension
+// needs no trie walk.
+struct BeamSharedLm : BeamShared {
+    uint16_t ctx[BEAM_CAP][LM_CTX], s_ctx[BEAM_CAP][LM_CTX];
+};
+
+struct LmSearch {
+    masr_lm_tables lm;
+    const float* blank_lp;                       // ln p_blank per frame, rows as cand_cnt
+    float alpha, beta;
+    float* out_approx;                           // [B]
+};
+
+constexpr int LM_STATE_INTS = 3 * BEAM_CAP + 2 + BEAM_CAP * LM_CTX / 2;   // + the windows, two ids per int
+
 // pool layout: [0, BEAM_CAP) existing prefixes (rank order), then BEAM_CAP + i*K + k children of (rank i, candidate k);
 // K = this frame's candidate count (usually a handful, cutoff_prob 0.99), so the pool the selection scans is 512 + beam*K
 // entries, not 512 + beam*40
+template <bool LM>
 __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
     const int* __restrict__ cand_id, const float* __restrict__ cand_logp, const int* __restrict__ cand_cnt, int64_t bstride,
     const int* __restrict__ lens, int beam, int blank, float* __restrict__ pool_all, int* __restrict__ trie_parent,
     int* __restrict__ trie_tok, int64_t trie_cap, int* __restrict__ out_tok, int64_t tok_stride, int* __restrict__ out_n,
-    float* __restrict__ out_score, int* __restrict__ state_i, float* __restrict__ state_f, int resume) {
-    // state_i / state_f (optional, per utterance 3*BEAM_CAP+2 ints / 3*BEAM_CAP floats): the beam after the last frame, so the
-    // search can be resumed with the next chunk of frames (`resume` != 0) — CTCBeamSearchDecoder.next()/decode() of the
-    // reference's streaming path (beam_search_decoder.py:75-91); the trie and its hash persist in trie_parent / trie_tok.
+    float* __restrict__ out_score, int* __restrict__ state_i, float* __restrict__ state_f, int resume, const LmSearch lms) {
+    // state_i / state_f (optional, per utterance 3*BEAM_CAP+2 ints / 3*BEAM_CAP floats; LM: LM_STATE_INTS ints): the beam
+    // after the last frame, so the search can be resumed with the next chunk of frames (`resume` != 0) —
+    // CTCBeamSearchDecoder.next()/decode() of the reference's streaming path (beam_search_decoder.py:75-91); the trie and
+    // its hash persist in trie_parent / trie_tok.
+    // LM: shallow fusion per oracle/lm.py — an extension's pool entry is (base + alpha lnP) + beta, and when the beam is
+    // full a (prefix, candidate) pair with lp + score < min_cutoff contributes no transition at all.
+    using Shared = typename std::conditional<LM, BeamSharedLm, BeamShared>::type;
     extern __shared__ __align__(16) uint8_t smem_beam[];
-    BeamShared& S = *reinterpret_cast<BeamShared*>(smem_beam);
+    Shared& S = *reinterpret_cast<Shared*>(smem_beam);
     const int b = blockIdx.x, tid = threadIdx.x;
     const int T = lens[b];
     float* pool = pool_all + (int64_t)b * (BEAM_CAP + BEAM_CAP * BK_MAX);
@@ -190,7 +217,7 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
     const uint32_t hcap = (uint32_t)(trie_cap - node_cap);
     int* thash = tpar + node_cap;
     int nbeam = 1, nnodes = 1;
-    int* st_i = state_i ? state_i + (int64_t)b * (3 * BEAM_CAP + 2) : nullptr;
+    int* st_i = state_i ? state_i + (int64_t)b * (LM ? LM_STATE_INTS : 3 * BEAM_CAP + 2) : nullptr;
     float* st_f = state_f ? state_f + (int64_t)b * (3 * BEAM_CAP) : nullptr;
     if (resume && st_i) {
         nbeam = st_i[3 * BEAM_CAP];
@@ -198,18 +225,35 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
         if (tid < nbeam) {
             S.node[tid] = st_i[tid]; S.par[tid] = st_i[BEAM_CAP + tid]; S.last[tid] = st_i[2 * BEAM_CAP + tid];
             S.pb[tid] = st_f[tid]; S.pnb[tid] = st_f[BEAM_CAP + tid]; S.score[tid] = st_f[2 * BEAM_CAP + tid];
+            if constexpr (LM) {
+                const int* w = st_i + 3 * BEAM_CAP + 2 + tid * (LM_CTX / 2);
+#pragma unroll
+                for (int j = 0; j < LM_CTX / 2; ++j) {
+                    S.ctx[tid][2 * j] = (uint16_t)(w[j] & 0xFFFF);
+                    S.ctx[tid][2 * j + 1] = (uint16_t)((unsigned)w[j] >> 16);
+                }
+            }
         }
     } else {
         for (int64_t i = tid; i < hcap; i += BEAM_THREADS) thash[i] = -1;
         if (tid == 0) {
             S.node[0] = 0; S.par[0] = -1; S.last[0] = -1; S.pb[0] = 0.f; S.pnb[0] = -INFINITY; S.score[0] = 0.f;
             tpar[0] = -1; ttok[0] = -1;
+            if constexpr (LM) {
+#pragma unroll
+                for (int j = 0; j < LM_CTX; ++j) S.ctx[0][j] = (uint16_t)lms.lm.bos;
+            }
         }
     }
     __syncthreads();
     for (int t = 0; t < T; ++t) {
         const int64_t row = (int64_t)b * bstride + t;
         const int K = cand_cnt[row];
+        // min_cutoff (LM only, full beam): (score(worst) + ln p_blank(t)) - max(0, beta); -inf = no cut
+        float cut = -INFINITY;
+        if constexpr (LM) {
+            if (nbeam == beam) cut = __fsub_rn(__fadd_rn(S.score[nbeam - 1], __ldg(lms.blank_lp + row)), fmaxf(0.f, lms.beta));
+        }
         if (tid < K) { S.cid[tid] = cand_id[row * BK_MAX + tid]; S.clp[tid] = cand_logp[row * BK_MAX + tid]; }
         for (int i = tid; i < 2 * BEAM_CAP; i += BEAM_THREADS) S.hkey[i] = -1;
         const int pool_n = BEAM_CAP + nbeam * K;
@@ -222,6 +266,9 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
             S.hval[h] = tid;
             float nb = -INFINITY, nnb = -INFINITY;
             for (int k = 0; k < K; ++k) {
+                if constexpr (LM) {
+                    if (__fadd_rn(S.clp[k], S.score[tid]) < cut) continue;
+                }
                 if (S.cid[k] == blank) nb = logaddexp_f(nb, S.score[tid] + S.clp[k]);
                 else if (S.cid[k] == S.last[tid]) nnb = logaddexp_f(nnb, S.pnb[tid] + S.clp[k]);
             }
@@ -233,9 +280,18 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
             const int i = e / K, k = e - i * K;
             const int c = S.cid[k];
             if (c == blank) continue;
+            if constexpr (LM) {
+                if (__fadd_rn(S.clp[k], S.score[i]) < cut) continue;       // (the pool entry stays -inf)
+            }
             float add;
             if (c == S.last[i]) add = S.pb[i] == -INFINITY ? -INFINITY : S.pb[i] + S.clp[k];
             else add = S.score[i] + S.clp[k];
+            if constexpr (LM) {
+                if (add != -INFINITY) {
+                    const float lnp = lm_lnp(lms.lm, S.ctx[i], lm_word(lms.lm, c));
+                    add = __fadd_rn(__fadd_rn(add, __fmul_rn(lms.alpha, lnp)), lms.beta);
+                }
+            }
             pool[BEAM_CAP + i * K + k] = add;
         }
         __syncthreads();
@@ -374,11 +430,20 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
                 S.s_node[tid] = S.node[src]; S.s_par[tid] = S.par[src]; S.s_last[tid] = S.last[src];
                 S.s_pb[tid] = S.nb[src]; S.s_pnb[tid] = S.nnb[src];
                 S.s_src[tid] = -1;
+                if constexpr (LM) {
+#pragma unroll
+                    for (int j = 0; j < LM_CTX; ++j) S.s_ctx[tid][j] = S.ctx[src][j];
+                }
             } else {                                  // a new child: gets a trie node below
                 const int i = (src - BEAM_CAP) / K, k = (src - BEAM_CAP) - i * K;
                 S.s_node[tid] = -1; S.s_par[tid] = S.node[i]; S.s_last[tid] = S.cid[k];
                 S.s_pb[tid] = -INFINITY; S.s_pnb[tid] = pool[src];
                 S.s_src[tid] = 1;
+                if constexpr (LM) {                   // window of l+c = window of l shifted by one + c
+                    const int n1 = lms.lm.order - 1;
+                    for (int j = 0; j + 1 < n1; ++j) S.s_ctx[tid][j] = S.ctx[i][j + 1];
+                    if (n1 > 0) S.s_ctx[tid][n1 - 1] = lm_word(lms.lm, S.cid[k]);
+                }
             }
         }
         __syncthreads();
@@ -423,6 +488,10 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
         if (tid < n_sel) {
             S.node[tid] = S.s_node[tid]; S.par[tid] = S.s_par[tid]; S.last[tid] = S.s_last[tid];
             S.pb[tid] = S.s_pb[tid]; S.pnb[tid] = S.s_pnb[tid]; S.score[tid] = S.r_score[tid];
+            if constexpr (LM) {
+#pragma unroll
+                for (int j = 0; j < LM_CTX; ++j) S.ctx[tid][j] = S.s_ctx[tid][j];
+            }
         }
         nbeam = n_sel;
         __syncthreads();
@@ -432,6 +501,11 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
         if (tid < nbeam) {
             st_i[tid] = S.node[tid]; st_i[BEAM_CAP + tid] = S.par[tid]; st_i[2 * BEAM_CAP + tid] = S.last[tid];
             st_f[tid] = S.pb[tid]; st_f[BEAM_CAP + tid] = S.pnb[tid]; st_f[2 * BEAM_CAP + tid] = S.score[tid];
+            if constexpr (LM) {
+                int* w = st_i + 3 * BEAM_CAP + 2 + tid * (LM_CTX / 2);
+#pragma unroll
+                for (int j = 0; j < LM_CTX / 2; ++j) w[j] = (int)((unsigned)S.ctx[tid][2 * j] | ((unsigned)S.ctx[tid][2 * j + 1] << 16));
+            }
         }
         if (tid == 0) { st_i[3 * BEAM_CAP] = nbeam; st_i[3 * BEAM_CAP + 1] = nnodes; }
     }
@@ -449,6 +523,28 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
         }
         out_n[b] = n;
         out_score[b] = sc;
+        if constexpr (LM) {
+            // approx_ctc: score - len * beta - alpha * lnP(sentence), sentence = <s>^(N-1) tokens </s> (<s>^N </s> if empty)
+            float apx = sc;
+            if (nbeam > 0) {
+                const masr_lm_tables& lm = lms.lm;
+                const int n1 = lm.order - 1;
+                uint16_t win[LM_CTX];
+#pragma unroll
+                for (int j = 0; j < LM_CTX; ++j) win[j] = (uint16_t)lm.bos;
+                float s = 0.f;
+                if (n == 0) s = lm_lnp(lm, win, (uint32_t)lm.bos);
+                for (int p = 0; p < n; ++p) {
+                    const uint16_t w = lm_word(lm, out_tok[(int64_t)b * tok_stride + p]);
+                    s = __fadd_rn(s, lm_lnp(lm, win, w));
+                    for (int j = 0; j + 1 < n1; ++j) win[j] = win[j + 1];
+                    if (n1 > 0) win[n1 - 1] = w;
+                }
+                s = __fadd_rn(s, lm_lnp(lm, win, (uint32_t)lm.eos));
+                apx = __fsub_rn(__fsub_rn(sc, __fmul_rn((float)n, lms.beta)), __fmul_rn(lms.alpha, s));
+            }
+            lms.out_approx[b] = apx;
+        }
     }
 }
 
@@ -462,8 +558,21 @@ extern "C" int masr_ctc_topk_f32(const float* logits, int64_t ldl, int M, int V,
     MASR_REQUIRE(logits && cand_id && cand_logp && cand_cnt, "masr_ctc_topk_f32: null pointer");
     MASR_REQUIRE(top_n >= 1 && top_n <= BK_MAX, "masr_ctc_topk_f32: cutoff_top_n=%d out of range (1..%d)", top_n, BK_MAX);
     MASR_REQUIRE(V <= 20 * 256, "masr_ctc_topk_f32: vocabulary %d > 5120 not supported by this build", V);
-    ctc_topk_kernel<<<M, 256, 0, (cudaStream_t)stream>>>(logits, ldl, V, top_n, cutoff_prob, cand_id, cand_logp, cand_cnt);
+    ctc_topk_kernel<false><<<M, 256, 0, (cudaStream_t)stream>>>(logits, ldl, V, top_n, cutoff_prob, cand_id, cand_logp, cand_cnt,
+                                                                 0, nullptr);
     return check_launch("ctc_topk_kernel");
+}
+
+extern "C" int masr_ctc_topk_blank_f32(const float* logits, int64_t ldl, int M, int V, int top_n, float cutoff_prob, int blank,
+                                       int* cand_id, float* cand_logp, int* cand_cnt, float* blank_logp, void* stream) {
+    if (M == 0) return MASR_OK;
+    MASR_REQUIRE(logits && cand_id && cand_logp && cand_cnt && blank_logp, "masr_ctc_topk_blank_f32: null pointer");
+    MASR_REQUIRE(top_n >= 1 && top_n <= BK_MAX, "masr_ctc_topk_blank_f32: cutoff_top_n=%d out of range (1..%d)", top_n, BK_MAX);
+    MASR_REQUIRE(V <= 20 * 256, "masr_ctc_topk_blank_f32: vocabulary %d > 5120 not supported by this build", V);
+    MASR_REQUIRE(blank >= 0 && blank < V, "masr_ctc_topk_blank_f32: blank=%d out of range", blank);
+    ctc_topk_kernel<true><<<M, 256, 0, (cudaStream_t)stream>>>(logits, ldl, V, top_n, cutoff_prob, cand_id, cand_logp, cand_cnt,
+                                                                blank, blank_logp);
+    return check_launch("ctc_topk_kernel<blank>");
 }
 
 extern "C" int masr_ctc_prefix_beam_workspace(int B, int Tmax, int64_t* pool_floats, int64_t* trie_ints_per_utt) {
@@ -486,13 +595,13 @@ extern "C" int masr_ctc_prefix_beam(const int* cand_id, const float* cand_logp, 
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) dev = 0;
     if (!attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BeamShared));
+        cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BeamShared));
         if (e != cudaSuccess) { set_last_error("prefix_beam smem attr: %s", cudaGetErrorString(e)); return (int)e; }
         attr_set[dev] = true;
     }
-    prefix_beam_kernel<<<B, BEAM_THREADS, sizeof(BeamShared), (cudaStream_t)stream>>>(
+    prefix_beam_kernel<false><<<B, BEAM_THREADS, sizeof(BeamShared), (cudaStream_t)stream>>>(
         cand_id, cand_logp, cand_cnt, bstride, lens, beam_size, blank, pool, trie_parent, trie_tok, trie_cap, out_tok, tok_stride,
-        out_n, out_score, nullptr, nullptr, 0);
+        out_n, out_score, nullptr, nullptr, 0, LmSearch{});
     return check_launch("prefix_beam_kernel");
 }
 
@@ -516,10 +625,60 @@ extern "C" int masr_ctc_prefix_beam_stream(const int* cand_id, const float* cand
     MASR_REQUIRE(cand_id && cand_logp && cand_cnt && lens && pool && trie_parent && trie_tok && out_tok && out_n && out_score &&
                  state_i && state_f, "masr_ctc_prefix_beam_stream: null pointer");
     MASR_REQUIRE(beam_size >= 1 && beam_size <= BEAM_CAP, "masr_ctc_prefix_beam_stream: beam_size=%d out of range (1..%d)", beam_size, BEAM_CAP);
-    cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BeamShared));
+    cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BeamShared));
     if (e != cudaSuccess) { set_last_error("prefix_beam smem attr: %s", cudaGetErrorString(e)); return (int)e; }
-    prefix_beam_kernel<<<B, BEAM_THREADS, sizeof(BeamShared), (cudaStream_t)stream>>>(
+    prefix_beam_kernel<false><<<B, BEAM_THREADS, sizeof(BeamShared), (cudaStream_t)stream>>>(
         cand_id, cand_logp, cand_cnt, bstride, lens, beam_size, blank, pool, trie_parent, trie_tok, trie_cap, out_tok, tok_stride,
-        out_n, out_score, state_i, state_f, resume);
+        out_n, out_score, state_i, state_f, resume, LmSearch{});
     return check_launch("prefix_beam_kernel<stream>");
+}
+
+// ---- with the LM (BeamSearchDecoder with its Scorer: beam_search_decoder.py:29-32,47-56) ----
+static int launch_beam_lm(const char* what, const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
+                          int64_t bstride, const int* lens, int B, int beam_size, int blank, const masr_lm_tables* lm, float alpha,
+                          float beta, float* pool, int* trie_parent, int* trie_tok, int64_t trie_cap, int* state_i, float* state_f,
+                          int resume, int* out_tok, int64_t tok_stride, int* out_n, float* out_score, float* out_approx,
+                          cudaStream_t stream) {
+    MASR_REQUIRE(cand_id && cand_logp && cand_cnt && blank_logp && lens && pool && trie_parent && trie_tok && out_tok && out_n &&
+                 out_score && out_approx && lm, "%s: null pointer", what);
+    MASR_REQUIRE(lm->keys && lm->vals && lm->tok2lm, "%s: LM tables not set", what);
+    MASR_REQUIRE(lm->order >= 1 && lm->order <= LM_MAX_ORDER, "%s: LM order %d out of range (1..%d)", what, lm->order, LM_MAX_ORDER);
+    MASR_REQUIRE(beam_size >= 1 && beam_size <= BEAM_CAP, "%s: beam_size=%d out of range (1..%d)", what, beam_size, BEAM_CAP);
+    cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BeamSharedLm));
+    if (e != cudaSuccess) { set_last_error("prefix_beam<lm> smem attr: %s", cudaGetErrorString(e)); return (int)e; }
+    const LmSearch lms{*lm, blank_logp, alpha, beta, out_approx};
+    prefix_beam_kernel<true><<<B, BEAM_THREADS, sizeof(BeamSharedLm), stream>>>(
+        cand_id, cand_logp, cand_cnt, bstride, lens, beam_size, blank, pool, trie_parent, trie_tok, trie_cap, out_tok, tok_stride,
+        out_n, out_score, state_i, state_f, resume, lms);
+    return check_launch(what);
+}
+
+extern "C" int masr_ctc_prefix_beam_lm(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
+                                       int64_t bstride, const int* lens, int B, int beam_size, int blank, const masr_lm_tables* lm_host,
+                                       float alpha, float beta, float* pool, int* trie_parent, int* trie_tok, int64_t trie_cap,
+                                       int* out_tok, int64_t tok_stride, int* out_n, float* out_score, float* out_approx,
+                                       void* stream) {
+    if (B == 0) return MASR_OK;
+    return launch_beam_lm("masr_ctc_prefix_beam_lm", cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size, blank,
+                          lm_host, alpha, beta, pool, trie_parent, trie_tok, trie_cap, nullptr, nullptr, 0, out_tok, tok_stride,
+                          out_n, out_score, out_approx, (cudaStream_t)stream);
+}
+
+extern "C" int masr_ctc_prefix_beam_lm_state_size(int64_t* ints_per_utt, int64_t* floats_per_utt) {
+    MASR_REQUIRE(ints_per_utt && floats_per_utt, "masr_ctc_prefix_beam_lm_state_size: null pointer");
+    *ints_per_utt = LM_STATE_INTS;
+    *floats_per_utt = 3 * BEAM_CAP;
+    return MASR_OK;
+}
+
+extern "C" int masr_ctc_prefix_beam_lm_stream(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
+                                              int64_t bstride, const int* lens, int B, int beam_size, int blank,
+                                              const masr_lm_tables* lm_host, float alpha, float beta, float* pool, int* trie_parent,
+                                              int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int resume, int* out_tok,
+                                              int64_t tok_stride, int* out_n, float* out_score, float* out_approx, void* stream) {
+    if (B == 0) return MASR_OK;
+    MASR_REQUIRE(state_i && state_f, "masr_ctc_prefix_beam_lm_stream: null pointer");
+    return launch_beam_lm("masr_ctc_prefix_beam_lm_stream", cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size,
+                          blank, lm_host, alpha, beta, pool, trie_parent, trie_tok, trie_cap, state_i, state_f, resume, out_tok,
+                          tok_stride, out_n, out_score, out_approx, (cudaStream_t)stream);
 }

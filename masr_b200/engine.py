@@ -564,12 +564,14 @@ class ConformerEngine:
                 _p(ws["tokens"]), ws["tokens"].shape[1], _p(ws["ntok"]), _p(ws["psum"]), _p(ws["pcount"]))
         return probs
 
-    # ---- CTC prefix beam search (no LM) ----------------------------------------------------------
+    # ---- CTC prefix beam search (optionally with a character LM) -------------------------------------
     def ctc_beam(self, enc: torch.Tensor, out_lens: Sequence[int], T: int, ws, beam_size: int = 300,
-                 cutoff_prob: float = 0.99, cutoff_top_n: int = 40):
-        """`ctc_beam_search_decoding(probs, vocab, beam_size, cutoff_prob, cutoff_top_n, None, blank_id=0)` of the reference's
-        external decoder (masr/decoders/swig_wrapper.py:35-64) for a whole batch on the GPU -> device tensors
-        (tokens [B,T], count [B], log-score [B]).  Parity unpinned (DESIGN.md)."""
+                 cutoff_prob: float = 0.99, cutoff_top_n: int = 40, lm=None, alpha: float = 0.0, beta: float = 0.0):
+        """`ctc_beam_search_decoding(probs, vocab, beam_size, cutoff_prob, cutoff_top_n, scorer, blank_id=0)` of the
+        reference's external decoder (masr/decoders/swig_wrapper.py:35-64) for a whole batch on the GPU -> device tensors
+        (tokens [B,T], count [B], log-score [B]).  ``lm`` (a masr_b200.lm.CharLM, or None): shallow fusion with weight
+        ``alpha`` and insertion bonus ``beta``; the log-score is then the reference's approx_ctc (the fused score with the
+        LM terms taken out again; the fused score is in ws["beam_score"]).  Parity unpinned (DESIGN.md)."""
         B = len(out_lens)
         M = B * T
         dev = self.device
@@ -587,6 +589,19 @@ class ConformerEngine:
             ws["beam_tok"] = torch.zeros(B, max(1, T), device=dev, dtype=torch.int32)
             ws["beam_n"] = torch.zeros(B, device=dev, dtype=torch.int32)
             ws["beam_score"] = torch.zeros(B, device=dev, dtype=torch.float32)
+        if lm is not None:
+            if ws.get("blank_lp") is None or ws["blank_lp"].numel() < M:
+                ws["blank_lp"] = torch.empty(M, device=dev, dtype=torch.float32)
+            if ws.get("beam_approx") is None or ws["beam_approx"].numel() < ws["beam_score"].numel():
+                ws["beam_approx"] = torch.zeros_like(ws["beam_score"])
+            self._k("ctc_topk", "masr_ctc_topk_blank_f32", _p(logits), self.Vpad, M, self.V, int(cutoff_top_n), float(cutoff_prob),
+                    0, _p(ws["cand_id"]), _p(ws["cand_lp"]), _p(ws["cand_n"]), _p(ws["blank_lp"]))
+            self._k("prefix_beam", "masr_ctc_prefix_beam_lm", _p(ws["cand_id"]), _p(ws["cand_lp"]), _p(ws["cand_n"]),
+                    _p(ws["blank_lp"]), T, _p(ws["tlens"]), B, int(beam_size), 0, _lib.C.byref(lm.tables(dev)), float(alpha),
+                    float(beta), _p(ws["beam_pool"]), _p(ws["trie_par"]), _p(ws["trie_tok"]), ws["trie_cap"], _p(ws["beam_tok"]),
+                    ws["beam_tok"].shape[1], _p(ws["beam_n"]), _p(ws["beam_score"]), _p(ws["beam_approx"]))
+            self._last_beam = (ws, T, B)
+            return ws["beam_tok"], ws["beam_n"], ws["beam_approx"]
         self._k("ctc_topk", "masr_ctc_topk_f32", _p(logits), self.Vpad, M, self.V, int(cutoff_top_n), float(cutoff_prob),
                 _p(ws["cand_id"]), _p(ws["cand_lp"]), _p(ws["cand_n"]))
         self._k("prefix_beam", "masr_ctc_prefix_beam", _p(ws["cand_id"]), _p(ws["cand_lp"]), _p(ws["cand_n"]), T, _p(ws["tlens"]),
@@ -606,18 +621,22 @@ class ConformerEngine:
         return [[[(int(ids[b, t, k]), np.float32(lp[b, t, k])) for k in range(int(n[b, t]))] for t in range(T)] for b in range(B)]
 
     def transcribe_beam(self, waves: Sequence[np.ndarray], beam_size: int = 300, cutoff_prob: float = 0.99,
-                        cutoff_top_n: int = 40, use_db_normalization: bool = True, target_db: float = -20.0):
-        """Host waveforms -> (token ids per utterance, log-scores) with the GPU prefix beam search."""
+                        cutoff_top_n: int = 40, use_db_normalization: bool = True, target_db: float = -20.0, lm=None,
+                        alpha: float = 0.0, beta: float = 0.0):
+        """Host waveforms -> (token ids per utterance, log-scores) with the GPU prefix beam search (``lm``: see ctc_beam)."""
         feats, frames, status = self.fbank(waves, use_db_normalization, target_db)
-        return self.beam_features(feats, frames, beam_size, cutoff_prob, cutoff_top_n)
+        return self.beam_features(feats, frames, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta)
 
     def transcribe_beam_pipelined(self, batches, beam_size: int = 300, cutoff_prob: float = 0.99, cutoff_top_n: int = 40,
-                                  use_db_normalization: bool = True, target_db: float = -20.0):
+                                  use_db_normalization: bool = True, target_db: float = -20.0, lm=None, alpha: float = 0.0,
+                                  beta: float = 0.0):
         """Generator over ``batches`` (iterable of lists of float32 waveforms) yielding ``transcribe_beam(batch)`` per batch, in
         order, one batch late.  The prefix beam search is one CTA per utterance — 32 of 132 SMs busy for milliseconds — so it
         runs on a SECOND stream, concurrently with the fbank / encoder / top-k kernels of the next batch on the idle SMs
-        (two sets of candidate / trie / output buffers).  Same results as the blocking call."""
+        (two sets of candidate / trie / output buffers; the LM tables are shared read-only).  Same results as the blocking
+        call."""
         dev = self.device
+        lm_t = _lib.C.byref(lm.tables(dev)) if lm is not None else None
         main = torch.cuda.current_stream(dev)
         if getattr(self, "_beam_stream", None) is None:
             self._beam_stream = torch.cuda.Stream(device=dev)
@@ -661,7 +680,8 @@ class ConformerEngine:
                                 tok=torch.zeros(B, max(1, T), device=dev, dtype=i32), n=torch.zeros(B, device=dev, dtype=i32),
                                 sc=torch.zeros(B, device=dev, dtype=f32), tlens=torch.zeros(B, device=dev, dtype=i32),
                                 h_tok=torch.zeros(B, max(1, T), dtype=i32, pin_memory=True), h_n=torch.zeros(B, dtype=i32, pin_memory=True),
-                                h_sc=torch.zeros(B, dtype=f32, pin_memory=True), ready=torch.cuda.Event(), done=torch.cuda.Event())
+                                h_sc=torch.zeros(B, dtype=f32, pin_memory=True), ready=torch.cuda.Event(), done=torch.cuda.Event(),
+                                blank_lp=torch.empty(M, device=dev, dtype=f32), fused=torch.zeros(B, device=dev, dtype=f32))
                 if T == 0:
                     slot["h_n"][:B].zero_()
                     slot["h_sc"][:B].zero_()
@@ -669,15 +689,26 @@ class ConformerEngine:
                     item = (slot, B)
                 else:
                     logits = self.ctc_logits(enc, ws)
-                    self._k("ctc_topk", "masr_ctc_topk_f32", _p(logits), self.Vpad, B * T, self.V, int(cutoff_top_n), float(cutoff_prob),
-                            _p(slot["cand_id"]), _p(slot["cand_lp"]), _p(slot["cand_n"]))
+                    if lm_t is None:
+                        self._k("ctc_topk", "masr_ctc_topk_f32", _p(logits), self.Vpad, B * T, self.V, int(cutoff_top_n),
+                                float(cutoff_prob), _p(slot["cand_id"]), _p(slot["cand_lp"]), _p(slot["cand_n"]))
+                    else:
+                        self._k("ctc_topk", "masr_ctc_topk_blank_f32", _p(logits), self.Vpad, B * T, self.V, int(cutoff_top_n),
+                                float(cutoff_prob), 0, _p(slot["cand_id"]), _p(slot["cand_lp"]), _p(slot["cand_n"]), _p(slot["blank_lp"]))
                     slot["tlens"][:B].copy_(ws["tlens"][:B])
                     slot["ready"].record(main)
                     side.wait_event(slot["ready"])
                     with torch.cuda.stream(side):
-                        self._k("prefix_beam", "masr_ctc_prefix_beam", _p(slot["cand_id"]), _p(slot["cand_lp"]), _p(slot["cand_n"]), T,
-                                _p(slot["tlens"]), B, int(beam_size), 0, _p(slot["pool"]), _p(slot["trie_par"]), _p(slot["trie_tok"]),
-                                slot["trie_cap"], _p(slot["tok"]), slot["tok"].shape[1], _p(slot["n"]), _p(slot["sc"]))
+                        if lm_t is None:
+                            self._k("prefix_beam", "masr_ctc_prefix_beam", _p(slot["cand_id"]), _p(slot["cand_lp"]), _p(slot["cand_n"]), T,
+                                    _p(slot["tlens"]), B, int(beam_size), 0, _p(slot["pool"]), _p(slot["trie_par"]), _p(slot["trie_tok"]),
+                                    slot["trie_cap"], _p(slot["tok"]), slot["tok"].shape[1], _p(slot["n"]), _p(slot["sc"]))
+                        else:                      # the reported score is approx_ctc (see ctc_beam)
+                            self._k("prefix_beam", "masr_ctc_prefix_beam_lm", _p(slot["cand_id"]), _p(slot["cand_lp"]),
+                                    _p(slot["cand_n"]), _p(slot["blank_lp"]), T, _p(slot["tlens"]), B, int(beam_size), 0, lm_t,
+                                    float(alpha), float(beta), _p(slot["pool"]), _p(slot["trie_par"]), _p(slot["trie_tok"]),
+                                    slot["trie_cap"], _p(slot["tok"]), slot["tok"].shape[1], _p(slot["n"]), _p(slot["fused"]),
+                                    _p(slot["sc"]))
                         slot["h_tok"][:B, :slot["tok"].shape[1]].copy_(slot["tok"][:B], non_blocking=True)
                         slot["h_n"][:B].copy_(slot["n"][:B], non_blocking=True)
                         slot["h_sc"][:B].copy_(slot["sc"][:B], non_blocking=True)
@@ -689,12 +720,13 @@ class ConformerEngine:
         if prev is not None:
             yield finish(prev)
 
-    def beam_features(self, feats, frames, beam_size: int = 300, cutoff_prob: float = 0.99, cutoff_top_n: int = 40):
+    def beam_features(self, feats, frames, beam_size: int = 300, cutoff_prob: float = 0.99, cutoff_top_n: int = 40, lm=None,
+                      alpha: float = 0.0, beta: float = 0.0):
         B = feats.shape[0]
         enc, tl, T, ws = self.encode(feats, frames)
         if T == 0:
             return [[] for _ in range(B)], [0.0] * B
-        tok, n, sc = self.ctc_beam(enc, tl, T, ws, beam_size, cutoff_prob, cutoff_top_n)
+        tok, n, sc = self.ctc_beam(enc, tl, T, ws, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta)
         tok, n, sc = tok.cpu().numpy(), n.cpu().numpy(), sc.cpu().numpy()
         self.d2h_bytes += tok.nbytes + n.nbytes + sc.nbytes
         return [tok[b, :n[b]].tolist() for b in range(B)], [float(s) for s in sc]
@@ -1134,16 +1166,19 @@ class StreamBeam:
     """Streaming CTC prefix beam search of ONE stream on the GPU — ``BeamSearchDecoder.decode_chunk / reset_decoder``
     (masr/decoders/beam_search_decoder.py:75-96, called at masr/predict.py:322,353): the beam, the prefix trie and its hash
     stay on the device between chunks (masr_ctc_prefix_beam_stream), so after every chunk the best prefix equals the
-    whole-utterance search over all frames seen so far.  No language model (DESIGN.md: parity unpinned)."""
+    whole-utterance search over all frames seen so far.  ``lm`` / ``alpha`` / ``beta``: shallow fusion of a character LM as
+    in ConformerEngine.ctc_beam (each beam entry's LM window is part of the device state); the score is then approx_ctc.
+    Parity unpinned (DESIGN.md)."""
 
     def __init__(self, eng: "ConformerEngine", beam_size: int = 300, cutoff_prob: float = 0.99, cutoff_top_n: int = 40,
-                 max_frames: int = 3000, max_chunk: int = 64):
+                 max_frames: int = 3000, max_chunk: int = 64, lm=None, alpha: float = 0.0, beta: float = 0.0):
         self.eng, self.beam, self.cutoff, self.top_n = eng, int(beam_size), float(cutoff_prob), int(cutoff_top_n)
         self.max_frames, self.max_chunk = int(max_frames), int(max_chunk)
+        self.lm, self.alpha, self.beta = lm, float(alpha), float(beta)
         dev, C = eng.device, _lib.C
         pool_n, trie_n, si, sf = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_int64(0)
         call("masr_ctc_prefix_beam_workspace", 1, self.max_frames, C.byref(pool_n), C.byref(trie_n))
-        call("masr_ctc_prefix_beam_state_size", C.byref(si), C.byref(sf))
+        call("masr_ctc_prefix_beam_lm_state_size" if lm is not None else "masr_ctc_prefix_beam_state_size", C.byref(si), C.byref(sf))
         i32, f32 = torch.int32, torch.float32
         self.cand_id = torch.empty(self.max_chunk, 40, device=dev, dtype=i32)
         self.cand_lp = torch.empty(self.max_chunk, 40, device=dev, dtype=f32)
@@ -1157,6 +1192,10 @@ class StreamBeam:
         self.lens = torch.zeros(1, device=dev, dtype=i32)
         self.out_tok = torch.zeros(1, self.max_frames, device=dev, dtype=i32)
         self.out = torch.zeros(2, device=dev, dtype=f32)             # [score, count (int32 bits)]
+        if lm is not None:
+            self.blank_lp = torch.empty(self.max_chunk, device=dev, dtype=f32)
+            self.fused = torch.zeros(1, device=dev, dtype=f32)
+            self.lm_t = C.byref(lm.tables(dev))
         self.frames = 0
 
     def reset(self):
@@ -1170,14 +1209,24 @@ class StreamBeam:
             raise ValueError(f"a chunk has at most {self.max_chunk} frames")
         if self.frames + rows > self.max_frames:
             raise AssertionError(f"stream longer than {self.max_frames} frames: create the StreamBeam with a larger max_frames")
-        if rows > 0:
+        lm = self.lm is not None
+        if rows > 0 and lm:
+            eng._k("ctc_topk", "masr_ctc_topk_blank_f32", _p(logits), logits.stride(0), rows, eng.V, self.top_n, self.cutoff, 0,
+                   _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n), _p(self.blank_lp))
+        elif rows > 0:
             eng._k("ctc_topk", "masr_ctc_topk_f32", _p(logits), logits.stride(0), rows, eng.V, self.top_n, self.cutoff,
                    _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n))
         self.lens.fill_(rows)
         n_view = self.out[1:2].view(torch.int32)
-        eng._k("prefix_beam", "masr_ctc_prefix_beam_stream", _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n), self.max_chunk,
-               _p(self.lens), 1, self.beam, 0, _p(self.pool), _p(self.trie_par), _p(self.trie_tok), self.trie_cap, _p(self.state_i),
-               _p(self.state_f), 1 if self.frames else 0, _p(self.out_tok), self.out_tok.shape[1], _p(n_view), _p(self.out[0:1]))
+        if lm:
+            eng._k("prefix_beam", "masr_ctc_prefix_beam_lm_stream", _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n),
+                   _p(self.blank_lp), self.max_chunk, _p(self.lens), 1, self.beam, 0, self.lm_t, self.alpha, self.beta,
+                   _p(self.pool), _p(self.trie_par), _p(self.trie_tok), self.trie_cap, _p(self.state_i), _p(self.state_f),
+                   1 if self.frames else 0, _p(self.out_tok), self.out_tok.shape[1], _p(n_view), _p(self.fused), _p(self.out[0:1]))
+        else:
+            eng._k("prefix_beam", "masr_ctc_prefix_beam_stream", _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n), self.max_chunk,
+                   _p(self.lens), 1, self.beam, 0, _p(self.pool), _p(self.trie_par), _p(self.trie_tok), self.trie_cap, _p(self.state_i),
+                   _p(self.state_f), 1 if self.frames else 0, _p(self.out_tok), self.out_tok.shape[1], _p(n_view), _p(self.out[0:1]))
         self.frames += rows
         oh = self.out.cpu()
         n = int(oh[1:2].view(torch.int32).item())

@@ -95,14 +95,18 @@ class MASRPredictor:
         self._use_db = bool(pc.get('use_dB_normalization', True))
         self._target_db = float(pc.get('target_dB', -20))
         self._beam_conf = None
+        self.lm = None
         if self.configs.decoder == 'ctc_beam_search':
-            # GPU prefix beam search without a language model (the reference's external decoder + KenLM file are not
-            # available; alpha/beta/language_model_path are ignored): whole-utterance calls (engine.ctc_beam) and streaming
-            # (engine.StreamBeam = BeamSearchDecoder.decode_chunk / reset_decoder); both report the beam's log score.
+            # GPU prefix beam search: whole-utterance calls (engine.ctc_beam) and streaming (engine.StreamBeam =
+            # BeamSearchDecoder.decode_chunk / reset_decoder).  With a character-based ARPA file at language_model_path the
+            # LM is fused into the search (the reference's Scorer, beam_search_decoder.py:28-37) and the score is
+            # approx_ctc; otherwise the search runs without LM and reports the beam's log score.
             bc = dict(self.configs.get('ctc_beam_search_decoder_conf', {}) or {})
             self._beam_conf = {'beam_size': int(bc.get('beam_size', 300)), 'cutoff_prob': float(bc.get('cutoff_prob', 0.99)),
                                'cutoff_top_n': int(bc.get('cutoff_top_n', 40))}
-            logger.warning('ctc_beam_search: GPU prefix beam search without LM (alpha/beta ignored)')
+            self.lm = self._load_lm(bc)
+            if self.lm is not None:
+                self._beam_conf.update(lm=self.lm, alpha=float(bc.get('alpha', 0.0)), beta=float(bc.get('beta', 0.0)))
         if not os.path.exists(model_path):
             raise Exception("模型文件不存在，请检查{}是否存在！".format(model_path))
         from .squeezeformer import SqueezeformerEngine
@@ -131,6 +135,26 @@ class MASRPredictor:
         self.reset_stream()
 
     # ---------------------------------------------------------------------------------------------
+    def _load_lm(self, bc):
+        """The CharLM at ``language_model_path`` when that is a character-based ARPA file (judged by content, not by
+        extension), loaded once; else None with a warning that names the reason."""
+        from .lm import CharLM, sniff
+        path = bc.get('language_model_path') or ''
+        kind = sniff(path)
+        reason = {'missing': f'language model {path!r} not found',
+                  'kenlm_binary': f'{path!r} is a KenLM binary; only plain-text ARPA language models are read',
+                  'unknown': f'{path!r} is not an ARPA file'}.get(kind)
+        lm = None
+        if reason is None:
+            lm = CharLM(path, self._text_featurizer.vocab_list)
+            if not lm.is_character_based:
+                reason, lm = f'{path!r} is a word-based LM; only character-based LMs are supported', None
+        if lm is None:
+            logger.warning(f'ctc_beam_search: {reason}: GPU prefix beam search without LM (alpha/beta ignored)')
+            return None
+        logger.info(f'language model: model path = {path}, {lm.describe()}')
+        return lm
+
     def _check_rate(self, sr):
         if sr != self._sample_rate:
             raise Exception(f"masr_b200: resampling is outside the hot-path scope (got {sr} Hz, model expects "

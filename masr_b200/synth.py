@@ -262,6 +262,78 @@ def write_mean_istd(path: str, seed: int = 0, dim: int = 80):
                    "feature_method": "fbank"}, f)
 
 
+def character_lm_arpa(path: str, seed: int = 0, order: int = 3, n_chars: int = 60, n_sentences: int = 400,
+                      max_len: int = 20, vocab_size: int = DEFAULT_VOCAB_SIZE, discount: float = 0.5, branch: int = 4):
+    """Write a character n-gram LM as ARPA with lmplz conventions and return its character list.
+
+    A corpus of ``n_sentences`` sentences is sampled from a random first-order Markov chain over ``n_chars`` characters
+    of the synthetic CJK vocabulary (each character has ``branch`` likely successors); the rest of the vocabulary is left
+    out of the LM, so decoding with it exercises the out-of-vocabulary rule.  The model is a backoff model with absolute discounting D:
+      unigrams  P(w) = (c(w) + 1) / (N + |W|) over W = characters + </s> + <unk>  (<s> is written with log10 p = -99)
+      n >= 2    P(w | h) = (c(h w) - D) / c(h) for seen (h, w); otherwise bo(h) P(w | h[1:]) with
+                bo(h) = (D N1+(h .) / c(h)) / (1 - sum over seen w of P(w | h[1:]))
+    so every P(. | h) sums to 1.  Backoffs are written only on n-grams that prefix a longer one, as lmplz does.
+    Sentences are ``<s> c1 .. cm </s>``."""
+    rng = np.random.default_rng(seed)
+    cjk = vocabulary(vocab_size)[2:-2]
+    assert n_chars < len(cjk)
+    pick = rng.permutation(len(cjk))[:n_chars]
+    chars = [cjk[i] for i in sorted(pick)]
+    succ = rng.integers(0, n_chars, (n_chars, branch))
+    weights = rng.dirichlet(np.ones(branch))
+    sents = []
+    for _ in range(n_sentences):
+        m = int(rng.integers(1, max_len + 1))
+        s = [int(rng.integers(0, n_chars))]
+        for _ in range(m - 1):
+            s.append(int(succ[s[-1], rng.choice(branch, p=weights)]) if rng.random() < 0.85 else int(rng.integers(0, n_chars)))
+        sents.append(["<s>"] + [chars[i] for i in s] + ["</s>"])
+    counts: List[Dict[tuple, int]] = [dict() for _ in range(order + 1)]
+    for s in sents:
+        for n in range(1, order + 1):
+            for i in range(len(s) - n + 1):
+                g = tuple(s[i:i + n])
+                if g[-1] == "<s>":
+                    continue
+                counts[n][g] = counts[n].get(g, 0) + 1
+    words = chars + ["</s>", "<unk>"]
+    N = sum(counts[1].values())
+    prob: List[Dict[tuple, float]] = [dict() for _ in range(order + 1)]
+    for w in words:
+        prob[1][(w,)] = (counts[1].get((w,), 0) + 1) / (N + len(words))
+    ctx_total: List[Dict[tuple, list]] = [dict() for _ in range(order + 1)]   # h -> [c(h), N1+(h .), seen lower mass]
+    for n in range(2, order + 1):
+        for g, c in counts[n].items():
+            e = ctx_total[n - 1].setdefault(g[:-1], [0, 0, 0.0])
+            e[0] += c
+            e[1] += 1
+        for g, c in counts[n].items():
+            h = g[:-1]
+            prob[n][g] = (c - discount) / ctx_total[n - 1][h][0]
+            ctx_total[n - 1][h][2] += prob[n - 1][g[1:]]          # (h[1:], w) is a sub-n-gram, so it is stored
+    backoff: Dict[tuple, float] = {}
+    for n in range(1, order):
+        for h, (ch, n1p, lower) in ctx_total[n].items():
+            backoff[h] = (discount * n1p / ch) / (1.0 - lower)
+    os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
+    grams = [None] + [sorted(prob[n]) for n in range(1, order + 1)]
+    grams[1] = [("<s>",)] + grams[1]
+    with open(path, "w", encoding="utf-8") as f:
+        f.write("\\data\\\n")
+        for n in range(1, order + 1):
+            f.write(f"ngram {n}={len(grams[n])}\n")
+        for n in range(1, order + 1):
+            f.write(f"\n\\{n}-grams:\n")
+            for g in grams[n]:
+                p = -99.0 if g == ("<s>",) else math.log10(prob[n][g])
+                line = f"{p:.8g}\t{' '.join(g)}"
+                if n < order and g in backoff:
+                    line += f"\t{math.log10(backoff[g]):.8g}"
+                f.write(line + "\n")
+        f.write("\n\\end\\\n")
+    return chars
+
+
 def noise_audio(seed: int, num_samples: int, sigma: float = 0.1) -> np.ndarray:
     """BASELINE.md §5 synthetic input: ``0.1 * standard_normal`` float32 (RMS ~ -20 dB)."""
     rng = np.random.default_rng(seed)

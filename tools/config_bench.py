@@ -3,6 +3,8 @@ per-GPU shard of every BASELINE.json config that is not the headline — one JSO
     config 2  conformer.yml streaming=False, 32 x 10 s, ctc_greedy
     config 4  efficient_conformer.yml streaming=False, 32 x 10 s per GPU (256 over 8), ctc_beam_search (no LM)
     config 5  conformer.yml (streaming-trained), 64 utterances of 1-30 s per GPU (512 over 8), ctc_beam_search (no LM)
+    config 4lm / 4plm / 5lm  the same beam-search configs with a synthetic character 5-gram ARPA LM (alpha 2.2, beta 4.3, the
+              shipped configs' values; a few million n-grams, generated into a temporary directory on first use)
     plus      squeezeformer.yml / deepspeech2.yml whole-utterance, 32 x 10 s, ctc_greedy
 Numbers printed here are dev measurements (CUDA-synchronised wall clock around the public engine call), not bench values."""
 import json
@@ -47,6 +49,50 @@ def run(name, eng, waves, fn, reps=5, oracle=None, sample=(0,)):
                       "ids_match_cpu_oracle_on_sample": None if verified is None else {"utterances": list(sample), "ok": verified}}), flush=True)
 
 
+def beam_kernel_ms(name, eng, waves, fn, reps=3):
+    """Event-timed prefix_beam kernel time of one blocking call (the engine's per-kernel profile)."""
+    if only and name.split()[0] not in only:
+        return
+    fn(waves)
+    eng.profile(True)
+    for _ in range(reps):
+        fn(waves)
+    torch.cuda.synchronize()
+    n, ms = eng.profile_summary()["prefix_beam"]
+    eng.profile(False)
+    print(json.dumps({"config": name, "prefix_beam_kernel_ms": ms / reps}), flush=True)
+
+
+_LM = []
+
+
+def big_lm():
+    """The synthetic 5-gram (3000 characters, 200k sentences): loaded once, with its size and host load time printed."""
+    if not _LM:
+        import tempfile
+        from masr_b200.lm import CharLM
+        d = tempfile.mkdtemp(prefix="masr_lm_")
+        p = os.path.join(d, "char5.arpa")
+        t0 = time.perf_counter()
+        synth.character_lm_arpa(p, seed=5, order=5, n_chars=3000, n_sentences=200000)
+        t_gen = time.perf_counter() - t0
+        lm = CharLM(p, synth.vocabulary())
+        print(json.dumps({"lm": "synthetic character 5-gram", "arpa_bytes": os.path.getsize(p), "ngrams": lm.read_counts,
+                          "kept": lm.kept_counts, "table_bytes": lm.table_bytes, "load_cpu_s": lm.load_seconds,
+                          "generate_s": t_gen}), flush=True)
+        os.remove(p)
+        os.rmdir(d)
+        _LM.append(lm)
+    return _LM[0]
+
+
+def want(*names):
+    return not only or bool(only & set(names))
+
+
+LMW = dict(alpha=2.2, beta=4.3)
+
+
 def greedy_oracle(mod, sd, cfg, batched=True):
     from oracle import ctc as octc, fbank as ob
 
@@ -72,6 +118,12 @@ del e
 sdn = synth.efficient_conformer_state_dict(0)
 e = EfficientConformerEngine(sdn, streaming=False)
 run("config4 efficient_conformer.yml streaming=False 32x10s/GPU ctc_beam_search(300,40,0.99,no LM)", e, tens, lambda w: e.transcribe_beam(w, **BEAM))
+beam_kernel_ms("config4 prefix beam kernel, no LM", e, tens, lambda w: e.transcribe_beam(w, **BEAM))
+if want("config4lm", "config4plm"):
+    lm = big_lm()
+    run("config4lm efficient_conformer.yml streaming=False 32x10s/GPU ctc_beam_search(300,40,0.99, char 5-gram LM)", e, tens,
+        lambda w: e.transcribe_beam(w, **BEAM, lm=lm, **LMW))
+    beam_kernel_ms("config4lm prefix beam kernel, char 5-gram LM", e, tens, lambda w: e.transcribe_beam(w, **BEAM, lm=lm, **LMW))
 def piped(w, e_=None):
     return list(e.transcribe_beam_pipelined([w] * 4, **BEAM))[-1]
 
@@ -89,12 +141,29 @@ if not only or "config4p" in only:
     print(json.dumps({"config": "config4p efficient_conformer.yml streaming=False 32x10s/GPU ctc_beam_search, PIPELINED stream of batches (beam search of batch k on a second stream under the encoder of batch k+1)",
                       "utterances": 32, "audio_s": 320.0, "ms_per_batch": dt * 1e3, "audio_seconds_per_second": 320.0 / dt,
                       "equals_blocking_call": bool(same)}), flush=True)
+if want("config4plm"):
+    lm = big_lm()
+    torch.cuda.synchronize(); t0 = time.perf_counter()
+    n_b = 12
+    res = list(e.transcribe_beam_pipelined([tens] * n_b, **BEAM, lm=lm, **LMW))
+    torch.cuda.synchronize(); dt = (time.perf_counter() - t0) / n_b
+    same = res[-1] == e.transcribe_beam(tens, **BEAM, lm=lm, **LMW)
+    assert same
+    print(json.dumps({"config": "config4plm efficient_conformer.yml 32x10s/GPU ctc_beam_search + char 5-gram LM, PIPELINED stream of batches",
+                      "utterances": 32, "audio_s": 320.0, "ms_per_batch": dt * 1e3, "audio_seconds_per_second": 320.0 / dt,
+                      "equals_blocking_call": bool(same)}), flush=True)
 run("config4g efficient_conformer.yml streaming=False 32x10s/GPU ctc_greedy", e, tens, lambda w: e.transcribe(w),
     oracle=greedy_oracle(oe, synth.to_torch(sdn), oe.EfficientConfig(causal=False)), sample=(0, 31))
 del e
 sdn = synth.conformer_state_dict(0)
 e = ConformerEngine(sdn, streaming=True)
 run("config5 conformer.yml streaming-trained 64 x 1-30s/GPU ctc_beam_search(300,40,0.99,no LM)", e, varlen, lambda w: e.transcribe_beam(w, **BEAM), reps=3)
+beam_kernel_ms("config5 prefix beam kernel, no LM", e, varlen, lambda w: e.transcribe_beam(w, **BEAM))
+if want("config5lm"):
+    lm = big_lm()
+    run("config5lm conformer.yml streaming-trained 64 x 1-30s/GPU ctc_beam_search(300,40,0.99, char 5-gram LM)", e, varlen,
+        lambda w: e.transcribe_beam(w, **BEAM, lm=lm, **LMW), reps=3)
+    beam_kernel_ms("config5lm prefix beam kernel, char 5-gram LM", e, varlen, lambda w: e.transcribe_beam(w, **BEAM, lm=lm, **LMW))
 run("config5g conformer.yml streaming-trained 64 x 1-30s/GPU ctc_greedy", e, varlen, lambda w: e.transcribe(w), reps=3,
     oracle=greedy_oracle(oc, synth.to_torch(sdn), oc.ConformerConfig()), sample=(int(np.argmin([len(w) for w in varlen])), 5))
 del e
