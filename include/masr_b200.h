@@ -110,6 +110,16 @@ int masr_gemm_tc_f16x2(const void* Ah, const void* Al, int64_t lda, const void* 
                        const float* bias, const float* residual, int64_t ldr, float* C, void* Ch, void* Cl,
                        int64_t ldc, int M, int N, int K, int epilogue, float alpha, void* stream);
 
+/* Conformer feed-forward module in ONE tensor-core kernel (positionwise.py:37):
+ *   x <- x + alpha * (SiLU(A.W1^T + b1) . W2^T + b2)
+ * A: the LayerNorm-ed [M, D] (h, l) pair (row pitch lda), W1: [F, D] and W2: [D, F] dense pairs, x: the fp32 residual stream
+ * (row pitch ldx), updated in place.  The [M, F] hidden activation stays in shared memory.  D == 256, F % 256 == 0,
+ * lda % 8 == 0, ldx even.  Bit-identical to masr_gemm_tc_f16x2(MASR_EPI_BIAS_SILU -> pair) followed by
+ * masr_gemm_tc_f16x2(MASR_EPI_RESIDUAL, alpha) with residual = C = x. */
+int masr_ffn_tc_f16x2(const void* Ah, const void* Al, int64_t lda, const void* W1h, const void* W1l, const float* b1,
+                      const void* W2h, const void* W2l, const float* b2, float* x, int64_t ldx, int M, int D, int F,
+                      float alpha, void* stream);
+
 /* Sub-layer output projection (N = 256) + residual add + the LayerNorm(s) that follow it, in ONE tensor-core kernel:
  *   x_new = residual + alpha * (A.W^T + bias)
  *   gamma2 == NULL:  X <- x_new,                      (Yh, Yl) <- LN(x_new; gamma1, beta1)

@@ -41,6 +41,7 @@ SIGNATURES = {
     "masr_conv2_s2_relu_f32": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp],
     "masr_gemm_f32": [_vp, _i64, _vp, _vp, _vp, _i64, _vp, _i64, _i, _i, _i, _i, _f, _vp],
     "masr_gemm_tc_f16x2": [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _f, _vp],
+    "masr_ffn_tc_f16x2": [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _f, _vp],
     "masr_gemm_tc_residual_ln_f16x2": [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64,
                                        _i, _i, _i, _f, _vp],
     "masr_gemm_tc_residual_postln_f16x2": [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64,

@@ -183,17 +183,45 @@ class ConformerEngine:
                 _p(x), _p(ln[0]), _p(ln[1]), None if ada is None else _p(ada[0]), None if ada is None else _p(ada[1]),
                 _p(yp[0]), _p(yp[1]), d, M, d, K, 1e-5)
 
+    def _ffn_fused(self) -> bool:
+        """The Conformer FFN modules run as one masr_ffn_tc_f16x2 launch each (shape permitting) unless MASR_FUSE_LN=1,
+        whose w_2 launch carries the following LayerNorm(s) instead."""
+        return self.gemm_path == "tc" and not self.fuse and self.d == 256 and self.w.ffn % 256 == 0
+
+    def _ffn_tc(self, A, W1, b1, W2, b2, M, x, alpha=0.5):
+        """x <- x + alpha * (SiLU(A.W1^T + b1) . W2^T + b2) in one launch (masr_ffn_tc_f16x2), A the LayerNorm-ed pair; the
+        [M, ffn] hidden activation stays on chip.  Bit-identical to the w_1 (EPI_BIAS_SILU -> pair) + w_2 (EPI_RESIDUAL) pair
+        of launches.  Event-timed under the tag "ffn_fused" (profile_summary reports it as ffn_w1 + ffn_w2)."""
+        d = self.d
+        self._k("ffn_fused", "masr_ffn_tc_f16x2", _p(A[0]), _p(A[1]), d, _p(W1[0]), _p(W1[1]), _p(b1), _p(W2[0]), _p(W2[1]),
+                _p(b2), _p(x), d, M, d, self.w.ffn, alpha)
+
+    def _hidp(self, ws):
+        """The [M, ffn] hidden pair of the two-launch FFN form, allocated on first use (the fused FFN does not need it)."""
+        if "hidp" not in ws:
+            Mx, f16 = ws["x"].shape[0], torch.float16
+            ws["hidp"] = (torch.empty(Mx, self.w.ffn, device=self.device, dtype=f16),
+                          torch.empty(Mx, self.w.ffn, device=self.device, dtype=f16))
+        return ws["hidp"]
+
     def time_ffn_gemms(self, ws, M: int, reps: int = 12, iters: int = 5) -> float:
         """Mean milliseconds per FFN GEMM launch (w_1 and w_2 of block 0 alternating, the shapes and epilogues of the step) with
         the launches replayed back to back from a CUDA graph and CUDA events around the replay — i.e. without the per-launch
-        host/launch latency that event pairs around single eager launches include (bench.py's roofline leg)."""
+        host/launch latency that event pairs around single eager launches include (bench.py's roofline leg).
+        With the fused FFN kernel (``_ffn_fused``) the replay is of that kernel, and the result is HALF a fused launch: one
+        fused launch does the work of one w_1 and one w_2 launch, so the FLOPs per "GEMM launch" stay 2 M 256 ffn."""
         w, d, tw, L = self.w, self.d, self._tcw, self.w.layers[0]
-        t0p, hidp = ws["t0p"], ws["hidp"]
+        t0p = ws["t0p"]
         xs = torch.zeros_like(ws["x"])                       # scratch residual stream (the replays keep adding into it)
         dev = self.device
+        fused = self._ffn_fused()
 
         def body():
             for _ in range(reps):
+                if fused:
+                    self._ffn_tc(t0p, tw[0, "ffm1"], L.ffm[1], tw[0, "ffm2"], L.ffm[3], M, xs)
+                    continue
+                hidp = self._hidp(ws)
                 self._tc(t0p, d, tw[0, "ffm1"], L.ffm[1], M, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn, tag="ffn_w1")
                 self._tc(hidp, w.ffn, tw[0, "ffm2"], L.ffm[3], M, d, w.ffn, EPI_RESIDUAL, 0.5, xs, d, C=xs, ldc=d, tag="ffn_w2")
 
@@ -218,7 +246,7 @@ class ConformerEngine:
             e1.synchronize()
             best = min(best, e0.elapsed_time(e1))
         self.launches, self.prof = n0, prof
-        return best / (2 * reps)
+        return best / (2 * reps)           # fused: reps launches, each counted as a w_1 + w_2 pair
 
     def _ln_tc(self, x, gb, yp, W, bias, M, N, epi=EPI_BIAS, C=None, Cp=None, ldc=0, tag="gemm"):
         """C / Cp = epi(LN(x; gb) . W^T + bias) with yp as the operand pair: one launch (masr_gemm_tc_lnpre_f16x2: every CTA
@@ -278,10 +306,17 @@ class ConformerEngine:
         self.prof = {} if enable else None
 
     def profile_summary(self) -> Dict[str, Tuple[int, float]]:
-        """tag -> (launch count, total milliseconds); call after a synchronize."""
+        """tag -> (launch count, total milliseconds); call after a synchronize.
+        A fused FFN launch (tag "ffn_fused") is reported under both "ffn_w1" and "ffn_w2", as one launch with half its time
+        under each: the FFN keeps the two keys (and its share of the step) it had as two launches."""
         out = {}
         for tag, evs in (self.prof or {}).items():
             out[tag] = (len(evs), float(sum(a.elapsed_time(b) for a, b in evs)))
+        fused = out.pop("ffn_fused", None)
+        if fused is not None:
+            for tag in ("ffn_w1", "ffn_w2"):
+                n, ms = out.get(tag, (0, 0.0))
+                out[tag] = (n + fused[0], ms + 0.5 * fused[1])
         return out
 
     def _ln(self, x, gb, y, M, ld=None):
@@ -328,7 +363,6 @@ class ConformerEngine:
             ws["c2p"] = (torch.empty(Mx * self.f2, d, device=dev, dtype=f16), torch.empty(Mx * self.f2, d, device=dev, dtype=f16))
             ws["t0p"] = (torch.empty(Mx, d, device=dev, dtype=f16), torch.empty(Mx, d, device=dev, dtype=f16))
             ws["t1p"] = (torch.empty(Mx, d, device=dev, dtype=f16), torch.empty(Mx, d, device=dev, dtype=f16))
-            ws["hidp"] = (torch.empty(Mx, self.w.ffn, device=dev, dtype=f16), torch.empty(Mx, self.w.ffn, device=dev, dtype=f16))
             ws["qkvp"] = (torch.empty(Mx, 3 * d, device=dev, dtype=f16), torch.empty(Mx, 3 * d, device=dev, dtype=f16))
         if len(self._ws) > 8:
             self._ws.clear()
@@ -470,7 +504,10 @@ class ConformerEngine:
         travel as fp16 (h,l) pairs written by the producing kernel's epilogue, the residual stream stays fp32."""
         w, d, tw = self.w, self.d, self._tcw
         x, g, qkv = ws["x"], ws["g"], ws["qkv"]
-        t0p, t1p, hidp, c1p, c2p = ws["t0p"], ws["t1p"], ws["hidp"], ws["c1p"], ws["c2p"]
+        t0p, t1p, c1p, c2p = ws["t0p"], ws["t1p"], ws["c1p"], ws["c2p"]
+        # the FFN modules: one fused launch each (masr_ffn_tc_f16x2), or w_1 + w_2 through the hidden pair
+        ffn_fused = self._ffn_fused()
+        hidp = None if ffn_fused else self._hidp(ws)
         self._k("conv1", "masr_conv1_cmvn_relu_planes_f16", _p(feats), _p(w.cmvn_mean), _p(w.cmvn_istd), _p(w.conv1_w),
                 _p(w.conv1_b), _p(c1p[0]), _p(c1p[1]), B, Fmax, w.idim, F1, self.w1_cols, d)
         self._k("conv2", "masr_conv2_tc_f16x2", _p(c1p[0]), _p(c1p[1]), _p(tw["conv2"][0]), _p(tw["conv2"][1]),
@@ -481,7 +518,11 @@ class ConformerEngine:
         nl = len(w.layers)
         for i, L in enumerate(w.layers):
             fuse = self.fuse and d == 256
-            if i == 0:                                # later blocks: fused with the previous block's norm_final (below)
+            if ffn_fused:
+                if i == 0:                            # later blocks: t0p is written by the previous block's norm_final (below)
+                    self._ln_split(x, L.ln_ffm, t0p, M)
+                self._ffn_tc(t0p, tw[i, "ffm1"], L.ffm[1], tw[i, "ffm2"], L.ffm[3], M, x)
+            elif i == 0:                              # later blocks: fused with the previous block's norm_final (below)
                 self._ln_tc(x, L.ln_ffm, t0p, tw[i, "ffm1"], L.ffm[1], M, w.ffn, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn, tag="ffn_w1")
             else:
                 self._tc(t0p, d, tw[i, "ffm1"], L.ffm[1], M, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn, tag="ffn_w1")
@@ -489,7 +530,7 @@ class ConformerEngine:
             # operand pair in its epilogue (masr_gemm_tc_residual_ln_f16x2); MASR_FUSE=0: separate LayerNorm launches
             if fuse:
                 self._tc_ln(hidp, w.ffn, tw[i, "ffm2"], L.ffm[3], M, w.ffn, 0.5, x, L.ln_mha, t0p, tag="ffn_w2")
-            else:
+            elif not ffn_fused:
                 self._tc(hidp, w.ffn, tw[i, "ffm2"], L.ffm[3], M, d, w.ffn, EPI_RESIDUAL, 0.5, x, d, C=x, ldc=d, tag="ffn_w2")
             if fuse:
                 self._tc(t0p, d, tw[i, "qkv"], L.bqkv, M, 3 * d, d, C=qkv, Cp=ws["qkvp"], ldc=3 * d, tag="qkv_proj")
@@ -513,6 +554,9 @@ class ConformerEngine:
                 self._tc(t1p, d, tw[i, "pw2"], L.pw2_b, M, d, d, EPI_RESIDUAL, 1.0, x, d, C=x, ldc=d, tag="pw2")
             if fuse:
                 self._tc(t0p, d, tw[i, "ff1"], L.ff[1], M, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn, tag="ffn_w1")
+            elif ffn_fused:
+                self._ln_split(x, L.ln_ff, t0p, M)
+                self._ffn_tc(t0p, tw[i, "ff1"], L.ff[1], tw[i, "ff2"], L.ff[3], M, x)
             else:
                 self._ln_tc(x, L.ln_ff, t0p, tw[i, "ff1"], L.ff[1], M, w.ffn, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn, tag="ffn_w1")
             # x = norm_final(x + 0.5 ffn), then in the same pass the next consumer's LayerNorm: the next block's
@@ -522,7 +566,8 @@ class ConformerEngine:
             if fuse:
                 self._tc_ln(hidp, w.ffn, tw[i, "ff2"], L.ff[3], M, w.ffn, 0.5, x, L.ln_final, t0p, ln2=nxt, y2=y2, tag="ffn_w2")
             else:
-                self._tc(hidp, w.ffn, tw[i, "ff2"], L.ff[3], M, d, w.ffn, EPI_RESIDUAL, 0.5, x, d, C=x, ldc=d, tag="ffn_w2")
+                if not ffn_fused:
+                    self._tc(hidp, w.ffn, tw[i, "ff2"], L.ff[3], M, d, w.ffn, EPI_RESIDUAL, 0.5, x, d, C=x, ldc=d, tag="ffn_w2")
                 self._k("layernorm", "masr_layernorm2_split_f16", _p(x), d, _p(L.ln_final[0]), _p(L.ln_final[1]), _p(x), _p(nxt[0]),
                         _p(nxt[1]), _p(y2), _p(t0p[0]), _p(t0p[1]), d, M, d, 1e-5)
         return ws["t0"][:M], tl, T, ws
@@ -1282,7 +1327,7 @@ class EfficientConformerEngine(ConformerEngine):
     def _encode_tc(self, feats, ws, tl, tlens, B, Fmax, F1, T, M):
         w, d, tw = self.w, self.d, self._tcw
         x, g, qkv = ws["x"], ws["g"], ws["qkv"]
-        t0p, t1p, hidp, c1p, c2p = ws["t0p"], ws["t1p"], ws["hidp"], ws["c1p"], ws["c2p"]
+        t0p, t1p, hidp, c1p, c2p = ws["t0p"], ws["t1p"], self._hidp(ws), ws["c1p"], ws["c2p"]
         T2 = self.final_len(T)
         if "tlens2" not in ws:
             ws["tlens2"] = torch.zeros(B, device=self.device, dtype=torch.int32)

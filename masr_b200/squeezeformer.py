@@ -199,7 +199,7 @@ class SqueezeformerEngine(ConformerEngine):
     def _encode_tc(self, feats, ws, tl, tlens, B, Fmax, F1, T, M):
         w, d, tw = self.w, self.d, self._tcw
         x, g, qkv, y = ws["x"], ws["g"], ws["qkv"], ws["t1"]        # y: pre-LayerNorm sums
-        t0p, t1p, hidp, c1p, c2p = ws["t0p"], ws["t1p"], ws["hidp"], ws["c1p"], ws["c2p"]
+        t0p, t1p, hidp, c1p, c2p = ws["t0p"], ws["t1p"], self._hidp(ws), ws["c1p"], ws["c2p"]
         T2 = (T + 1) // 2
         if "tlens2" not in ws:
             ws["tlens2"] = torch.zeros(B, device=self.device, dtype=torch.int32)
