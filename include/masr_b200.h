@@ -238,7 +238,10 @@ int masr_relpos_attention_tc(const float* Q, int64_t ldq, int64_t q_bstride, con
 /* masr_relpos_attention_tc on the Hopper tensor cores (wgmma, S and O accumulators in registers, K / linear_pos(pe) / V
  * tiles by TMA, V consumed as an MN-major operand, softmax between the two products inside the kernel): one CTA per
  * (utterance, head), for utterances of up to 256 frames — max_q <= 256 and every k_lens[b] <= 256 (the batched whole-utterance
- * path of 10 s audio: T = 248).  Same arguments plus `table_rows` (rows of the P table), same results (fp32-grade). */
+ * path of 10 s audio: T = 248).  Same arguments plus `table_rows` (rows of the P table), same results (fp32-grade).
+ * Supported K / V layout: the K and V matrices hold B * k_bstride rows and every k_lens[b] <= k_bstride — one [B*T, 3d] qkv
+ * buffer with k_bstride = T, or a cache of B slots of k_bstride rows, where any slot (the last included) may hold more keys
+ * than max_q.  The K / V tensor maps end at row B * k_bstride. */
 int masr_relpos_attention_tc5(const float* Q, int64_t ldq, int64_t q_bstride, const void* Kh, const void* Kl, const void* Vh,
                               const void* Vl, int64_t ldk, int64_t k_bstride, const void* Ph, const void* Pl, int64_t ldp,
                               int64_t table_rows, const float* pos_u, const float* pos_v, float* O, void* Oh, void* Ol,

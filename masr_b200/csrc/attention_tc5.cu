@@ -389,8 +389,10 @@ using namespace masr;
 using namespace masr::at5;
 
 // Same arguments and results as masr_relpos_attention_tc, computed with wgmma / TMA.  Restrictions of this kernel:
-// max_q <= 256, every k_lens[b] <= 256, d_k = 64, table_rows >= 1 rows in the linear_pos(pe) table (rows beyond it read as zero and
-// only meet masked keys).  Callers fall back to masr_relpos_attention_tc otherwise.
+// max_q <= 256, every k_lens[b] <= min(256, k_bstride), d_k = 64, and the K / V matrices hold B * k_bstride rows (one
+// [B*T, 3d] qkv buffer with k_bstride = T; a cache of B slots of k_bstride rows): the K / V tensor maps end there, so every
+// slot, the last included, may hold more keys than max_q.  table_rows >= 1 rows in the linear_pos(pe) table.  Rows past
+// either map read as zero and only meet masked keys.  Callers fall back to masr_relpos_attention_tc otherwise.
 extern "C" int masr_relpos_attention_tc5(const float* Q, int64_t ldq, int64_t q_bstride, const void* Kh, const void* Kl,
                                          const void* Vh, const void* Vl, int64_t ldk, int64_t k_bstride, const void* Ph,
                                          const void* Pl, int64_t ldp, int64_t table_rows, const float* pos_u, const float* pos_v,
@@ -401,6 +403,9 @@ extern "C" int masr_relpos_attention_tc5(const float* Q, int64_t ldq, int64_t q_
                  "masr_relpos_attention_tc5: null pointer");
     MASR_REQUIRE(d_k == AT_D, "masr_relpos_attention_tc5: d_k=%d unsupported (this build: 64)", d_k);
     MASR_REQUIRE(max_q <= 2 * AT_ROWS, "masr_relpos_attention_tc5: max_q=%d > 256 (use masr_relpos_attention_tc)", max_q);
+    MASR_REQUIRE(k_bstride >= 1 && table_rows >= 1, "masr_relpos_attention_tc5: k_bstride=%lld table_rows=%lld",
+                 (long long)k_bstride, (long long)table_rows);
+    const int64_t kv_rows = (int64_t)B * k_bstride;                     // rows of the K / V matrices (see the restrictions)
     MASR_REQUIRE(ldq % 4 == 0 && ldk % 8 == 0 && ldp % 8 == 0 && ldo % 8 == 0, "masr_relpos_attention_tc5: leading dimensions misaligned");
     MASR_REQUIRE(((reinterpret_cast<uintptr_t>(Kh) | reinterpret_cast<uintptr_t>(Kl) | reinterpret_cast<uintptr_t>(Vh) |
                    reinterpret_cast<uintptr_t>(Vl) | reinterpret_cast<uintptr_t>(Ph) | reinterpret_cast<uintptr_t>(Pl) |
@@ -408,7 +413,6 @@ extern "C" int masr_relpos_attention_tc5(const float* Q, int64_t ldq, int64_t q_
                  "masr_relpos_attention_tc5: pair pointers must be 16-byte aligned");
     AttnTc5Maps maps;
     memset(&maps, 0, sizeof(maps));
-    const int64_t kv_rows = (int64_t)(B - 1) * k_bstride + max_q;        // rows of the K / V matrices that exist
     int rc;
     if ((rc = make_map(&maps.kh, Kh, kv_rows, (int64_t)H * AT_D, ldk))) return rc;
     if ((rc = make_map(&maps.kl, Kl, kv_rows, (int64_t)H * AT_D, ldk))) return rc;

@@ -25,77 +25,16 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from kernel_contract import P, assert_pair_reconstructs, err, garbage, nan, pair_value, relpos_reference, report, runtime, same
+
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GARBAGE = 1e3
 
 
 @pytest.fixture(scope="module")
 def rt():
-    if not torch.cuda.is_available():
-        pytest.fail("gpu tests need a CUDA device (no CPU fallback exists)")
-    from masr_b200 import _lib
-    _lib.load()
-    _lib.call("masr_check_device")
-
-    class RT:
-        dev = torch.device("cuda", torch.cuda.current_device())
-        call = staticmethod(_lib.call)
-
-        @staticmethod
-        def st():
-            return torch.cuda.current_stream().cuda_stream
-
-    return RT
-
-
-def P(t):
-    # (device copies passed this way are bound to names first: a temporary freed inside one call's argument list can hand
-    # its memory to the next argument's copy)
-    return None if t is None else t.data_ptr()
-
-
-# ---- helpers ---------------------------------------------------------------------------------------------------------------
-
-def garbage(shape, seed):
-    """Finite, large, seeded filler for every row past a valid length."""
-    g = torch.Generator().manual_seed(10_000 + seed)
-    return (torch.rand(shape, generator=g) * 2 - 1) * GARBAGE
-
-
-def nan(shape, device, dtype=torch.float32):
-    return torch.full(shape, float("nan"), dtype=dtype, device=device)
-
-
-def pair_value(h, l):
-    """The fp32-grade value an fp16 (h, l) operand pair stands for."""
-    return h.double().cpu() + l.double().cpu() / 2048.0
-
-
-def assert_pair_reconstructs(h, l, y):
-    """h + l/2048 reproduces the kernel's fp32 result to 2^-21 relative (a tiny floor covers fp16 subnormals)."""
-    y = y.double().cpu()
-    r = pair_value(h, l)
-    assert torch.isfinite(r).all()
-    assert torch.all((r - y).abs() <= 2.0 ** -21 * y.abs() + 1e-10), (r - y).abs().max().item()
-
-
-def same(a, b):
-    """Bit-identical, NaN where the other is NaN (untouched rows of NaN-filled buffers)."""
-    na, nb = torch.isnan(a), torch.isnan(b)
-    return torch.equal(na, nb) and torch.equal(a[~na], b[~nb])
-
-
-def err(out, ref):
-    """max |out - ref|; the kernel output must be finite."""
-    out = out.detach().double().cpu()
-    assert torch.isfinite(out).all(), "non-finite kernel output in a valid row"
-    return (out - ref.double()).abs().max().item() if out.numel() else 0.0
-
-
-def report(name, **errs):
-    print(f"[max error] {name}: " + ", ".join(f"{k}={v:.3g}" for k, v in errs.items()))
+    return runtime()
 
 
 def ceil2(n):
@@ -417,18 +356,24 @@ def test_grouped_attention_cache(rt):
 # ---- relative-position attention at the stream pools' shapes -------------------------------------------------------------
 
 @pytest.mark.parametrize("skew", [False, True])
-@pytest.mark.parametrize("fn", ["masr_relpos_attention_f32", "masr_relpos_attention_tc"])
+@pytest.mark.parametrize("fn", ["masr_relpos_attention_f32", "masr_relpos_attention_tc", "masr_relpos_attention_tc5"])
 def test_relpos_attention_stream_shapes(rt, fn, skew):
     """The stream pools' call (stream_pool.py:207,339,475): q_lens <= 16 < k_lens (16 .. 300, many 32-key tiles); Q in its
-    own [S*C, 3d] buffer; K/V as the pool's cache (pitch 2d, slot pitch cap; fp32 for _f32, fp16 pairs for _tc).  skew:
-    scores with a standard deviation near 10 and, for the first queries of each slot, a dominant key in the LAST key tile
-    (the online-softmax rescale).  Query rows in [q_len, max_q) are written as zeros.
-    Observed max error (H100): f32 1.7e-6 / skewed 9.1e-6, tc 1.1e-6 / skewed 7.7e-6; tolerance 4e-6 / 2e-5 (the
+    own [S*C, 3d] buffer; K/V as the pool's cache (pitch 2d, slot pitch cap; fp32 for _f32, fp16 pairs for _tc / _tc5).
+    skew: scores with a standard deviation near 10 and, for the first queries of each slot, a dominant key in the LAST key
+    tile (the online-softmax rescale).  Query rows in [q_len, max_q) are written as zeros.  _tc5 (keys <= 256) runs the
+    layout its header allows beyond the engine's q_lens == k_lens == max_q: every key set is longer than max_q, and the
+    LAST slot holds the longest one (256 keys), so its K/V rows reach far past (S-1)*cap + max_q.
+    Observed max error (H100): f32 1.7e-6 / skewed 9.1e-6, tc 1.1e-6 / skewed 7.7e-6, tc5 9.2e-7 / skewed 4.2e-6;
+    tolerance 4e-6 / 2e-5 (the
     skewed scores are ~10x larger, and so is their fp32 rounding)."""
     g = torch.Generator().manual_seed(11 + skew)
     S, C, cap, H, dk, d = 6, 16, 320, 4, 64, 256
     q_lens = [16, 16, 16, 1, 9, 0]
     k_lens = [16, 33, 96, 300, 41, 20]
+    if fn == "masr_relpos_attention_tc5":
+        q_lens = [16, 16, 1, 9, 0, 16]
+        k_lens = [17, 33, 96, 41, 20, 256]
     qs = 7.0 if skew else 1.0
     Q = garbage((S, C, 3 * d), 6)
     KV = garbage((S, cap, 2 * d), 7)
@@ -446,29 +391,28 @@ def test_relpos_attention_stream_shapes(rt, fn, skew):
     qld, kld = torch.tensor(q_lens, dtype=torch.int32, device=rt.dev), torch.tensor(k_lens, dtype=torch.int32, device=rt.dev)
     O = nan((S * C, d), rt.dev)
     Oh, Ol = nan((S * C, d), rt.dev, torch.float16), nan((S * C, d), rt.dev, torch.float16)
-    if fn == "masr_relpos_attention_tc":
+    if fn == "masr_relpos_attention_f32":
+        rt.call(fn, P(qd), 3 * d, C, P(kvd), kvd.data_ptr() + 4 * d, 2 * d, cap, P(pd), d, P(ud), P(vd), P(O), P(Oh), P(Ol), d, C,
+                P(qld), P(kld), S, H, dk, C, rt.st())
+    else:
         def split(x):
             h = torch.empty(x.shape, dtype=torch.float16, device=rt.dev); l = torch.empty_like(h)
             rt.call("masr_split_f16", P(x), P(h), P(l), x.numel(), rt.st())
             return h, l
         (kh, kl), (ph, pl) = split(kvd), split(pd)
-        rt.call(fn, P(qd), 3 * d, C, P(kh), P(kl), kh.data_ptr() + 2 * d, kl.data_ptr() + 2 * d, 2 * d, cap, P(ph), P(pl), d,
-                P(ud), P(vd), P(O), P(Oh), P(Ol), d, C, P(qld), P(kld), S, H, dk, C, rt.st())
-    else:
-        rt.call(fn, P(qd), 3 * d, C, P(kvd), kvd.data_ptr() + 4 * d, 2 * d, cap, P(pd), d, P(ud), P(vd), P(O), P(Oh), P(Ol), d, C,
-                P(qld), P(kld), S, H, dk, C, rt.st())
+        if fn == "masr_relpos_attention_tc5":
+            rt.call(fn, P(qd), 3 * d, C, P(kh), P(kl), kh.data_ptr() + 2 * d, kl.data_ptr() + 2 * d, 2 * d, cap, P(ph),
+                    P(pl), d, ptab.shape[0], P(ud), P(vd), P(O), P(Oh), P(Ol), d, C, P(qld), P(kld), S, H, dk, C, rt.st())
+        else:
+            rt.call(fn, P(qd), 3 * d, C, P(kh), P(kl), kh.data_ptr() + 2 * d, kl.data_ptr() + 2 * d, 2 * d, cap, P(ph), P(pl), d,
+                    P(ud), P(vd), P(O), P(Oh), P(Ol), d, C, P(qld), P(kld), S, H, dk, C, rt.st())
     torch.cuda.synchronize()
     O, Oh, Ol = O.cpu().view(S, C, d), Oh.cpu().view(S, C, d), Ol.cpu().view(S, C, d)
     e = 0.0
     for s in range(S):
         n, kl_ = q_lens[s], k_lens[s]
         if n:
-            q = Q[s, :n, :d].double().view(n, H, dk).transpose(0, 1)
-            k = KV[s, :kl_, :d].double().view(kl_, H, dk).transpose(0, 1)
-            v = KV[s, :kl_, d:].double().view(kl_, H, dk).transpose(0, 1)
-            p = ptab[:kl_].double().view(kl_, H, dk).transpose(0, 1)
-            sc = ((q + pu.double()[:, None]) @ k.transpose(1, 2) + (q + pv.double()[:, None]) @ p.transpose(1, 2)) / math.sqrt(dk)
-            ref = (torch.softmax(sc, -1) @ v).transpose(0, 1).reshape(n, d)
+            ref = relpos_reference(Q[s, :n, :d], KV[s, :kl_, :d], KV[s, :kl_, d:], ptab[:kl_], pu, pv, H)
             e = max(e, err(O[s, :n], ref))
             assert_pair_reconstructs(Oh[s, :n], Ol[s, :n], O[s, :n])
         assert torch.all(O[s, n:] == 0) and torch.all(Oh[s, n:] == 0) and torch.all(Ol[s, n:] == 0)

@@ -249,6 +249,46 @@ def test_pair_kernel_bit_identical_to_single_cta(rt, M, N, K, epi, monkeypatch):
     assert torch.isfinite(outs["1"][0][:, :No]).all()
 
 
+@pytest.mark.parametrize("kernel,shape", [("conv2", (2, 998)), ("conv2", (3, 131)), ("ctc_head", (7936, 4233)),
+                                          ("ctc_head", (300, 33))])
+def test_pair_kernel_bit_identical_conv2_and_ctc_head(rt, kernel, shape, monkeypatch):
+    """MASR_TC_PAIR=1 for the other two users of the pair form: masr_conv2_tc_f16x2 (several 6-row time tiles per
+    utterance) and masr_ctc_head_argmax_tc_f16x2 (several row blocks; ids and maxp) give bit-identical outputs."""
+    g = torch.Generator().manual_seed(sum(shape))
+    C = 256
+    if kernel == "conv2":
+        B, Fm = shape
+        F1 = (Fm - 1) // 2
+        T2, TH = (F1 - 1) // 2, (F1 + 1) // 2
+        ph, pl = split(rt, (torch.rand(4 * B * TH * 20 * C, generator=g) * 2).to(rt.dev))
+        wh, wl = split(rt, (torch.randn(C, 9 * C, generator=g) / 48).to(rt.dev))
+        b = torch.randn(C, generator=g).to(rt.dev)
+    else:
+        M, V = shape
+        ah, al = split(rt, torch.randn(M, C, generator=g).to(rt.dev))
+        wh, wl = split(rt, (torch.randn(V, C, generator=g) * (3.0 / math.sqrt(C))).to(rt.dev))
+        b = torch.randn(V, generator=g).to(rt.dev)
+        ws = torch.empty(3 * ((V + 31) // 32) * M * 4, dtype=torch.uint8, device=rt.dev)
+    outs = {}
+    for mode in ("0", "1"):
+        monkeypatch.setenv("MASR_TC_PAIR", mode)
+        if kernel == "conv2":
+            rows = B * T2 * 19
+            o = (torch.full((rows, C), float("nan"), device=rt.dev), torch.full((rows, C), float("nan"), dtype=torch.float16, device=rt.dev),
+                 torch.full((rows, C), float("nan"), dtype=torch.float16, device=rt.dev))
+            rt.call("masr_conv2_tc_f16x2", P(ph), P(pl), P(wh), P(wl), P(b), P(o[0]), P(o[1]), P(o[2]), B, F1, T2, C, rt.st())
+        else:
+            o = (torch.full((M,), -1, dtype=torch.int32, device=rt.dev), torch.full((M,), float("nan"), device=rt.dev))
+            rt.call("masr_ctc_head_argmax_tc_f16x2", P(ah), P(al), C, P(wh), P(wl), P(b), M, V, C, P(ws), ws.numel(), P(o[0]), P(o[1]),
+                    rt.st())
+        torch.cuda.synchronize()
+        outs[mode] = o
+    for a, c in zip(outs["0"], outs["1"]):
+        assert torch.isfinite(a.float()).all()
+        assert torch.equal(a.view(torch.int32 if a.element_size() == 4 else torch.int16),
+                           c.view(torch.int32 if c.element_size() == 4 else torch.int16))
+
+
 @pytest.mark.parametrize("M,N,epi", [(7936, 768, 0), (7936, 2048, 1), (7936, 512, 3), (1000, 768, 0), (129, 2048, 1), (77, 512, 3),
                                      (385, 4233, 0)])
 @pytest.mark.parametrize("pair", ["0", "1"])
