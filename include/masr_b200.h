@@ -429,6 +429,23 @@ int masr_ctc_prefix_beam_lm_stream(const int* cand_id, const float* cand_logp, c
                                    int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int resume, int* out_tok,
                                    int64_t tok_stride, int* out_n, float* out_score, float* out_approx, void* stream);
 
+/* Pool forms of the two streaming searches, for the slots of a stream pool that start and end utterances independently:
+ * as masr_ctc_prefix_beam_stream / masr_ctc_prefix_beam_lm_stream with a device flag per slot, fresh[B], in place of
+ * `resume`.  fresh[b] != 0 starts slot b at the root (the kernel clears the flag once the slot is initialised), else the
+ * slot resumes from its state.  The kernel never clears a slot's hash: whoever marks slot b fresh also sets
+ * trie_parent[b*trie_cap + trie_cap/5, (b+1)*trie_cap) to -1 (the hash is also -1 before the first launch).  A slot with
+ * lens[b] == 0 is not touched at all (state, trie and outputs unchanged).  trie_cap per slot = 5 * (frames * beam_size + 1)
+ * suffices for `frames` frames of that slot (at most beam_size new prefixes per frame). */
+int masr_ctc_prefix_beam_pool(const int* cand_id, const float* cand_logp, const int* cand_cnt, int64_t bstride,
+                              const int* lens, int B, int beam_size, int blank, float* pool, int* trie_parent,
+                              int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int* fresh, int* out_tok,
+                              int64_t tok_stride, int* out_n, float* out_score, void* stream);
+int masr_ctc_prefix_beam_lm_pool(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
+                                 int64_t bstride, const int* lens, int B, int beam_size, int blank,
+                                 const masr_lm_tables* lm_host, float alpha, float beta, float* pool, int* trie_parent,
+                                 int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int* fresh, int* out_tok,
+                                 int64_t tok_stride, int* out_n, float* out_score, float* out_approx, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -97,6 +97,10 @@ SIGNATURES = {
     "masr_ctc_prefix_beam_lm_state_size": [C.POINTER(_i64), C.POINTER(_i64)],
     "masr_ctc_prefix_beam_lm_stream": [_vp, _vp, _vp, _vp, _i64, _vp, _i, _i, _i, _lmp, _f, _f, _vp, _vp, _vp, _i64, _vp, _vp, _i,
                                        _vp, _i64, _vp, _vp, _vp, _vp],
+    "masr_ctc_prefix_beam_pool": [_vp, _vp, _vp, _i64, _vp, _i, _i, _i, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _vp, _vp,
+                                  _vp],
+    "masr_ctc_prefix_beam_lm_pool": [_vp, _vp, _vp, _vp, _i64, _vp, _i, _i, _i, _lmp, _f, _f, _vp, _vp, _vp, _i64, _vp, _vp, _vp,
+                                     _vp, _i64, _vp, _vp, _vp, _vp],
 }
 
 

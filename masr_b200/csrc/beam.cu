@@ -191,23 +191,33 @@ constexpr int LM_STATE_INTS = 3 * BEAM_CAP + 2 + BEAM_CAP * LM_CTX / 2;   // + t
 // pool layout: [0, BEAM_CAP) existing prefixes (rank order), then BEAM_CAP + i*K + k children of (rank i, candidate k);
 // K = this frame's candidate count (usually a handful, cutoff_prob 0.99), so the pool the selection scans is 512 + beam*K
 // entries, not 512 + beam*40
-template <bool LM>
+template <bool LM, bool POOL = false>
 __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
     const int* __restrict__ cand_id, const float* __restrict__ cand_logp, const int* __restrict__ cand_cnt, int64_t bstride,
     const int* __restrict__ lens, int beam, int blank, float* __restrict__ pool_all, int* __restrict__ trie_parent,
     int* __restrict__ trie_tok, int64_t trie_cap, int* __restrict__ out_tok, int64_t tok_stride, int* __restrict__ out_n,
-    float* __restrict__ out_score, int* __restrict__ state_i, float* __restrict__ state_f, int resume, const LmSearch lms) {
+    float* __restrict__ out_score, int* __restrict__ state_i, float* __restrict__ state_f, int resume, const LmSearch lms,
+    int* __restrict__ fresh) {
     // state_i / state_f (optional, per utterance 3*BEAM_CAP+2 ints / 3*BEAM_CAP floats; LM: LM_STATE_INTS ints): the beam
     // after the last frame, so the search can be resumed with the next chunk of frames (`resume` != 0) —
     // CTCBeamSearchDecoder.next()/decode() of the reference's streaming path (beam_search_decoder.py:75-91); the trie and
     // its hash persist in trie_parent / trie_tok.
     // LM: shallow fusion per oracle/lm.py — an extension's pool entry is (base + alpha lnP) + beta, and when the beam is
     // full a (prefix, candidate) pair with lp + score < min_cutoff contributes no transition at all.
+    // POOL (slots of a stream pool that start and end utterances independently; state_i / state_f required): `resume` is
+    // per slot — fresh[b] != 0 starts slot b from the root and is cleared here once the slot is initialised (a replayed CUDA
+    // graph needs no host write), else the slot resumes from its state.  The kernel never clears the hash: the host does
+    // when it marks a slot fresh (one memset of the slot's hash range instead of hcap stores by one CTA, which would hold up
+    // every other slot of the launch).  A slot with no frames this launch (lens[b] == 0) returns at once: its state, trie
+    // and outputs stay byte for byte as they were.
     using Shared = typename std::conditional<LM, BeamSharedLm, BeamShared>::type;
     extern __shared__ __align__(16) uint8_t smem_beam[];
     Shared& S = *reinterpret_cast<Shared*>(smem_beam);
     const int b = blockIdx.x, tid = threadIdx.x;
     const int T = lens[b];
+    if constexpr (POOL) {
+        if (T == 0) return;                                         // (uniform across the CTA)
+    }
     float* pool = pool_all + (int64_t)b * (BEAM_CAP + BEAM_CAP * BK_MAX);
     int* tpar = trie_parent + (int64_t)b * trie_cap;
     int* ttok = trie_tok + (int64_t)b * trie_cap;
@@ -219,7 +229,10 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
     int nbeam = 1, nnodes = 1;
     int* st_i = state_i ? state_i + (int64_t)b * (LM ? LM_STATE_INTS : 3 * BEAM_CAP + 2) : nullptr;
     float* st_f = state_f ? state_f + (int64_t)b * (3 * BEAM_CAP) : nullptr;
-    if (resume && st_i) {
+    bool cont;
+    if constexpr (POOL) cont = fresh[b] == 0;
+    else cont = resume && st_i;
+    if (cont) {
         nbeam = st_i[3 * BEAM_CAP];
         nnodes = st_i[3 * BEAM_CAP + 1];
         if (tid < nbeam) {
@@ -235,7 +248,9 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
             }
         }
     } else {
-        for (int64_t i = tid; i < hcap; i += BEAM_THREADS) thash[i] = -1;
+        if constexpr (!POOL) {
+            for (int64_t i = tid; i < hcap; i += BEAM_THREADS) thash[i] = -1;
+        }
         if (tid == 0) {
             S.node[0] = 0; S.par[0] = -1; S.last[0] = -1; S.pb[0] = 0.f; S.pnb[0] = -INFINITY; S.score[0] = 0.f;
             tpar[0] = -1; ttok[0] = -1;
@@ -246,6 +261,9 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
         }
     }
     __syncthreads();
+    if constexpr (POOL) {
+        if (tid == 0 && !cont) fresh[b] = 0;                       // (every thread has read the flag: after the barrier)
+    }
     for (int t = 0; t < T; ++t) {
         const int64_t row = (int64_t)b * bstride + t;
         const int K = cand_cnt[row];
@@ -601,7 +619,7 @@ extern "C" int masr_ctc_prefix_beam(const int* cand_id, const float* cand_logp, 
     }
     prefix_beam_kernel<false><<<B, BEAM_THREADS, sizeof(BeamShared), (cudaStream_t)stream>>>(
         cand_id, cand_logp, cand_cnt, bstride, lens, beam_size, blank, pool, trie_parent, trie_tok, trie_cap, out_tok, tok_stride,
-        out_n, out_score, nullptr, nullptr, 0, LmSearch{});
+        out_n, out_score, nullptr, nullptr, 0, LmSearch{}, nullptr);
     return check_launch("prefix_beam_kernel");
 }
 
@@ -629,27 +647,71 @@ extern "C" int masr_ctc_prefix_beam_stream(const int* cand_id, const float* cand
     if (e != cudaSuccess) { set_last_error("prefix_beam smem attr: %s", cudaGetErrorString(e)); return (int)e; }
     prefix_beam_kernel<false><<<B, BEAM_THREADS, sizeof(BeamShared), (cudaStream_t)stream>>>(
         cand_id, cand_logp, cand_cnt, bstride, lens, beam_size, blank, pool, trie_parent, trie_tok, trie_cap, out_tok, tok_stride,
-        out_n, out_score, state_i, state_f, resume, LmSearch{});
+        out_n, out_score, state_i, state_f, resume, LmSearch{}, nullptr);
     return check_launch("prefix_beam_kernel<stream>");
 }
 
+// Pool form (a stream pool's slots, each starting and ending utterances on its own): as masr_ctc_prefix_beam_stream with
+// `fresh[b]` (device) in place of `resume`.  fresh[b] != 0 starts slot b at the root and is cleared by the kernel; the caller
+// marks a slot fresh AND resets its hash range [b*trie_cap + trie_cap/5, (b+1)*trie_cap) of trie_parent to -1 (0xFF bytes)
+// before its next launch.  Slots with lens[b] == 0 are left untouched (state, trie and outputs).  Every argument that varies
+// between launches is device data, so the launch can be captured once into a CUDA graph and replayed.
+// The function attribute is set once per device (not while a graph is being captured).
+template <bool LM>
+static int pool_smem_attr() {
+    using Shared = typename std::conditional<LM, BeamSharedLm, BeamShared>::type;
+    static bool done[64] = {};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev < 0 || dev >= 64) dev = 0;
+    if (!done[dev]) {
+        cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<LM, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Shared));
+        if (e != cudaSuccess) { set_last_error("prefix_beam<pool> smem attr: %s", cudaGetErrorString(e)); return (int)e; }
+        done[dev] = true;
+    }
+    return MASR_OK;
+}
+
+extern "C" int masr_ctc_prefix_beam_pool(const int* cand_id, const float* cand_logp, const int* cand_cnt, int64_t bstride,
+                                         const int* lens, int B, int beam_size, int blank, float* pool, int* trie_parent,
+                                         int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int* fresh,
+                                         int* out_tok, int64_t tok_stride, int* out_n, float* out_score, void* stream) {
+    if (B == 0) return MASR_OK;
+    MASR_REQUIRE(cand_id && cand_logp && cand_cnt && lens && pool && trie_parent && trie_tok && out_tok && out_n && out_score &&
+                 state_i && state_f && fresh, "masr_ctc_prefix_beam_pool: null pointer");
+    MASR_REQUIRE(beam_size >= 1 && beam_size <= BEAM_CAP, "masr_ctc_prefix_beam_pool: beam_size=%d out of range (1..%d)", beam_size, BEAM_CAP);
+    const int rc = pool_smem_attr<false>();
+    if (rc) return rc;
+    prefix_beam_kernel<false, true><<<B, BEAM_THREADS, sizeof(BeamShared), (cudaStream_t)stream>>>(
+        cand_id, cand_logp, cand_cnt, bstride, lens, beam_size, blank, pool, trie_parent, trie_tok, trie_cap, out_tok, tok_stride,
+        out_n, out_score, state_i, state_f, 0, LmSearch{}, fresh);
+    return check_launch("prefix_beam_kernel<pool>");
+}
+
 // ---- with the LM (BeamSearchDecoder with its Scorer: beam_search_decoder.py:29-32,47-56) ----
+template <bool POOL = false>
 static int launch_beam_lm(const char* what, const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
                           int64_t bstride, const int* lens, int B, int beam_size, int blank, const masr_lm_tables* lm, float alpha,
                           float beta, float* pool, int* trie_parent, int* trie_tok, int64_t trie_cap, int* state_i, float* state_f,
                           int resume, int* out_tok, int64_t tok_stride, int* out_n, float* out_score, float* out_approx,
-                          cudaStream_t stream) {
+                          cudaStream_t stream, int* fresh = nullptr) {
     MASR_REQUIRE(cand_id && cand_logp && cand_cnt && blank_logp && lens && pool && trie_parent && trie_tok && out_tok && out_n &&
                  out_score && out_approx && lm, "%s: null pointer", what);
     MASR_REQUIRE(lm->keys && lm->vals && lm->tok2lm, "%s: LM tables not set", what);
     MASR_REQUIRE(lm->order >= 1 && lm->order <= LM_MAX_ORDER, "%s: LM order %d out of range (1..%d)", what, lm->order, LM_MAX_ORDER);
     MASR_REQUIRE(beam_size >= 1 && beam_size <= BEAM_CAP, "%s: beam_size=%d out of range (1..%d)", what, beam_size, BEAM_CAP);
-    cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BeamSharedLm));
-    if (e != cudaSuccess) { set_last_error("prefix_beam<lm> smem attr: %s", cudaGetErrorString(e)); return (int)e; }
+    if constexpr (POOL) {
+        MASR_REQUIRE(state_i && state_f && fresh, "%s: null pointer", what);
+        const int rc = pool_smem_attr<true>();
+        if (rc) return rc;
+    } else {
+        cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BeamSharedLm));
+        if (e != cudaSuccess) { set_last_error("prefix_beam<lm> smem attr: %s", cudaGetErrorString(e)); return (int)e; }
+    }
     const LmSearch lms{*lm, blank_logp, alpha, beta, out_approx};
-    prefix_beam_kernel<true><<<B, BEAM_THREADS, sizeof(BeamSharedLm), stream>>>(
+    prefix_beam_kernel<true, POOL><<<B, BEAM_THREADS, sizeof(BeamSharedLm), stream>>>(
         cand_id, cand_logp, cand_cnt, bstride, lens, beam_size, blank, pool, trie_parent, trie_tok, trie_cap, out_tok, tok_stride,
-        out_n, out_score, state_i, state_f, resume, lms);
+        out_n, out_score, state_i, state_f, resume, lms, fresh);
     return check_launch(what);
 }
 
@@ -681,4 +743,15 @@ extern "C" int masr_ctc_prefix_beam_lm_stream(const int* cand_id, const float* c
     return launch_beam_lm("masr_ctc_prefix_beam_lm_stream", cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size,
                           blank, lm_host, alpha, beta, pool, trie_parent, trie_tok, trie_cap, state_i, state_f, resume, out_tok,
                           tok_stride, out_n, out_score, out_approx, (cudaStream_t)stream);
+}
+
+extern "C" int masr_ctc_prefix_beam_lm_pool(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
+                                            int64_t bstride, const int* lens, int B, int beam_size, int blank,
+                                            const masr_lm_tables* lm_host, float alpha, float beta, float* pool, int* trie_parent,
+                                            int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int* fresh, int* out_tok,
+                                            int64_t tok_stride, int* out_n, float* out_score, float* out_approx, void* stream) {
+    if (B == 0) return MASR_OK;
+    return launch_beam_lm<true>("masr_ctc_prefix_beam_lm_pool", cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size,
+                                blank, lm_host, alpha, beta, pool, trie_parent, trie_tok, trie_cap, state_i, state_f, 0, out_tok,
+                                tok_stride, out_n, out_score, out_approx, (cudaStream_t)stream, fresh);
 }

@@ -349,6 +349,17 @@ class MASRPredictor:
             raise Exception("masr_b200: inverse text normalisation (is_itn) is outside the hot-path scope")
         return {'text': text, 'score': score}
 
+    def create_stream_pool(self, n_slots: int, max_frames: int = 3000):
+        """Additive: a ``StreamPool`` of ``n_slots`` concurrent streams over this predictor's model, decoding as the YAML
+        says — greedy, or the GPU prefix beam search with the character LM this predictor loaded (if any).  Each slot's
+        ``push`` results equal ``predict_stream`` on that stream alone.  ``max_frames``: encoder frames one stream may reach
+        before it must be reset (40 ms each; 3000 = 2 minutes)."""
+        if not self.configs.streaming:
+            raise Exception(f"不支持改该模型流式识别，当前模型：{self.configs.use_model}，参数streaming为：{self.configs.streaming}")
+        from .stream_pool import StreamPool
+        return StreamPool(self.predictor, self._text_featurizer.vocab_list, n_slots, use_db_normalization=self._use_db,
+                          target_db=self._target_db, max_frames=max_frames, beam=self._beam_conf)
+
     def reset_stream(self):
         """predict.py:346-353."""
         if self._stream is not None:

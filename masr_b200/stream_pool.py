@@ -7,16 +7,19 @@ config 3/5 ask for dozens to hundreds of concurrent streams.  ``ConformerStreamP
 that has a chunk ready in ONE pass of tensor-core GEMMs (M = slots x 16 rows) — each slot computed exactly like the
 single-stream ``encode_chunk`` / reference ``forward_chunk`` with ``required_cache_size < 0`` (all history kept, which
 is what ``predict_stream`` passes).  ``StreamPool`` adds the per-stream host logic of ``predict_stream`` (sample
-carry-over with in-place dB renormalisation, 67/64/3 feature windowing, greedy history).
+carry-over with in-place dB renormalisation, 67/64/3 feature windowing, greedy history) and, with ``beam=...``, the
+streaming CTC prefix beam search of every slot (``PoolBeam``: two more launches per chunk step, inside its CUDA graph).
 """
 from __future__ import annotations
 
+import gc
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 import torch
 
-from ._lib import EPI_BIAS, EPI_BIAS_GLU, EPI_BIAS_SCALE, EPI_BIAS_SILU, EPI_RESIDUAL
+from . import _lib
+from ._lib import EPI_BIAS, EPI_BIAS_GLU, EPI_BIAS_SCALE, EPI_BIAS_SILU, EPI_RESIDUAL, call
 from .audio import pcm_bytes_to_float32, samples_to_float32
 from .engine import ConformerEngine, _p, greedy_score, subsampled_len
 from .predict import CACHED_FEATURE_NUM, DECODING_WINDOW, FRAME_SHIFT, chunk_starts
@@ -55,6 +58,7 @@ class _PoolBase:
         # both; not measured faster on the H100).
         import os
         self.fuse_ln = os.environ.get("MASR_POOL_FUSE_LN", "0") == "1" and eng.d == 256
+        self.beam = None              # PoolBeam: the prefix beam search runs after every step (captured with it)
         self._graph = None
         self._graph_launches = 0
         self._warm = False
@@ -90,22 +94,35 @@ class _PoolBase:
         """Eager on the first step (one-time setup: function attributes, tables), then capture once and replay."""
         eng = self.eng
         if not self.use_graph:
-            self._body()
+            self._step_body()
             return
         if not self._warm:
-            self._body()
+            self._step_body()
             self._warm = True
             return
         if self._graph is None:
             n0 = eng.launches
             g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, capture_error_mode="thread_local"):
-                self._body()
+            # no garbage collection inside the capture: a collected object that owns a CUDA graph (e.g. a dropped pool in a
+            # reference cycle) would destroy it here, which is not permitted while a stream captures and invalidates this graph
+            gc_on = gc.isenabled()
+            gc.disable()
+            try:
+                with torch.cuda.graph(g, capture_error_mode="thread_local"):
+                    self._step_body()
+            finally:
+                if gc_on:
+                    gc.enable()
             self._graph_launches = eng.launches - n0
             eng.launches = n0
             self._graph = g
         self._graph.replay()
         eng.launches += self._graph_launches
+
+    def _step_body(self):
+        self._body()
+        if self.beam is not None:
+            self.beam.launch()
 
     def _append_pair(self, src, ld_src_elems, col0_elems, ncols, dst, cap, base_row, cnt_row, rows_per_slot, elem_bytes=2):
         """dst pair rows (s*cap + base[s] + t) <- src pair rows (s*rows_per_slot + t), columns [col0, col0+ncols)."""
@@ -543,6 +560,104 @@ def make_pool(eng, n_slots: int, max_frames: int = 3000):
     raise NotImplementedError(f"no stream pool for {type(eng).__name__}")
 
 
+class PoolBeam:
+    """Streaming CTC prefix beam search of EVERY slot of a chunk-decoding pool (``engine.StreamBeam`` for many streams; the
+    reference's ``BeamSearchDecoder.decode_chunk / reset_decoder`` per stream, beam_search_decoder.py:75-96).
+
+    Each pool step adds two launches, captured into the step's CUDA graph with the encoder: the top-k candidates of all
+    ``S * OUT_ROWS`` CTC-head rows (``pool.b["logits"]``), then ``masr_ctc_prefix_beam[_lm]_pool`` with one CTA per slot
+    over that slot's valid rows (the length row of the pool's device ``meta``).  Slots without frames in a step are not
+    touched.  Per slot the beam, its trie and the trie's hash stay on the device, so after every step a slot's best
+    prefix equals the whole-utterance search over its frames since the last ``reset`` — what ``predict_stream`` returns.
+    The trie is sized by ``beam_size`` and the pool's frame capacity (at most ``beam_size`` new prefixes per frame), so
+    no stream the pool accepts can overflow it.  ``lm`` / ``alpha`` / ``beta``: character-LM shallow fusion as in
+    ``StreamBeam``; the reported score is then approx_ctc."""
+
+    def __init__(self, pool, beam_size: int = 300, cutoff_prob: float = 0.99, cutoff_top_n: int = 40, lm=None,
+                 alpha: float = 0.0, beta: float = 0.0):
+        beam_size = int(beam_size)
+        if not 1 <= beam_size <= 512:
+            raise ValueError(f"beam_size={beam_size} out of range (1..512)")
+        self.beam, self.cutoff, self.top_n = beam_size, float(cutoff_prob), int(cutoff_top_n)
+        self.lm, self.alpha, self.beta = lm, float(alpha), float(beta)
+        eng, S, R = pool.eng, pool.S, pool.OUT_ROWS
+        dev, C = eng.device, _lib.C
+        # what the launches read from the pool (the pool holds this object: no reference back to it, so dropping a pool frees
+        # its CUDA graph at once instead of in a later garbage collection, which may fall inside another pool's capture)
+        self.eng, self.S, self.R, self.logits = eng, S, R, pool.b["logits"]
+        self.lens = pool._m(pool.QLEN if R == CHUNK_OUT else pool.QLEN2)          # valid rows per slot (device meta row)
+        # beam frames one slot can reach: the pool's cap at its output rate (+1: the EfficientConformer halves an odd final chunk up)
+        self.frames = pool.cap * R // CHUNK_OUT + 1
+        pool_n, trie_n, si, sf = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_int64(0)
+        call("masr_ctc_prefix_beam_workspace", S, 1, C.byref(pool_n), C.byref(trie_n))
+        call("masr_ctc_prefix_beam_lm_state_size" if lm is not None else "masr_ctc_prefix_beam_state_size", C.byref(si), C.byref(sf))
+        self.trie_cap = 5 * (self.frames * beam_size + 1)          # nodes + 4 hash slots per node; the kernel reads node_cap = cap / 5
+        i32, f32 = torch.int32, torch.float32
+        self.cand_id = torch.zeros(S * R, 40, device=dev, dtype=i32)
+        self.cand_lp = torch.zeros(S * R, 40, device=dev, dtype=f32)
+        self.cand_n = torch.zeros(S * R, device=dev, dtype=i32)
+        self.scratch = torch.empty(pool_n.value, device=dev, dtype=f32)
+        self.trie_par = torch.full((S * self.trie_cap,), -1, device=dev, dtype=i32)     # every slot's hash starts empty
+        self.trie_tok = torch.empty(S * self.trie_cap, device=dev, dtype=i32)
+        self.state_i = torch.zeros(S, si.value, device=dev, dtype=i32)
+        self.state_f = torch.zeros(S, sf.value, device=dev, dtype=f32)
+        self.fresh = torch.ones(S, device=dev, dtype=i32)
+        self.out_tok = torch.zeros(S, self.frames, device=dev, dtype=i32)
+        self.out = torch.zeros(3, S, device=dev, dtype=f32)         # [reported score, token count (int32 bits), fused score]
+        if lm is not None:
+            self.blank_lp = torch.zeros(S * R, device=dev, dtype=f32)
+            self.lm_t = C.byref(lm.tables(dev))
+
+    def reset(self, slot: int):
+        """``reset_decoder`` for one slot: start it at the root on its next frames (the kernel clears the flag) with an empty
+        prefix hash."""
+        cap = self.trie_cap
+        self.fresh[slot] = 1
+        self.trie_par[slot * cap + cap // 5:(slot + 1) * cap].fill_(-1)
+
+    def launch(self):
+        """The two launches of one pool step (device inputs only: safe to capture and replay)."""
+        eng, S, R, logits = self.eng, self.S, self.R, self.logits
+        n_view = self.out[1].view(torch.int32)
+        if self.lm is not None:
+            eng._k("ctc_topk", "masr_ctc_topk_blank_f32", _p(logits), eng.Vpad, S * R, eng.V, self.top_n, self.cutoff, 0,
+                   _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n), _p(self.blank_lp))
+            eng._k("prefix_beam", "masr_ctc_prefix_beam_lm_pool", _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n),
+                   _p(self.blank_lp), R, self.lens, S, self.beam, 0, self.lm_t, self.alpha, self.beta,
+                   _p(self.scratch), _p(self.trie_par), _p(self.trie_tok), self.trie_cap, _p(self.state_i), _p(self.state_f),
+                   _p(self.fresh), _p(self.out_tok), self.frames, _p(n_view), _p(self.out[2]), _p(self.out[0]))
+        else:
+            eng._k("ctc_topk", "masr_ctc_topk_f32", _p(logits), eng.Vpad, S * R, eng.V, self.top_n, self.cutoff,
+                   _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n))
+            eng._k("prefix_beam", "masr_ctc_prefix_beam_pool", _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n), R,
+                   self.lens, S, self.beam, 0, _p(self.scratch), _p(self.trie_par), _p(self.trie_tok), self.trie_cap,
+                   _p(self.state_i), _p(self.state_f), _p(self.fresh), _p(self.out_tok), self.frames, _p(n_view), _p(self.out[0]))
+
+    def results(self, slots: Sequence[int], frames: Sequence[int]) -> Dict[int, tuple]:
+        """slot -> (token ids of its best prefix, score) after the last step: one D2H copy of every slot's count and score,
+        then one of the token rows spanning `slots`.  ``frames[slot]``: the slot's encoder frames since its reset; a slot
+        without any gets ([], 0.0), as ``predict_stream`` does."""
+        slots = list(slots)
+        if not slots:
+            return {}
+        eng = self.eng
+        oh = self.out.cpu()
+        n = oh[1].view(torch.int32).numpy()
+        score = oh[0].numpy()
+        had = [s for s in slots if frames[s] > 0]
+        nmax = max((int(n[s]) for s in had), default=0)
+        lo, hi = (min(had), max(had) + 1) if had else (0, 0)
+        toks = self.out_tok[lo:hi, :nmax].cpu().numpy() if nmax else None
+        eng.d2h_bytes += oh.numel() * 4 + (0 if toks is None else toks.size * 4)
+        out = {}
+        for s in slots:
+            if frames[s] == 0:
+                out[s] = ([], 0.0)
+            else:
+                out[s] = (toks[s - lo, :n[s]].tolist() if n[s] else [], float(score[s]))
+        return out
+
+
 class StreamPool:
     """`predict_stream` for many streams at once (same per-stream results as one ``MASRPredictor`` per stream).
 
@@ -554,9 +669,20 @@ class StreamPool:
     RING = 1024                    # feature frames kept per slot (un-consumed frames never exceed one push + one window)
 
     def __init__(self, eng: ConformerEngine, vocab: Sequence[str], n_slots: int, use_db_normalization: bool = True,
-                 target_db: float = -20.0, max_frames: int = 3000):
+                 target_db: float = -20.0, max_frames: int = 3000, beam: Optional[dict] = None, use_graph: bool = True):
+        """``beam``: None decodes greedily (``ctc_greedy``); a dict ``{beam_size, cutoff_prob, cutoff_top_n, lm, alpha,
+        beta}`` (``MASRPredictor``'s ``ctc_beam_search`` settings; ``lm`` a ``CharLM`` or None) runs the streaming prefix
+        beam search of every slot on the GPU (``PoolBeam``), and every result is the beam's, as ``predict_stream`` with
+        ``decoder: ctc_beam_search`` returns it.  ``use_graph=False`` launches every step eagerly instead of replaying
+        its CUDA graph (same results)."""
         self.eng, self.vocab, self.S = eng, list(vocab), n_slots
         self.pool = make_pool(eng, n_slots, max_frames)
+        if not use_graph:
+            self.pool.use_graph = False
+        self.beam = None
+        if beam is not None:
+            self.beam = PoolBeam(self.pool, **beam)
+            self.pool.beam = self.beam
         self.use_db, self.target_db = use_db_normalization, target_db
         self.remained: List[Optional[np.ndarray]] = [None] * n_slots
         dev = eng.device
@@ -605,6 +731,8 @@ class StreamPool:
 
     def reset_stream(self, slot: int):
         self.pool.reset(slot)
+        if self.beam is not None:
+            self.beam.reset(slot)
         self.remained[slot] = None
         self.head[slot], self.count[slot] = 0, 0
         self._reset_hist([slot])
@@ -729,7 +857,9 @@ class StreamPool:
                         ends[s] = int(c_ + n_)
                 batch = self.ring.index_select(0, self._dev_index(idx.reshape(-1))).view(S, CHUNK_FRAMES, 80)
                 ids, maxp, tout = self.pool.step(batch, nfr)
-                self._fold(ids.cpu().numpy(), maxp.cpu().numpy(), tout)
+                if self.beam is None:                # (the beam's state stays on the device: no copy per round)
+                    self._fold(ids.cpu().numpy(), maxp.cpu().numpy(), tout)
+            beam_out = self.beam.results([s for s in live if pending[s]], self.pool.lens_host) if self.beam is not None else None
             for s in live:
                 if not pending[s]:
                     out[s] = None
@@ -737,7 +867,11 @@ class StreamPool:
                 consumed = ends[s] - CACHED_FEATURE_NUM              # predict.py:330: keep the last 3 frames of the window
                 self.head[s] = (self.head[s] + consumed) % R
                 self.count[s] -= consumed
-                out[s] = {"text": ids_to_text(self.toks[s], self.vocab), "score": greedy_score(self.acc[s], int(self.nprob[s]))}
+                if beam_out is not None:
+                    toks, score = beam_out[s]
+                    out[s] = {"text": ids_to_text(toks, self.vocab), "score": score}
+                else:
+                    out[s] = {"text": ids_to_text(self.toks[s], self.vocab), "score": greedy_score(self.acc[s], int(self.nprob[s]))}
         if errors and on_error == "raise":
             raise StreamSlotError(errors, out)
         return out
