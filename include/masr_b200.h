@@ -62,6 +62,18 @@ int masr_check_device(void);
 int masr_stage_waves_f32(const void* const* waves, const int64_t* lengths, int B, float* pinned, float* dev, int nthreads,
                          void* stream);
 
+/* resampy.resample(x, src_rates[b], dst_rate, filter='kaiser_best') per utterance of a packed ragged batch
+ * (masr/data_utils/audio.py:306-317, called by AudioFeaturizer.featurize, audio_featurizer.py:45-47), bit-identical to
+ * the restatement in oracle/resample.py.  x: packed float32 input, x_offsets int64[B+1]; src_rates int32[B] (device);
+ * table: float64[table_len], the right wing of the kaiser_best filter (512 entries per zero crossing);
+ * y: packed float32 output, y_offsets int64[B+1] with y_len[b] = int(x_len[b] * dst_rate / src_rates[b]).
+ * Rows with src_rates[b] == dst_rate are copied verbatim (y_len[b] == x_len[b]).  Host-side launch bounds:
+ * max_out >= every y_len[b]; max_src_rate >= every src_rates[b] (it sizes the shared input window; rows above it
+ * are left untouched).  Fails for max_src_rate > 512 * dst_rate. */
+int masr_resample_f32(const float* x, const int64_t* x_offsets, const int* src_rates, int dst_rate, int B,
+                      const double* table, int table_len, float* y, const int64_t* y_offsets, int64_t max_out,
+                      int max_src_rate, void* stream);
+
 /* Bytes of scratch masr_wave_gain_f32 needs for B utterances of at most max_samples samples. */
 int masr_fbank_workspace_bytes(int B, int64_t max_samples, int64_t* bytes_host);
 

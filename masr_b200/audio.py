@@ -7,7 +7,8 @@ Mirrors the parts of ``masr.data_utils.audio.AudioSegment`` that ``MASRPredictor
   * ``from_file`` / ``from_bytes`` for PCM WAV containers (the reference uses soundfile/PyAV,
     which are not part of the path's arithmetic; only RIFF/WAVE PCM is supported here).
 dB normalisation, int16 quantisation and fbank happen on the GPU (csrc/fbank.cu).
-Resampling (resampy, audio.py:306-317) is outside the hot-path scope: a sample-rate mismatch raises.
+Resampling (resampy kaiser_best, audio.py:306-317) runs on the GPU (``masr_b200.resample``, csrc/resample.cu) when the
+predictor is built with ``resample=True``; otherwise a sample-rate mismatch raises.
 """
 from __future__ import annotations
 

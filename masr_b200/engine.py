@@ -19,6 +19,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from . import resample as resampling
 from ._lib import EPI_BIAS, EPI_BIAS_GLU, EPI_BIAS_SCALE, EPI_BIAS_SILU, EPI_RESIDUAL, call
 from .weights import ConformerWeights, load_state_dict, pack_conformer
 
@@ -105,6 +106,7 @@ class ConformerEngine:
         self._pinned: Optional[torch.Tensor] = None      # grow-only pinned staging buffer for H2D copies
         self._out_pinned: Optional[torch.Tensor] = None  # pinned landing buffer of the packed per-step outputs
         self._staged: Optional[torch.cuda.Event] = None
+        self._rs_in: Dict[str, torch.Tensor] = {}         # original-rate inputs of a graph replay that resamples first
         self.h2d_bytes = 0
         self.d2h_bytes = 0
         self.last_gain = None
@@ -385,11 +387,13 @@ class ConformerEngine:
     def fbank(self, waves: Sequence[np.ndarray], use_db_normalization: bool = True, target_db: float = -20.0,
               wave_dev: Optional[torch.Tensor] = None, offsets_dev: Optional[torch.Tensor] = None,
               lengths: Optional[Sequence[int]] = None, force_fmax: Optional[int] = None,
-              status_out: Optional[torch.Tensor] = None):
+              status_out: Optional[torch.Tensor] = None, rates: Optional[Sequence[int]] = None):
         """float32 waveforms in [-1,1) -> (feats [B,Fmax,80] on device, frame counts, status flags).
 
         Either host arrays (copied through pinned memory) or an already packed device buffer
-        (``wave_dev`` float32[total], ``offsets_dev`` int64[B+1], ``lengths``)."""
+        (``wave_dev`` float32[total], ``offsets_dev`` int64[B+1], ``lengths``).  ``rates``: per-utterance sample rates of
+        the host arrays; rows not at 16 kHz are resampled on the device first (audio_featurizer.py:45-47), and the frame
+        counts are those of the resampled rows."""
         if wave_dev is None:
             lengths = [int(w.shape[0]) for w in waves]
             nb = len(waves)
@@ -412,6 +416,8 @@ class ConformerEngine:
             self._staged = torch.cuda.Event()
             self._staged.record(torch.cuda.current_stream(self.device))
             self.h2d_bytes += 4 * total + 8 * (nb + 1)
+            if resampling.needs_resampling(rates):
+                wave_dev, offsets_dev, lengths = self._resample_packed(wave_dev, offsets_dev, lengths, rates)
         B = len(lengths)
         frames = [num_frames(n) for n in lengths]
         Fmax = max(frames) if frames else 0
@@ -438,6 +444,34 @@ class ConformerEngine:
         if Fmax > 0:
             self._k("fbank", "masr_fbank_f32", _p(wave_dev), _p(offsets_dev), _p(gain), B, Fmax, _p(feats), None)
         return feats, frames, status
+
+    def _resample_packed(self, x, x_offs, lengths, rates):
+        """Packed device batch at ``rates`` -> (packed 16 kHz batch, its offsets, its lengths), one kernel launch."""
+        rates = [int(r) for r in rates]
+        out_lengths = [resampling.output_length(n, r) for n, r in zip(lengths, rates)]
+        offs = resampling.offsets(out_lengths)
+        y = torch.empty(max(1, int(offs[-1])), device=self.device, dtype=torch.float32)
+        y_offs = torch.from_numpy(offs).to(self.device)
+        rates_dev = torch.tensor(rates, dtype=torch.int32).to(self.device)
+        self.h2d_bytes += 8 * len(offs) + 4 * len(rates)
+        resampling.launch(self, x, x_offs, rates_dev, y, y_offs, rates, out_lengths)
+        return y, y_offs, out_lengths
+
+    def resample(self, waves: Sequence[np.ndarray], rates: Sequence[int]) -> List[np.ndarray]:
+        """Host float32 waveforms at ``rates`` -> the same waveforms at 16 kHz (``AudioSegment.resample``, audio.py:306-317),
+        computed on the device and copied back; rows already at 16 kHz come back unchanged."""
+        lengths = [int(w.shape[0]) for w in waves]
+        if not waves:
+            return []
+        x = torch.from_numpy(np.concatenate([np.asarray(w, np.float32) for w in waves]) if sum(lengths) else
+                             np.zeros(1, np.float32)).to(self.device)
+        x_offs = torch.from_numpy(resampling.offsets(lengths)).to(self.device)
+        self.h2d_bytes += 4 * sum(lengths) + 8 * (len(lengths) + 1)
+        y, _, out_lengths = self._resample_packed(x, x_offs, lengths, rates)
+        yh = y.cpu().numpy()
+        self.d2h_bytes += 4 * sum(out_lengths)
+        offs = resampling.offsets(out_lengths)
+        return [yh[offs[i]:offs[i + 1]].copy() for i in range(len(waves))]
 
     # ---- encoder -----------------------------------------------------------------------------
     def encode(self, feats: torch.Tensor, feat_lens: Sequence[int], tlens_dev: Optional[torch.Tensor] = None):
@@ -667,17 +701,18 @@ class ConformerEngine:
 
     def transcribe_beam(self, waves: Sequence[np.ndarray], beam_size: int = 300, cutoff_prob: float = 0.99,
                         cutoff_top_n: int = 40, use_db_normalization: bool = True, target_db: float = -20.0, lm=None,
-                        alpha: float = 0.0, beta: float = 0.0):
-        """Host waveforms -> (token ids per utterance, log-scores) with the GPU prefix beam search (``lm``: see ctc_beam)."""
-        feats, frames, status = self.fbank(waves, use_db_normalization, target_db)
+                        alpha: float = 0.0, beta: float = 0.0, rates: Optional[Sequence[int]] = None):
+        """Host waveforms -> (token ids per utterance, log-scores) with the GPU prefix beam search (``lm``: see ctc_beam;
+        ``rates``: see transcribe)."""
+        feats, frames, status = self.fbank(waves, use_db_normalization, target_db, rates=rates)
         return self.beam_features(feats, frames, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta)
 
     def transcribe_beam_pipelined(self, batches, beam_size: int = 300, cutoff_prob: float = 0.99, cutoff_top_n: int = 40,
                                   use_db_normalization: bool = True, target_db: float = -20.0, lm=None, alpha: float = 0.0,
-                                  beta: float = 0.0):
-        """Generator over ``batches`` (iterable of lists of float32 waveforms) yielding ``transcribe_beam(batch)`` per batch, in
-        order, one batch late.  The prefix beam search is one CTA per utterance — 32 of 132 SMs busy for milliseconds — so it
-        runs on a SECOND stream, concurrently with the fbank / encoder / top-k kernels of the next batch on the idle SMs
+                                  beta: float = 0.0, with_rates: bool = False):
+        """Generator over ``batches`` (iterable of lists of float32 waveforms; with ``with_rates``, of ``(waves, rates)``
+        pairs, see transcribe) yielding ``transcribe_beam(batch)`` per batch, in order, one batch late.  The prefix beam
+        search is one CTA per utterance — 32 of 132 SMs busy for milliseconds — so it runs on a SECOND stream, concurrently with the fbank / encoder / top-k kernels of the next batch on the idle SMs
         (two sets of candidate / trie / output buffers; the LM tables are shared read-only).  Same results as the blocking
         call."""
         dev = self.device
@@ -702,6 +737,7 @@ class ConformerEngine:
             return [tok[b, :n[b]].tolist() for b in range(B)], [float(x) for x in sc]
 
         for waves in batches:
+            waves, rates = waves if with_rates else (waves, None)
             slot = self._beam_slots[k & 1]
             k += 1
             B = len(waves)
@@ -710,7 +746,7 @@ class ConformerEngine:
             else:
                 if "done" in slot:
                     main.wait_event(slot["done"])          # the slot's previous search (batch k-2) has consumed its buffers
-                feats, frames, status = self.fbank(waves, use_db_normalization, target_db)
+                feats, frames, status = self.fbank(waves, use_db_normalization, target_db, rates=rates)
                 enc, tl, T, ws = self.encode(feats, frames)
                 M = B * max(1, T)
                 if slot.get("M", 0) < M or slot.get("B", 0) < B or slot.get("T", 0) < T:
@@ -778,11 +814,12 @@ class ConformerEngine:
 
     # ---- public batched entry points -----------------------------------------------------------
     def transcribe(self, waves: Sequence[np.ndarray], use_db_normalization: bool = True, target_db: float = -20.0,
-                   return_frames: bool = False) -> GreedyResult:
-        """Host float32 waveforms -> greedy token ids + scores.  One H2D copy in, a few KB out."""
+                   return_frames: bool = False, rates: Optional[Sequence[int]] = None) -> GreedyResult:
+        """Host float32 waveforms -> greedy token ids + scores.  One H2D copy in, a few KB out.  ``rates``: per-utterance
+        sample rates (None: all 16 kHz); other rates are resampled on the device before the fbank."""
         if self.use_graphs and self.prof is None and len(waves) > 0:
-            return self._transcribe_graph(waves, use_db_normalization, target_db, return_frames)
-        feats, frames, status = self.fbank(waves, use_db_normalization, target_db)
+            return self._transcribe_graph(waves, use_db_normalization, target_db, return_frames, rates)
+        feats, frames, status = self.fbank(waves, use_db_normalization, target_db, rates=rates)
         return self.transcribe_features(feats, frames, status, return_frames)
 
     def final_len(self, t: int) -> int:
@@ -846,8 +883,11 @@ class ConformerEngine:
         return g
 
     # ---- pipelined batches: host staging + H2D of batch k+1 overlap the device step of batch k ---------------------
-    def transcribe_pipelined(self, batches, use_db_normalization: bool = True, target_db: float = -20.0, device_hook=None):
-        """Generator over ``batches`` (an iterable of lists of float32 waveforms) yielding one ``GreedyResult`` per batch,
+    def transcribe_pipelined(self, batches, use_db_normalization: bool = True, target_db: float = -20.0, device_hook=None,
+                             with_rates: bool = False):
+        """Generator over ``batches`` (an iterable of lists of float32 waveforms; with ``with_rates``, of ``(waves, rates)``
+        pairs: a batch with rows off 16 kHz is staged at its own rates and resampled on the compute stream into the graph's
+        static inputs right before the replay) yielding one ``GreedyResult`` per batch,
         in order, each identical to ``transcribe(batch)``.  PIPE_DEPTH static input sets + pinned staging buffers: while the
         CUDA graph of batch k runs on the compute stream, batches k+1.. are packed into pinned memory by the native stager and
         copied H2D on a separate copy stream; the packed outputs of batch k come back in one D2H copy.  Results lag the
@@ -858,7 +898,7 @@ class ConformerEngine:
         comp = torch.cuda.current_stream(dev)
         if getattr(self, "_copy_stream", None) is None:
             self._copy_stream = torch.cuda.Stream(device=dev)
-            self._pipe = [{"pinned": None, "out": None, "staged": torch.cuda.Event(), "done": torch.cuda.Event()}
+            self._pipe = [{"pinned": None, "out": None, "rs": {}, "staged": torch.cuda.Event(), "done": torch.cuda.Event()}
                           for _ in range(self.PIPE_DEPTH)]
         copy = self._copy_stream
         k = 0
@@ -883,10 +923,11 @@ class ConformerEngine:
         from collections import deque
         pending = deque()                                   # items in flight: at most PIPE_DEPTH - 1 behind the one being staged
         for waves in batches:
+            waves, rates = waves if with_rates else (waves, None)
             slot = k % self.PIPE_DEPTH
             k += 1
             B = len(waves)
-            lengths = [int(w.shape[0]) for w in waves]
+            lengths, rates = self._batch_lengths(waves, rates)
             frames = [num_frames(n) for n in lengths]
             q = self.GRAPH_FRAME_QUANTUM
             Fpad = max(q, (max(frames) + q - 1) // q * q) if B else q
@@ -898,30 +939,15 @@ class ConformerEngine:
             else:
                 g = self._graph_for(B, Fpad, use_db_normalization, target_db, slot)      # (captures on first use)
                 P = self._pipe[slot]
-                offs = np.zeros(B + 1, np.int64)
-                np.cumsum(lengths, out=offs[1:])
-                total = int(offs[-1])
-                need = total + 4 * (B + 2) + 8
+                need = self.need_pinned(sum(int(w.shape[0]) for w in waves), B)
                 if P["pinned"] is None or P["pinned"].numel() < need:
                     P["pinned"] = torch.empty((int(1.25 * need) + 1024) // 2 * 2, dtype=torch.float32, pin_memory=True)
-                pin = P["pinned"]
-                waves = [w if (w.dtype == np.float32 and w.flags.c_contiguous) else np.ascontiguousarray(w, np.float32) for w in waves]
-                ptrs = (_lib.C.c_void_p * B)(*[w.ctypes.data for w in waves])
-                lens_c = (_lib.C.c_int64 * B)(*lengths)
                 # the slot's previous batch (k - PIPE_DEPTH) was consumed before its result was yielded: its buffers are free
-                call("masr_stage_waves_f32", ptrs, lens_c, B, pin.data_ptr(), g["wave"].data_ptr(), self.STAGE_THREADS,
-                     copy.cuda_stream)
-                t0 = (total + 1) // 2 * 2
-                po = pin[t0:t0 + 2 * (B + 1)].view(torch.int64)
-                po.numpy()[:] = offs
-                pt = pin[t0 + 2 * (B + 1):t0 + 2 * (B + 1) + B].view(torch.int32)
-                pt.numpy()[:] = tl1
-                with torch.cuda.stream(copy):
-                    g["offs"].copy_(po, non_blocking=True)
-                    g["tlens"].copy_(pt, non_blocking=True)
-                    P["staged"].record(copy)
-                self.h2d_bytes += 4 * total + 8 * (B + 1) + 4 * B
+                self._stage_graph_inputs(g, waves, lengths, tl1, rates, P["pinned"], P["rs"], copy)
+                P["staged"].record(copy)
                 comp.wait_event(P["staged"])
+                if rates is not None:
+                    self._resample_graph_inputs(g, P["rs"], rates, lengths)
                 g["graph"].replay()
                 self.launches += g["launches"]
                 pack = g["ws"]["out_pack"]
@@ -965,9 +991,66 @@ class ConformerEngine:
         step.g = g                                       # the static input buffers (a scatter may write g["wave"] directly)
         return step
 
-    def _transcribe_graph(self, waves, use_db, target_db, return_frames) -> GreedyResult:
+    def _stage_graph_inputs(self, g, waves, lengths, tl1, rates, pinned, rs, stream):
+        """Stage one batch for a replay of graph ``g`` on ``stream``: the samples, offsets and subsampled lengths go into
+        ``g``'s static inputs, packed by the native stager into ``pinned`` (which holds ``need_pinned`` floats).  A batch with
+        rows off 16 kHz (``rates``) is staged at its own rates into the device buffers ``rs`` instead (original samples,
+        their offsets, the rates); ``_resample_graph_inputs`` then fills ``g["wave"]`` / ``g["offs"]`` from them."""
         B = len(waves)
+        in_lengths = [int(w.shape[0]) for w in waves]
+        offs = resampling.offsets(lengths)
+        total = int(sum(in_lengths))
+        dest = g["wave"]
+        if rates is not None:
+            if rs.get("x") is None or rs["x"].numel() < total or rs["offs"].numel() < B + 1:
+                rs["x"] = torch.empty(max(1, int(1.25 * total)), device=self.device, dtype=torch.float32)
+                rs["offs"] = torch.empty(B + 1, device=self.device, dtype=torch.int64)
+                rs["rates"] = torch.empty(B, device=self.device, dtype=torch.int32)
+            dest = rs["x"]
+        waves = [w if (w.dtype == np.float32 and w.flags.c_contiguous) else np.ascontiguousarray(w, np.float32) for w in waves]
+        ptrs = (_lib.C.c_void_p * B)(*[w.ctypes.data for w in waves])
+        lens_c = (_lib.C.c_int64 * B)(*in_lengths)
+        call("masr_stage_waves_f32", ptrs, lens_c, B, pinned.data_ptr(), dest.data_ptr(), self.STAGE_THREADS,
+             stream.cuda_stream)
+        t0 = (total + 1) // 2 * 2
+        po = pinned[t0:t0 + 2 * (B + 1)].view(torch.int64)
+        po.numpy()[:] = offs
+        t1 = t0 + 2 * (B + 1)
+        pt = pinned[t1:t1 + B].view(torch.int32)
+        pt.numpy()[:] = tl1
+        with torch.cuda.stream(stream):
+            g["offs"].copy_(po, non_blocking=True)
+            g["tlens"].copy_(pt, non_blocking=True)
+            if rates is not None:
+                t2 = (t1 + B + 1) // 2 * 2
+                pi = pinned[t2:t2 + 2 * (B + 1)].view(torch.int64)
+                pi.numpy()[:] = resampling.offsets(in_lengths)
+                pr = pinned[t2 + 2 * (B + 1):t2 + 2 * (B + 1) + B].view(torch.int32)
+                pr.numpy()[:] = rates
+                rs["offs"][:B + 1].copy_(pi, non_blocking=True)
+                rs["rates"][:B].copy_(pr, non_blocking=True)
+        self.h2d_bytes += 4 * total + 8 * (B + 1) + 4 * B + (0 if rates is None else 8 * (B + 1) + 4 * B)
+
+    @staticmethod
+    def need_pinned(total: int, B: int) -> int:
+        """Floats of pinned staging ``_stage_graph_inputs`` uses for ``total`` samples in ``B`` rows."""
+        return total + 10 * (B + 2) + 8
+
+    def _resample_graph_inputs(self, g, rs, rates, lengths):
+        """Resample the staged original-rate batch ``rs`` into graph ``g``'s static 16 kHz inputs (current stream)."""
+        resampling.launch(self, rs["x"], rs["offs"], rs["rates"], g["wave"], g["offs"], rates, lengths)
+
+    def _batch_lengths(self, waves, rates):
+        """Samples per row as the fbank sees them (after resampling), and the rates when the batch needs resampling."""
         lengths = [int(w.shape[0]) for w in waves]
+        if not resampling.needs_resampling(rates):
+            return lengths, None
+        rates = [int(r) for r in rates]
+        return [resampling.output_length(n, r) for n, r in zip(lengths, rates)], rates
+
+    def _transcribe_graph(self, waves, use_db, target_db, return_frames, rates=None) -> GreedyResult:
+        B = len(waves)
+        lengths, rates = self._batch_lengths(waves, rates)
         frames = [num_frames(n) for n in lengths]
         Fmax = max(frames)
         q = self.GRAPH_FRAME_QUANTUM
@@ -981,29 +1064,17 @@ class ConformerEngine:
         g = self._graph_for(B, Fpad, use_db, target_db)
         # stage inputs: the native stager packs the utterances into the pinned buffer on a few host threads and issues the
         # H2D copy of every finished part at once (csrc/stage.cu); offsets + lengths follow as two tiny copies
-        offs = np.zeros(B + 1, np.int64)
-        np.cumsum(lengths, out=offs[1:])
-        total = int(offs[-1])
         if self._staged is not None:
             self._staged.synchronize()
-        need = total + 4 * (B + 2) + 8
+        need = self.need_pinned(sum(int(w.shape[0]) for w in waves), B)
         if self._pinned is None or self._pinned.numel() < need:
             self._pinned = torch.empty((int(1.25 * need) + 1024) // 2 * 2, dtype=torch.float32, pin_memory=True)
-        waves = [w if (w.dtype == np.float32 and w.flags.c_contiguous) else np.ascontiguousarray(w, np.float32) for w in waves]
-        ptrs = (_lib.C.c_void_p * B)(*[w.ctypes.data for w in waves])
-        lens_c = (_lib.C.c_int64 * B)(*lengths)
-        call("masr_stage_waves_f32", ptrs, lens_c, B, self._pinned.data_ptr(), g["wave"].data_ptr(), self.STAGE_THREADS,
-             self._stream())
-        t0 = (total + 1) // 2 * 2
-        po = self._pinned[t0:t0 + 2 * (B + 1)].view(torch.int64)
-        po.numpy()[:] = offs
-        pt = self._pinned[t0 + 2 * (B + 1):t0 + 2 * (B + 1) + B].view(torch.int32)
-        pt.numpy()[:] = tl1
-        g["offs"].copy_(po, non_blocking=True)
-        g["tlens"].copy_(pt, non_blocking=True)
+        cur =torch.cuda.current_stream(self.device)
+        self._stage_graph_inputs(g, waves, lengths, tl1, rates, self._pinned, self._rs_in, cur)
         self._staged = torch.cuda.Event()
-        self._staged.record(torch.cuda.current_stream(self.device))
-        self.h2d_bytes += 4 * total + 8 * (B + 1) + 4 * B
+        self._staged.record(cur)
+        if rates is not None:
+            self._resample_graph_inputs(g, self._rs_in, rates, lengths)
         g["graph"].replay()
         self.launches += g["launches"]
         ws = g["ws"]

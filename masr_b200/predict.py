@@ -8,9 +8,10 @@ ids + a score come back (the reference featurises on the CPU, copies features up
 [T,V] posterior down and decodes with numpy — predict.py:181-190, inference_predictor.py:59-64).
 
 Additive entry points (the reference API is single-utterance): ``predict_batch``.
+Audio at other sample rates than 16 kHz is resampled on the GPU, as the reference's featurizer does
+(audio_featurizer.py:45-47), when the predictor is built with ``resample=True``; by default a rate mismatch raises.
 Out of the hot-path scope and therefore explicit errors here: punctuation (``use_pun``), inverse
-text normalisation (``is_itn``), VAD long-audio segmentation (``predict_long``), model download
-(``configs=None``), resampling, and ``use_gpu=False`` (there is no CPU path).
+text normalisation (``is_itn``), model download (``configs=None``) and ``use_gpu=False`` (there is no CPU path).
 """
 from __future__ import annotations
 
@@ -25,6 +26,7 @@ import yaml
 from . import SUPPORT_MODEL
 from .audio import load_audio, pcm_bytes_to_float32, samples_to_float32
 from .engine import ConformerEngine, EfficientConformerEngine, greedy_score, subsampled_len
+from .resample import MODEL_RATE, needs_resampling
 from .text import TextFeaturizer, ids_to_text
 
 logger = logging.getLogger(__name__)
@@ -72,7 +74,10 @@ class MASRPredictor:
                  model_path='models/conformer_streaming_fbank/inference.pt',
                  use_pun=False,
                  pun_model_dir='models/pun_models/',
-                 use_gpu=True):
+                 use_gpu=True,
+                 resample=False):
+        """``resample``: accept audio at any sample rate and resample it to ``preprocess_conf.sample_rate`` on the GPU,
+        as the reference's featurizer does (audio_featurizer.py:45-47); False keeps a rate mismatch an error."""
         if not configs:
             raise Exception("masr_b200: model download (configs=None, model_tag=...) is not supported; "
                             "pass a YAML path or dict plus model_path")
@@ -94,6 +99,9 @@ class MASRPredictor:
         self._sample_rate = int(pc.get('sample_rate', 16000))
         self._use_db = bool(pc.get('use_dB_normalization', True))
         self._target_db = float(pc.get('target_dB', -20))
+        self._resample = bool(resample)
+        if self._resample and self._sample_rate != MODEL_RATE:
+            raise Exception(f"masr_b200 resamples to {MODEL_RATE} Hz only (preprocess_conf.sample_rate = {self._sample_rate})")
         self._beam_conf = None
         self.lm = None
         if self.configs.decoder == 'ctc_beam_search':
@@ -156,9 +164,19 @@ class MASRPredictor:
         return lm
 
     def _check_rate(self, sr):
-        if sr != self._sample_rate:
+        if sr != self._sample_rate and not self._resample:
             raise Exception(f"masr_b200: resampling is outside the hot-path scope (got {sr} Hz, model expects "
                             f"{self._sample_rate} Hz)")
+
+    def _load_batch(self, audio_list, sample_rate):
+        """-> (float32 waveforms, their rates or None when every row is at the model rate)."""
+        waves, rates = [], []
+        for a in audio_list:
+            s, sr = load_audio(a, sample_rate)
+            self._check_rate(sr)
+            waves.append(s)
+            rates.append(sr)
+        return waves, (rates if needs_resampling(rates) else None)
 
     def _finish(self, text, use_pun, is_itn):
         if use_pun:
@@ -169,31 +187,27 @@ class MASRPredictor:
 
     def predict(self, audio_data, use_pun=False, is_itn=False, sample_rate=16000):
         """Whole-utterance recognition (predict.py:167-192)."""
-        samples, sr = load_audio(audio_data, sample_rate)
-        self._check_rate(sr)
+        waves, rates = self._load_batch([audio_data], sample_rate)
         if self._beam_conf is not None:
-            toks, scores = self.predictor.transcribe_beam([samples], use_db_normalization=self._use_db,
-                                                          target_db=self._target_db, **self._beam_conf)
+            toks, scores = self.predictor.transcribe_beam(waves, use_db_normalization=self._use_db,
+                                                          target_db=self._target_db, rates=rates, **self._beam_conf)
             text = ids_to_text(toks[0], self._text_featurizer.vocab_list)
             return {'text': self._finish(text, use_pun, is_itn), 'score': scores[0]}
-        res = self.predictor.transcribe([samples], self._use_db, self._target_db)
+        res = self.predictor.transcribe(waves, self._use_db, self._target_db, rates=rates)
         self._raise_status(res.status)
         text = ids_to_text(res.tokens[0], self._text_featurizer.vocab_list)
         return {'text': self._finish(text, use_pun, is_itn), 'score': res.scores[0]}
 
     def predict_batch(self, audio_list: Sequence, sample_rate=16000):
-        """Additive: a list of utterances in one GPU pass; element i equals ``predict(audio_list[i])``."""
-        waves = []
-        for a in audio_list:
-            s, sr = load_audio(a, sample_rate)
-            self._check_rate(sr)
-            waves.append(s)
+        """Additive: a list of utterances in one GPU pass; element i equals ``predict(audio_list[i])``.  With
+        ``resample=True`` the rows may have different rates (WAV files carry their own)."""
+        waves, rates = self._load_batch(audio_list, sample_rate)
         if self._beam_conf is not None:
             toks, scores = self.predictor.transcribe_beam(waves, use_db_normalization=self._use_db,
-                                                          target_db=self._target_db, **self._beam_conf)
+                                                          target_db=self._target_db, rates=rates, **self._beam_conf)
             vocab = self._text_featurizer.vocab_list
             return [{'text': ids_to_text(t, vocab), 'score': s} for t, s in zip(toks, scores)]
-        res = self.predictor.transcribe(waves, self._use_db, self._target_db)
+        res = self.predictor.transcribe(waves, self._use_db, self._target_db, rates=rates)
         self._raise_status(res.status)
         vocab = self._text_featurizer.vocab_list
         return [{'text': ids_to_text(t, vocab), 'score': s} for t, s in zip(res.tokens, res.scores)]
@@ -206,28 +220,16 @@ class MASRPredictor:
         vocab = self._text_featurizer.vocab_list
         if self._beam_conf is not None:
             # the prefix beam search of batch k runs on a second stream under the encoder of batch k+1
-            def loaded_b():
-                for audio_list in batches:
-                    waves = []
-                    for a in audio_list:
-                        s, sr = load_audio(a, sample_rate)
-                        self._check_rate(sr)
-                        waves.append(s)
-                    yield waves
-            for toks, scores in self.predictor.transcribe_beam_pipelined(loaded_b(), use_db_normalization=self._use_db,
-                                                                         target_db=self._target_db, **self._beam_conf):
+            loaded_b = (self._load_batch(audio_list, sample_rate) for audio_list in batches)
+            for toks, scores in self.predictor.transcribe_beam_pipelined(loaded_b, use_db_normalization=self._use_db,
+                                                                         target_db=self._target_db, with_rates=True,
+                                                                         **self._beam_conf):
                 yield [{'text': ids_to_text(t, vocab), 'score': s} for t, s in zip(toks, scores)]
             return
 
-        def loaded():
-            for audio_list in batches:
-                waves = []
-                for a in audio_list:
-                    s, sr = load_audio(a, sample_rate)
-                    self._check_rate(sr)
-                    waves.append(s)
-                yield waves
-        for res in self.predictor.transcribe_pipelined(loaded(), self._use_db, self._target_db, device_hook=device_hook):
+        loaded = (self._load_batch(audio_list, sample_rate) for audio_list in batches)
+        for res in self.predictor.transcribe_pipelined(loaded, self._use_db, self._target_db, device_hook=device_hook,
+                                                       with_rates=True):
             self._raise_status(res.status)
             yield [{'text': ids_to_text(t, vocab), 'score': s} for t, s in zip(res.tokens, res.scores)]
 
@@ -256,6 +258,9 @@ class MASRPredictor:
         self.init_vad(vad_predictor, vad_model_path)
         samples, sr = load_audio(audio_data, sample_rate)
         self._check_rate(sr)
+        if sr != self._sample_rate:
+            # predict.py:212-213: the whole recording is resampled first (on the GPU); the VAD runs on the 16 kHz samples
+            samples, sr = self.predictor.resample([samples], [sr])[0], self._sample_rate
         stamps = self.vad_predictor.get_speech_timestamps(samples, sr)
         segs = [samples[t['start']:t['end']] for t in stamps]
         results = self.predict_batch(segs, sample_rate=sr) if segs else []
@@ -290,6 +295,10 @@ class MASRPredictor:
             raise Exception(f'不支持该数据类型，当前数据类型为：{type(audio_data)}')
         self._check_rate(sample_rate)
         self.remained_wav = new if self.remained_wav is None else np.concatenate([self.remained_wav, new])
+        if sample_rate != self._sample_rate:
+            # predict.py:267-274: the buffer (the carried-over tail, already at 16 kHz, plus the new chunk) is labelled with
+            # the chunk's rate and resampled as a whole on every push, as the reference does
+            self.remained_wav = self.predictor.resample([self.remained_wav], [sample_rate])[0]
 
         # featurise everything not yet consumed; the reference dB-normalises the remainder IN PLACE on
         # every push (predict.py:274 + audio_featurizer.py:49-50), so the carried-over tail keeps the gain
@@ -358,7 +367,7 @@ class MASRPredictor:
             raise Exception(f"不支持改该模型流式识别，当前模型：{self.configs.use_model}，参数streaming为：{self.configs.streaming}")
         from .stream_pool import StreamPool
         return StreamPool(self.predictor, self._text_featurizer.vocab_list, n_slots, use_db_normalization=self._use_db,
-                          target_db=self._target_db, max_frames=max_frames, beam=self._beam_conf)
+                          target_db=self._target_db, max_frames=max_frames, beam=self._beam_conf, resample=self._resample)
 
     def reset_stream(self):
         """predict.py:346-353."""

@@ -23,6 +23,7 @@ from ._lib import EPI_BIAS, EPI_BIAS_GLU, EPI_BIAS_SCALE, EPI_BIAS_SILU, EPI_RES
 from .audio import pcm_bytes_to_float32, samples_to_float32
 from .engine import ConformerEngine, _p, greedy_score, subsampled_len
 from .predict import CACHED_FEATURE_NUM, DECODING_WINDOW, FRAME_SHIFT, chunk_starts
+from .resample import MODEL_RATE, output_length
 from .text import ids_to_text
 
 CHUNK_FRAMES = DECODING_WINDOW          # 67 feature frames -> 16 encoder frames
@@ -669,13 +670,16 @@ class StreamPool:
     RING = 1024                    # feature frames kept per slot (un-consumed frames never exceed one push + one window)
 
     def __init__(self, eng: ConformerEngine, vocab: Sequence[str], n_slots: int, use_db_normalization: bool = True,
-                 target_db: float = -20.0, max_frames: int = 3000, beam: Optional[dict] = None, use_graph: bool = True):
+                 target_db: float = -20.0, max_frames: int = 3000, beam: Optional[dict] = None, use_graph: bool = True,
+                 resample: bool = False):
         """``beam``: None decodes greedily (``ctc_greedy``); a dict ``{beam_size, cutoff_prob, cutoff_top_n, lm, alpha,
         beta}`` (``MASRPredictor``'s ``ctc_beam_search`` settings; ``lm`` a ``CharLM`` or None) runs the streaming prefix
         beam search of every slot on the GPU (``PoolBeam``), and every result is the beam's, as ``predict_stream`` with
         ``decoder: ctc_beam_search`` returns it.  ``use_graph=False`` launches every step eagerly instead of replaying
-        its CUDA graph (same results)."""
+        its CUDA graph (same results).  ``resample``: accept pushes at other sample rates (``push(..., sample_rate=)``) and
+        resample them on the GPU as ``predict_stream`` does; False makes such a push a per-slot error."""
         self.eng, self.vocab, self.S = eng, list(vocab), n_slots
+        self.resample = bool(resample)
         self.pool = make_pool(eng, n_slots, max_frames)
         if not use_graph:
             self.pool.use_graph = False
@@ -760,9 +764,10 @@ class StreamPool:
         self.ring, self.RING = ring, R1
 
     def push(self, audio: Dict[int, object], is_end: bool = False, channels: int = 1, samp_width: int = 2,
-             on_error: str = "raise"):
+             on_error: str = "raise", sample_rate=MODEL_RATE):
         """audio: slot -> np.ndarray | PCM bytes (one push per slot).  -> slot -> {'text','score'} | None, exactly what
-        ``MASRPredictor.predict_stream(chunk, is_end)`` would return for that stream.
+        ``MASRPredictor.predict_stream(chunk, is_end, sample_rate=...)`` would return for that stream.  ``sample_rate``: one
+        rate for every slot, or a ``{slot: rate}`` dict (missing slots: 16 kHz); off 16 kHz needs ``resample=True``.
 
         Per-slot isolation: every slot is validated (decodable input, gain within 300 dB, pool / position-table capacity,
         no chunk after a short final chunk) BEFORE any state changes; a slot that fails keeps its previous state, is left
@@ -782,6 +787,24 @@ class StreamPool:
                 errors[s] = e
                 continue
             cand[s] = new if self.remained[s] is None else np.concatenate([self.remained[s], new])
+        rates = {s: int(sample_rate.get(s, MODEL_RATE) if isinstance(sample_rate, dict) else sample_rate) for s in cand}
+        off = []
+        for s in sorted(cand):
+            if rates[s] == MODEL_RATE:
+                continue
+            try:
+                if not self.resample:
+                    raise Exception(f"masr_b200: resampling is off for this pool (got {rates[s]} Hz, model expects "
+                                    f"{MODEL_RATE} Hz)")
+                output_length(len(cand[s]), rates[s])
+                off.append(s)
+            except Exception as e:                    # rate not accepted, or too few samples to resample: this slot only
+                errors[s] = e
+                del cand[s]
+        if off:
+            # predict.py:267-274 per slot: the carried-over tail plus the new chunk, labelled with the chunk's rate, resampled
+            for s, y in zip(off, eng.resample([cand[s] for s in off], [rates[s] for s in off])):
+                cand[s] = y
         slots = sorted(cand)
         out: Dict[int, Optional[dict]] = {}
         if slots:
