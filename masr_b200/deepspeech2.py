@@ -79,13 +79,17 @@ def pack_deepspeech2(sd: Dict[str, torch.Tensor], device) -> DS2Weights:
 
 
 class DeepSpeech2Stream:
-    """(h, c) of the 5 LSTM layers carried between chunks (inference_predictor.py:45-46,97-99)."""
+    """(h, c) of the 5 LSTM layers carried between chunks (inference_predictor.py:45-46,97-99), for `n` streams side by side
+    (one for ``predict_stream``, one per slot for ``DeepSpeech2StreamPool``): stream s is lane s % 32 of lane group s // 32
+    of every layer's h, in the kernels' transposed layout ``[ceil(n/32)][H][32]``, and row s of every layer's c ``[n][H]``.
+    ``hT[l, cur[l]]`` holds layer l's state; the persistent recurrence updates it in place, the per-step form ping-pongs
+    through ``hT[l, 1 - cur[l]]``."""
 
-    def __init__(self, eng: "DeepSpeech2Engine"):
+    def __init__(self, eng: "DeepSpeech2Engine", n: int = 1):
         self.eng = eng
         H, nl = eng.H, len(eng.w.rnn)
-        self.hT = torch.zeros(nl, 2, H, 32, device=eng.device, dtype=torch.float32)   # ping-pong, transposed [H][32]
-        self.c = torch.zeros(nl, 1, H, device=eng.device, dtype=torch.float32)
+        self.hT = torch.zeros(nl, 2, (n + 31) // 32, H, 32, device=eng.device, dtype=torch.float32)
+        self.c = torch.zeros(nl, n, H, device=eng.device, dtype=torch.float32)
         self.cur = [0] * nl
 
     def reset(self):
@@ -126,6 +130,14 @@ class DeepSpeech2Engine(ConformerEngine):
         ws = self._ws.get(key)
         if ws is not None:
             return ws
+        ws = self._alloc_workspace(B, Fmax)
+        if len(self._ws) > 8:
+            self._ws.clear()
+        self._ws[key] = ws
+        return ws
+
+    def _alloc_workspace(self, B: int, Fmax: int):
+        """The device buffers of one (B, Fmax) pass, owned by the caller (``_workspace`` caches them per shape)."""
         dev, f32, f16 = self.device, torch.float32, torch.float16
         F1 = (Fmax - 1) // 2
         T = subsampled_len(Fmax)
@@ -148,9 +160,6 @@ class DeepSpeech2Engine(ConformerEngine):
         }
         self._alloc_out_pack(ws, B, T)
         ws["t0p"] = ws["xp"]
-        if len(self._ws) > 8:
-            self._ws.clear()
-        self._ws[key] = ws
         return ws
 
     # ------------------------------------------------------------------------------------------------
@@ -171,16 +180,17 @@ class DeepSpeech2Engine(ConformerEngine):
                     c.zero_()
                     cur = 0
                 else:
-                    hT, c, cur = stream.hT[l].unsqueeze(1), stream.c[l], stream.cur[l]
+                    hT, c, cur = stream.hT[l], stream.c[l], stream.cur[l]
                 if self.persistent_lstm and H % 128 == 0 and H <= 1024:
-                    # the whole recurrence of this layer / direction in one persistent launch (W_hh slices resident in shared memory)
+                    # the whole recurrence of this layer / direction in one persistent launch (W_hh slices resident in shared memory).
+                    # The state is updated in place (h0_T == hN_T), so it never changes buffers: a captured pool step reads in the
+                    # next replay what it wrote in this one.
                     if ws.get("lstm_ws") is None:
                         nbytes = _lib.C.c_int64(0)
                         call("masr_lstm_seq_workspace_bytes", B, H, _lib.C.byref(nbytes))
                         ws["lstm_ws"] = torch.empty(nbytes.value, device=self.device, dtype=torch.uint8)
-                    self._k("lstm_seq", "masr_lstm_seq_f32", _p(gx), 4 * H, T, _p(ent["whh"][di]), _p(hT[cur]), _p(hT[1 - cur]), _p(c),
+                    self._k("lstm_seq", "masr_lstm_seq_f32", _p(gx), 4 * H, T, _p(ent["whh"][di]), _p(hT[cur]), _p(hT[cur]), _p(c),
                             _p(out), None, None, D, di * H, _p(tlens), B, H, T, di, _p(ws["lstm_ws"]), ws["lstm_ws"].numel())
-                    cur = 1 - cur
                 else:
                     for s in range(T):
                         self._k("lstm_step", "masr_lstm_step_f32", _p(gx), 4 * H, T, _p(ent["whh"][di]), _p(hT[cur]), _p(hT[1 - cur]),
@@ -229,10 +239,11 @@ class DeepSpeech2Engine(ConformerEngine):
         return ws["logits"]
 
     # ---- streaming ----------------------------------------------------------------------------------
-    def new_stream(self) -> DeepSpeech2Stream:
+    def new_stream(self, n: int = 1) -> DeepSpeech2Stream:
+        """The carried LSTM state of `n` streams (``DeepSpeech2StreamPool`` keeps one for all its slots)."""
         if self.dirs != 1:
             raise Exception("chunk decoding needs a streaming (forward-only) model")
-        return DeepSpeech2Stream(self)
+        return DeepSpeech2Stream(self, n)
 
     def encode_chunk(self, feats_chunk: torch.Tensor, st: DeepSpeech2Stream, required_cache_size: int = -1,
                      want_probs: bool = False):
@@ -248,9 +259,15 @@ class DeepSpeech2Engine(ConformerEngine):
             ws["tl_host"] = [T]
         self._front(feats_chunk.reshape(1, n, -1), ws, 1, n, (n - 1) // 2, T)
         self._rnn_stack(ws, 1, T, T, ws["tlens"], stream=st)
-        logits = self.ctc_logits(ws["t0"][:T], ws)
         probs = torch.empty(T, self.V, device=self.device, dtype=torch.float32) if want_probs else None
-        self._k("ctc_argmax", "masr_ctc_frame_argmax_f32", _p(logits), self.Vpad, T, self.V, _p(ws["ids"]), _p(ws["maxp"]),
-                _p(probs), self.V)
+        logits = self._ctc_argmax(ws, T, probs)
         st.last_logits = logits[:T]                    # (the streaming beam search reads the chunk's logits)
         return ws["ids"][:T], ws["maxp"][:T], probs
+
+    def _ctc_argmax(self, ws, M: int, probs: Optional[torch.Tensor] = None):
+        """CTC head over the M rows of the last LayerNorm output, then per row the argmax id and its probability (and the
+        posteriors into `probs` [M, V] when given) -> the logits [M, Vpad]."""
+        logits = self.ctc_logits(ws["t0"][:M], ws)
+        self._k("ctc_argmax", "masr_ctc_frame_argmax_f32", _p(logits), self.Vpad, M, self.V, _p(ws["ids"]), _p(ws["maxp"]),
+                _p(probs), self.V)
+        return logits

@@ -1,4 +1,5 @@
-"""Many live streams on one GPU: batched chunk decoding for the streaming Conformer, Squeezeformer and EfficientConformer.
+"""Many live streams on one GPU: batched chunk decoding for the streaming Conformer, Squeezeformer, EfficientConformer and
+DeepSpeech2 (``DeepSpeech2StreamPool``: every slot's LSTM state advanced in one pass per layer).
 
 The reference's streaming API is one stream per ``MASRPredictor`` (predict.py:237-343; ``forward_chunk`` asserts
 batch 1, conformer/encoder.py:378) and `infer_server.py` effectively serves one stream at a time.  BASELINE.json
@@ -68,15 +69,22 @@ class _PoolBase:
     def _m(self, row):
         return self.meta[row].data_ptr()
 
+    def frame_bounds(self):
+        """(cap, max_len): a slot may hold at most `cap` encoder frames since its reset (its K|V cache rows), and fewer than
+        `max_len` (the rows of the engine's relative-position table).  None: no such bound."""
+        return self.cap, self.eng.w.max_len
+
     def _prepare(self, nframes: Sequence[int], short_ok_once: bool):
         eng, S, C = self.eng, self.S, CHUNK_OUT
         tout = [subsampled_len(int(n)) for n in nframes]
         tout2 = [(t + 1) // 2 for t in tout]
+        cap, max_len = self.frame_bounds()
         for s in range(S):
             if short_ok_once and tout[s] and self.lens_host[s] % C:
                 raise AssertionError(f"stream slot {s}: a short (final) chunk was already decoded; reset the stream first")
-            if self.lens_host[s] + tout[s] > self.cap or self.lens_host[s] + tout[s] >= eng.w.max_len:
-                raise AssertionError(f"stream slot {s}: {self.lens_host[s] + tout[s]} cached frames exceed the pool capacity")
+            n = self.lens_host[s] + tout[s]
+            if (cap is not None and n > cap) or (max_len is not None and n >= max_len):
+                raise AssertionError(f"stream slot {s}: {n} cached frames exceed the pool capacity")
         if self._meta_ev is not None:
             self._meta_ev.synchronize()
         mh = self.meta_host.numpy()
@@ -521,6 +529,49 @@ class EfficientConformerStreamPool(_PoolBase):
         eng._k("ctc_argmax", "masr_ctc_frame_argmax_f32", _p(b["logits"]), eng.Vpad, M2, eng.V, _p(b["ids"]), _p(b["maxp"]), _p(self.probs), eng.V)
 
 
+class DeepSpeech2StreamPool(_PoolBase):
+    """Batched chunk decoding for the streaming (forward-only) DeepSpeech2 (``DeepSpeech2Model.get_encoder_out_chunk``,
+    masr/model_utils/deepspeech2/model.py:70-77, with the (h, c) state carried as inference_predictor.py:66-78 does).
+
+    One step is the launch sequence of ``DeepSpeech2Engine.encode_chunk`` over every slot at once (M = slots x 16 rows):
+    CMVN + conv1, conv2, per layer the input projection, the recurrence (16 steps over the `meta` lengths row: a lane past
+    its slot's valid frames is frozen, so an idle slot keeps its state byte for byte) and the LayerNorm, then the CTC head
+    and argmax.  No stage's result for a row or lane depends on the batch, so every slot equals ``encode_chunk`` on a
+    ``DeepSpeech2Stream`` bit for bit.  The state of all slots is one ``DeepSpeech2Stream`` in pool-owned buffers that stay
+    put across rounds, as a CUDA graph replay needs: the persistent recurrence updates it in place, and the per-step form
+    (``MASR_LSTM_PERSISTENT=0``) ping-pongs 16 times per round, so it ends where it started.
+
+    The persistent recurrence needs all its H / 8 CTAs co-resident (a grid barrier per step).  The pool launches on the
+    engine's stream like every other engine call; do not run its steps on a second stream beside another persistent launch.
+
+    There is no position table and the state has a constant size, so a greedy slot decodes any length; with a beam search
+    attached, `max_frames` sizes each slot's prefix trie and bounds the slot.  A short chunk may be followed by more."""
+
+    SHORT_ONCE = False
+
+    def __init__(self, eng, n_slots: int, max_frames: int = 3000, use_graph: bool = True, keep_probs: bool = False):
+        self.state = eng.new_stream(n_slots)
+        self._init_common(eng, n_slots, use_graph, keep_probs)
+        self.cap = max_frames
+        # pool-owned (not the engine's per-shape cache, which frees buffers a captured step still uses)
+        self.b = eng._alloc_workspace(n_slots, CHUNK_FRAMES)
+
+    def frame_bounds(self):
+        return (self.cap if self.beam is not None else None), None
+
+    def reset(self, slot: int):
+        """``InferencePredictor.reset_stream`` for one slot: zero state (inference_predictor.py:97-99)."""
+        self.lens_host[slot] = 0
+        self.state.hT[:, :, slot // 32, :, slot % 32].zero_()
+        self.state.c[:, slot].zero_()
+
+    def _body(self):
+        eng, S, C, ws = self.eng, self.S, CHUNK_OUT, self.b
+        eng._front(self.feats_in, ws, S, CHUNK_FRAMES, (CHUNK_FRAMES - 1) // 2, C)
+        eng._rnn_stack(ws, S, C, S * C, self.meta[self.QLEN], stream=self.state)
+        eng._ctc_argmax(ws, S * C, self.probs)
+
+
 class PoolStream:
     """One stream = a one-slot pool behind the single-stream interface ``MASRPredictor.predict_stream`` uses
     (``eng.new_stream()`` / ``eng.encode_chunk(chunk, stream)``)."""
@@ -550,8 +601,11 @@ class PoolStream:
 
 def make_pool(eng, n_slots: int, max_frames: int = 3000):
     """The batched chunk-decoding pool that matches the engine's model family."""
+    from .deepspeech2 import DeepSpeech2Engine
     from .engine import EfficientConformerEngine
     from .squeezeformer import SqueezeformerEngine
+    if isinstance(eng, DeepSpeech2Engine):
+        return DeepSpeech2StreamPool(eng, n_slots, max_frames)
     if isinstance(eng, SqueezeformerEngine):
         return SqueezeformerStreamPool(eng, n_slots, max_frames)
     if isinstance(eng, EfficientConformerEngine):
@@ -814,9 +868,8 @@ class StreamPool:
             status_h = status.cpu().numpy()
             Fmax = feats.shape[1]
             pool = self.pool
-            cap = getattr(pool, "cap", None)
-            max_len = getattr(getattr(eng, "w", None), "max_len", None)
             lens_host = getattr(pool, "lens_host", None)
+            cap, max_len = pool.frame_bounds() if lens_host is not None else (None, None)
             short_once = bool(getattr(pool, "SHORT_ONCE", False))
             good, pending = [], {}
             for j, s in enumerate(slots):

@@ -1,7 +1,8 @@
 """Dev tool / BASELINE.json config 3: `configs/squeezeformer.yml` streaming, N live streams (default 64), every stream pushes
 0.5 s (8000-sample) int16 PCM chunks; `StreamPool.push` = the `predict_stream` semantics of the reference for every stream
 (67-frame windows, stride 64, greedy) with one batched chunk step per round.  Prints one JSON line: audio-s/s, per-push
-latency (ms), launches per push.  Also runs the Conformer with --model conformer.  Synthetic audio + weights.
+latency (ms), launches per push.  Also runs the Conformer, the EfficientConformer and the DeepSpeech2 with --model.
+Synthetic audio + weights.
 
 --decoder ctc_beam_search decodes every slot with the GPU prefix beam search (``StreamPool(beam=...)``; --beam-size, and
 --lm-order N fuses a synthetic N-gram character ARPA LM from ``synth.character_lm_arpa``).  The beam kernels' time per
@@ -20,7 +21,7 @@ from masr_b200 import synth
 from masr_b200.stream_pool import StreamPool
 
 ap = argparse.ArgumentParser()
-ap.add_argument("--model", default="squeezeformer", choices=["squeezeformer", "conformer", "efficient_conformer"])
+ap.add_argument("--model", default="squeezeformer", choices=["squeezeformer", "conformer", "efficient_conformer", "deepspeech2"])
 ap.add_argument("--streams", type=int, default=64)
 ap.add_argument("--pushes", type=int, default=40)
 ap.add_argument("--warm", type=int, default=6)
@@ -40,6 +41,9 @@ if args.model == "squeezeformer":
 elif args.model == "efficient_conformer":
     from masr_b200.engine import EfficientConformerEngine
     eng = EfficientConformerEngine(synth.efficient_conformer_state_dict(0), streaming=True)
+elif args.model == "deepspeech2":
+    from masr_b200.deepspeech2 import DeepSpeech2Engine
+    eng = DeepSpeech2Engine(synth.deepspeech2_state_dict(0, streaming=True), streaming=True)
 else:
     from masr_b200.engine import ConformerEngine
     eng = ConformerEngine(synth.conformer_state_dict(0), streaming=True)
