@@ -315,6 +315,22 @@ int masr_lstm_seq_f32(const float* gates_x, int64_t ldg, int64_t bstride, const 
                       float* c_state, float* out, void* outh, void* outl, int64_t ld_out, int col_off, const int* lens, int B,
                       int H, int T, int reverse, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* The GRU forms of the two entry points above, for DeepSpeech2 with use_gru: True (masr/model_utils/deepspeech2/encoder.py:
+ * 24-33 -> gru.py:6-22, torch.nn.GRU, gate order r, z, n).  Same arguments as their LSTM counterparts except that there is
+ * no c_state (a GRU carries h only) and b_hn [H] takes its place: gates_x [., 3H] = W_ih x + b_ih + [b_hr, b_hz, 0];
+ * Whh [3H, H];
+ *     r = sigmoid(gx_r + W_hr h) ; z = sigmoid(gx_z + W_hz h) ; n = tanh(gx_n + r * (W_hn h + b_hn)) ; h' = n + z (h - n)
+ * (b_hn stays inside the product with r, so it cannot be folded into gates_x).  The persistent form keeps the three gate rows
+ * of 8 hidden units resident (96 KB at H = 1024) and uses the same workspace layout as masr_lstm_seq_f32, so
+ * masr_lstm_seq_workspace_bytes sizes it too.  masr_gru_step_f32: H % 4 == 0, in != out; masr_gru_seq_f32: H % 128 == 0,
+ * H <= 1024, H / 8 CTAs co-resident (h0_T == hN_T allowed). */
+int masr_gru_step_f32(const float* gates_x, int64_t ldg, int64_t bstride, const float* Whh, const float* h_in_T,
+                      float* h_out_T, const float* bhn, float* out, void* outh, void* outl, int64_t ld_out, int col_off,
+                      const int* lens, int B, int H, int step, int reverse, void* stream);
+int masr_gru_seq_f32(const float* gates_x, int64_t ldg, int64_t bstride, const float* Whh, const float* h0_T, float* hN_T,
+                     const float* bhn, float* out, void* outh, void* outl, int64_t ld_out, int col_off, const int* lens, int B,
+                     int H, int T, int reverse, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- batched chunk (streaming) state ------------------------------------------------------------ */
 
 /* Append the chunk's new rows to every slot's cache (the `torch.cat` on time of the attention K|V cache, conformer/

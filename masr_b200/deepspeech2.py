@@ -1,9 +1,11 @@
 """DeepSpeech2 engine (configs/deepspeech2.yml; masr/model_utils/deepspeech2/{conv,encoder,model}.py):
-CMVN -> Conv2d(1,32,3,2)+ReLU -> Conv2d(32,32,3,2)+ReLU -> 5 x [LSTM(1024) uni (streaming) / bi -> LayerNorm] -> CTC.
+CMVN -> Conv2d(1,32,3,2)+ReLU -> Conv2d(32,32,3,2)+ReLU -> 5 x [LSTM(1024) or GRU(1024) (use_gru), uni (streaming) / bi ->
+LayerNorm] -> CTC.
 
 Input projections and the CTC head are tensor-core GEMMs (FP16x2 split); the first projection (K = 608) and the
-recurrence run on the fp32 FMA pipe, one launch per time step (replayed as a CUDA graph).  Whole-utterance batches and
-the chunked streaming path with carried (h, c) state (inference_predictor.py:66-78) are both implemented."""
+recurrence run on the fp32 FMA pipe, one persistent launch per layer and direction (or one launch per time step).
+Whole-utterance batches and the chunked streaming path with carried state (inference_predictor.py:66-78: (h, c) for the
+LSTM, h for the GRU) are both implemented.  The cell type comes from the weights, as in the reference."""
 from __future__ import annotations
 
 import os
@@ -37,6 +39,9 @@ class DS2Weights:
     conv2_b: torch.Tensor = None
     layers: list = field(default_factory=list)      # unused (ConformerEngine plumbing)
     rnn: List[dict] = field(default_factory=list)   # per layer: {"wih": [dirs], "whh": [dirs], "bias": [dirs], "ln": (g, b)}
+                                                    # (+ "bhn": [dirs] for the GRU)
+    cell: str = "lstm"                              # "lstm" or "gru" (encoder_conf.use_gru)
+    gates: int = 4                                  # gate rows per hidden unit: 4 (LSTM) / 3 (GRU)
     ctc_w: torch.Tensor = None
     ctc_b: torch.Tensor = None
     pe: torch.Tensor = None
@@ -52,26 +57,37 @@ def pack_deepspeech2(sd: Dict[str, torch.Tensor], device) -> DS2Weights:
     C = sd["encoder.conv.conv.0.weight"].shape[0]
     from .weights import check_supported
     check_supported(sd, "deepspeech2")
-    H = sd["encoder.rnns.0.rnn.weight_hh_l0"].shape[1]
-    dirs = 2 if "encoder.rnns.0.rnn.weight_hh_l0_reverse" in sd else 1
+    gru = "encoder.rnns.0.rnn.rnn.weight_hh_l0" in sd       # the reference's GRU wrapper (gru.py:6-15)
+    rp = "rnn.rnn." if gru else "rnn."
+    G = 3 if gru else 4
+    H = sd[f"encoder.rnns.0.{rp}weight_hh_l0"].shape[1]
+    dirs = 2 if f"encoder.rnns.0.{rp}weight_hh_l0_reverse" in sd else 1
     nl = 1 + max(int(k.split(".")[2]) for k in sd if k.startswith("encoder.rnns."))
     vocab = sd["decoder.ctc_lo.weight"].shape[0]
-    w = DS2Weights(d_model=H * dirs, heads=1, ffn=0, kernel=0, idim=idim, vocab=vocab, max_len=0, hidden=H, dirs=dirs)
+    w = DS2Weights(d_model=H * dirs, heads=1, ffn=0, kernel=0, idim=idim, vocab=vocab, max_len=0, hidden=H, dirs=dirs,
+                   cell="gru" if gru else "lstm", gates=G)
     w.cmvn_mean, w.cmvn_istd = D(sd["encoder.global_cmvn.mean"]), D(sd["encoder.global_cmvn.istd"])
     w.conv1_w, w.conv1_b = D(sd["encoder.conv.conv.0.weight"].reshape(C, 9)), D(sd["encoder.conv.conv.0.bias"])
     w.conv2_w = D(sd["encoder.conv.conv.2.weight"].permute(0, 2, 3, 1).reshape(C, 9 * C))
     w.conv2_b = D(sd["encoder.conv.conv.2.bias"])
     f2 = ((idim - 1) // 2 - 1) // 2
     for l in range(nl):
-        p = f"encoder.rnns.{l}.rnn."
+        p = f"encoder.rnns.{l}.{rp}"
         ent = {"wih": [], "whh": [], "bias": []}
+        if gru:
+            ent["bhn"] = []
         for suf in ("", "_reverse")[:dirs]:
             wih = sd[p + "weight_ih_l0" + suf]
             if l == 0:   # conv output is channels-last here: permute the (c*19+f) input columns to (f*32+c)
-                wih = wih.reshape(4 * H, C, f2).permute(0, 2, 1).reshape(4 * H, f2 * C)
+                wih = wih.reshape(G * H, C, f2).permute(0, 2, 1).reshape(G * H, f2 * C)
             ent["wih"].append(D(wih))
             ent["whh"].append(D(sd[p + "weight_hh_l0" + suf]))
-            ent["bias"].append(D(sd[p + "bias_ih_l0" + suf] + sd[p + "bias_hh_l0" + suf]))
+            bih, bhh = sd[p + "bias_ih_l0" + suf], sd[p + "bias_hh_l0" + suf]
+            if gru:      # b_hr, b_hz fold into the input projection; b_hn is multiplied by r inside the cell
+                ent["bias"].append(D(bih + torch.cat([bhh[:2 * H], torch.zeros_like(bhh[2 * H:])])))
+                ent["bhn"].append(D(bhh[2 * H:]))
+            else:
+                ent["bias"].append(D(bih + bhh))
         ent["ln"] = (D(sd[f"encoder.rnns.{l}.layer_norm.weight"]), D(sd[f"encoder.rnns.{l}.layer_norm.bias"]))
         w.rnn.append(ent)
     w.ctc_w, w.ctc_b = D(sd["decoder.ctc_lo.weight"]), D(sd["decoder.ctc_lo.bias"])
@@ -79,9 +95,10 @@ def pack_deepspeech2(sd: Dict[str, torch.Tensor], device) -> DS2Weights:
 
 
 class DeepSpeech2Stream:
-    """(h, c) of the 5 LSTM layers carried between chunks (inference_predictor.py:45-46,97-99), for `n` streams side by side
-    (one for ``predict_stream``, one per slot for ``DeepSpeech2StreamPool``): stream s is lane s % 32 of lane group s // 32
-    of every layer's h, in the kernels' transposed layout ``[ceil(n/32)][H][32]``, and row s of every layer's c ``[n][H]``.
+    """The recurrent state of the 5 layers carried between chunks (inference_predictor.py:45-46,97-99), for `n` streams side
+    by side (one for ``predict_stream``, one per slot for ``DeepSpeech2StreamPool``): stream s is lane s % 32 of lane group
+    s // 32 of every layer's h, in the kernels' transposed layout ``[ceil(n/32)][H][32]``, and for the LSTM row s of every
+    layer's c ``[n][H]``.  A GRU carries h only (its c is h again, gru.py:21), so ``c`` is None for a GRU model.
     ``hT[l, cur[l]]`` holds layer l's state; the persistent recurrence updates it in place, the per-step form ping-pongs
     through ``hT[l, 1 - cur[l]]``."""
 
@@ -89,12 +106,13 @@ class DeepSpeech2Stream:
         self.eng = eng
         H, nl = eng.H, len(eng.w.rnn)
         self.hT = torch.zeros(nl, 2, (n + 31) // 32, H, 32, device=eng.device, dtype=torch.float32)
-        self.c = torch.zeros(nl, n, H, device=eng.device, dtype=torch.float32)
+        self.c = torch.zeros(nl, n, H, device=eng.device, dtype=torch.float32) if eng.w.cell == "lstm" else None
         self.cur = [0] * nl
 
     def reset(self):
         self.hT.zero_()
-        self.c.zero_()
+        if self.c is not None:
+            self.c.zero_()
         self.cur = [0] * len(self.cur)
 
 
@@ -106,10 +124,14 @@ class DeepSpeech2Engine(ConformerEngine):
         super().__init__(weights_src, streaming, device, max_len, gemm, use_graphs)
         self.H = self.w.hidden
         self.dirs = self.w.dirs
-        # one persistent launch per layer and direction (masr_lstm_seq_f32) instead of one launch per time step
+        # one persistent launch per layer and direction (masr_lstm_seq_f32 / masr_gru_seq_f32) instead of one launch per
+        # time step; the switch covers both cells
         self.persistent_lstm = os.environ.get("MASR_LSTM_PERSISTENT", "1") != "0"
         if bool(streaming) != (self.dirs == 1):
-            raise Exception("streaming DeepSpeech2 needs forward-only LSTM weights, non-streaming bidirectional ones")
+            raise Exception("streaming DeepSpeech2 needs forward-only recurrent weights, non-streaming bidirectional ones")
+        self.G = self.w.gates
+        self._seq_fn, self._step_fn = (("masr_gru_seq_f32", "masr_gru_step_f32") if self.w.cell == "gru" else
+                                       ("masr_lstm_seq_f32", "masr_lstm_step_f32"))
 
     def _pack(self, sd, max_len):
         return pack_deepspeech2(sd, self.device)
@@ -148,12 +170,12 @@ class DeepSpeech2Engine(ConformerEngine):
         ws = {
             "c1": torch.empty(B * max(1, F1) * self.w1_cols * C, device=dev, dtype=f32),
             "c2": torch.empty(M, self.f2 * C, device=dev, dtype=f32),
-            "gx": torch.empty(M, 4 * self.H, device=dev, dtype=f32),
+            "gx": torch.empty(M, self.G * self.H, device=dev, dtype=f32),
             "out": torch.zeros(M, D, device=dev, dtype=f32),
             "t0": torch.empty(M, D, device=dev, dtype=f32),
             "xp": (torch.empty(M, D, device=dev, dtype=f16), torch.empty(M, D, device=dev, dtype=f16)),
             "hT": torch.zeros(2, nb, self.H, 32, device=dev, dtype=f32),
-            "c": torch.zeros(B, self.H, device=dev, dtype=f32),
+            "c": torch.zeros(B, self.H, device=dev, dtype=f32) if self.w.cell == "lstm" else None,
             "logits": torch.empty(M, self.Vpad, device=dev, dtype=f32),
             "ids": torch.empty(M, device=dev, dtype=torch.int32),
             "maxp": torch.empty(M, device=dev, dtype=f32),
@@ -165,22 +187,26 @@ class DeepSpeech2Engine(ConformerEngine):
     # ------------------------------------------------------------------------------------------------
     def _rnn_stack(self, ws, B, T, M, tlens, hT_init=None, c_init=None, stream: Optional[DeepSpeech2Stream] = None):
         """x = ws['c2'] [M, 608] -> ws['xp'] pair of the last LayerNorm output (and ws['t0'] fp32)."""
-        w, H, dirs, D = self.w, self.H, self.dirs, self.H * self.dirs
+        w, H, dirs, D, GH = self.w, self.H, self.dirs, self.H * self.dirs, self.G * self.H
         out, gx, xp = ws["out"], ws["gx"], ws["xp"]
         for l, ent in enumerate(w.rnn):
             for di in range(dirs):
                 if l == 0:
                     K0 = ws["c2"].shape[1]
-                    self._gemm(ws["c2"], K0, ent["wih"][di], ent["bias"][di], gx, 4 * H, M, 4 * H, K0, EPI_BIAS, tag="lstm_xproj")
+                    self._gemm(ws["c2"], K0, ent["wih"][di], ent["bias"][di], gx, GH, M, GH, K0, EPI_BIAS, tag="lstm_xproj")
                 else:
-                    self._tc(xp, D, self._tcw[l, "wih"][di], ent["bias"][di], M, 4 * H, D, EPI_BIAS, C=gx, ldc=4 * H, tag="lstm_xproj")
+                    self._tc(xp, D, self._tcw[l, "wih"][di], ent["bias"][di], M, GH, D, EPI_BIAS, C=gx, ldc=GH, tag="lstm_xproj")
                 if stream is None:
                     hT, c = ws["hT"], ws["c"]
                     hT.zero_()
-                    c.zero_()
+                    if c is not None:
+                        c.zero_()
                     cur = 0
                 else:
-                    hT, c, cur = stream.hT[l], stream.c[l], stream.cur[l]
+                    hT, cur = stream.hT[l], stream.cur[l]
+                    c = None if stream.c is None else stream.c[l]
+                # the cell's per-unit operand: the LSTM's cell state c [B][H] (updated in place), the GRU's b_hn [H]
+                aux = ent["bhn"][di] if w.cell == "gru" else c
                 if self.persistent_lstm and H % 128 == 0 and H <= 1024:
                     # the whole recurrence of this layer / direction in one persistent launch (W_hh slices resident in shared memory).
                     # The state is updated in place (h0_T == hN_T), so it never changes buffers: a captured pool step reads in the
@@ -189,12 +215,12 @@ class DeepSpeech2Engine(ConformerEngine):
                         nbytes = _lib.C.c_int64(0)
                         call("masr_lstm_seq_workspace_bytes", B, H, _lib.C.byref(nbytes))
                         ws["lstm_ws"] = torch.empty(nbytes.value, device=self.device, dtype=torch.uint8)
-                    self._k("lstm_seq", "masr_lstm_seq_f32", _p(gx), 4 * H, T, _p(ent["whh"][di]), _p(hT[cur]), _p(hT[cur]), _p(c),
+                    self._k(f"{w.cell}_seq", self._seq_fn, _p(gx), GH, T, _p(ent["whh"][di]), _p(hT[cur]), _p(hT[cur]), _p(aux),
                             _p(out), None, None, D, di * H, _p(tlens), B, H, T, di, _p(ws["lstm_ws"]), ws["lstm_ws"].numel())
                 else:
                     for s in range(T):
-                        self._k("lstm_step", "masr_lstm_step_f32", _p(gx), 4 * H, T, _p(ent["whh"][di]), _p(hT[cur]), _p(hT[1 - cur]),
-                                _p(c), _p(out), None, None, D, di * H, _p(tlens), B, H, s, di)
+                        self._k(f"{w.cell}_step", self._step_fn, _p(gx), GH, T, _p(ent["whh"][di]), _p(hT[cur]), _p(hT[1 - cur]),
+                                _p(aux), _p(out), None, None, D, di * H, _p(tlens), B, H, s, di)
                         cur = 1 - cur
                 if stream is not None:
                     stream.cur[l] = cur
@@ -240,7 +266,7 @@ class DeepSpeech2Engine(ConformerEngine):
 
     # ---- streaming ----------------------------------------------------------------------------------
     def new_stream(self, n: int = 1) -> DeepSpeech2Stream:
-        """The carried LSTM state of `n` streams (``DeepSpeech2StreamPool`` keeps one for all its slots)."""
+        """The carried recurrent state of `n` streams (``DeepSpeech2StreamPool`` keeps one for all its slots)."""
         if self.dirs != 1:
             raise Exception("chunk decoding needs a streaming (forward-only) model")
         return DeepSpeech2Stream(self, n)
@@ -248,7 +274,7 @@ class DeepSpeech2Engine(ConformerEngine):
     def encode_chunk(self, feats_chunk: torch.Tensor, st: DeepSpeech2Stream, required_cache_size: int = -1,
                      want_probs: bool = False):
         """``DeepSpeech2Model.get_encoder_out_chunk`` for one stream (model.py:70-77): feats [n, 80] on device ->
-        (ids, max-prob[, posteriors]) for ((n-1)//2-1)//2 frames; the LSTM state is carried in ``st``."""
+        (ids, max-prob[, posteriors]) for ((n-1)//2-1)//2 frames; the recurrent state is carried in ``st``."""
         n = int(feats_chunk.shape[0])
         T = subsampled_len(n)
         if T == 0:

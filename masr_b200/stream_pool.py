@@ -563,7 +563,8 @@ class DeepSpeech2StreamPool(_PoolBase):
         """``InferencePredictor.reset_stream`` for one slot: zero state (inference_predictor.py:97-99)."""
         self.lens_host[slot] = 0
         self.state.hT[:, :, slot // 32, :, slot % 32].zero_()
-        self.state.c[:, slot].zero_()
+        if self.state.c is not None:                       # (a GRU carries h only)
+            self.state.c[:, slot].zero_()
 
     def _body(self):
         eng, S, C, ws = self.eng, self.S, CHUNK_OUT, self.b

@@ -202,9 +202,11 @@ def squeezeformer_state_dict(seed: int = 0, vocab_size: int = DEFAULT_VOCAB_SIZE
 
 
 def deepspeech2_state_dict(seed: int = 0, vocab_size: int = DEFAULT_VOCAB_SIZE, streaming: bool = True, input_dim: int = 80,
-                           layers: int = 5, hidden: int = 1024, ctc_gain: float = 4.0, blank_bias: float = 9.0) -> Dict[str, np.ndarray]:
+                           layers: int = 5, hidden: int = 1024, ctc_gain: float = 4.0, blank_bias: float = 9.0,
+                           use_gru: bool = False) -> Dict[str, np.ndarray]:
     """DeepSpeech2 tensors in the reference layout (deepspeech2/{conv,encoder,model}.py): Conv2d(1,32,3,2), Conv2d(32,32,3,2),
-    5 x LSTM(1024) (+ ``_reverse`` weights when not streaming) with LayerNorm, ``decoder.ctc_lo``."""
+    5 x LSTM(1024) (+ ``_reverse`` weights when not streaming) with LayerNorm, ``decoder.ctc_lo``.  ``use_gru``: GRU(1024)
+    layers instead, under the keys the reference's ``GRU`` wrapper gives them (``encoder.rnns.{l}.rnn.rnn.*``, gru.py:6-15)."""
     rng = np.random.default_rng(1300 + seed)
     sd: Dict[str, np.ndarray] = {}
     mean, istd = cmvn_stats(seed, input_dim)
@@ -219,13 +221,14 @@ def deepspeech2_state_dict(seed: int = 0, vocab_size: int = DEFAULT_VOCAB_SIZE, 
     dirs = 1 if streaming else 2
     insz = 32 * f2
     k = 1.0 / math.sqrt(hidden)
+    gates = 3 if use_gru else 4
     for l in range(layers):
-        p = f"encoder.rnns.{l}.rnn."
+        p = f"encoder.rnns.{l}.rnn." + ("rnn." if use_gru else "")
         for suf in ("", "_reverse")[:dirs]:
-            sd[p + "weight_ih_l0" + suf] = _uniform(rng, (4 * hidden, insz), k)
-            sd[p + "weight_hh_l0" + suf] = _uniform(rng, (4 * hidden, hidden), k)
-            sd[p + "bias_ih_l0" + suf] = _uniform(rng, (4 * hidden,), k)
-            sd[p + "bias_hh_l0" + suf] = _uniform(rng, (4 * hidden,), k)
+            sd[p + "weight_ih_l0" + suf] = _uniform(rng, (gates * hidden, insz), k)
+            sd[p + "weight_hh_l0" + suf] = _uniform(rng, (gates * hidden, hidden), k)
+            sd[p + "bias_ih_l0" + suf] = _uniform(rng, (gates * hidden,), k)
+            sd[p + "bias_hh_l0" + suf] = _uniform(rng, (gates * hidden,), k)
         _layer_norm(rng, sd, f"encoder.rnns.{l}.layer_norm", hidden * dirs)
         insz = hidden * dirs
     _linear(rng, sd, "decoder.ctc_lo", vocab_size, hidden * dirs, gain=ctc_gain)

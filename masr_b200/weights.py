@@ -119,8 +119,11 @@ def check_supported(sd: Dict[str, torch.Tensor], family: str = "conformer") -> N
     """Fail loudly on supported-by-the-reference variants this build does not implement, instead of mis-packing them
     (the packers read architecture from tensor names and shapes): ``cnn_module_norm='batch_norm'`` in a Conformer /
     EfficientConformer (convolution.py:60-63: same ``conv_module.norm.weight`` key as the LayerNorm variant, plus running
-    statistics), ``input_layer`` conv2d6 / conv2d8 (subsampling.py:115-236: extra ``embed.conv.4``), GRU recurrences in
-    DeepSpeech2 (deepspeech2/encoder.py:19-33), attention heads that are not 64 wide."""
+    statistics), ``input_layer`` conv2d6 / conv2d8 (subsampling.py:115-236: extra ``embed.conv.4``), attention heads that
+    are not 64 wide.  A DeepSpeech2 checkpoint is an LSTM one (``encoder.rnns.{l}.rnn.*``, 4H gate rows) or a GRU one
+    (``use_gru: True``: the reference's ``GRU`` wrapper nests ``nn.GRU`` one level deeper, ``encoder.rnns.{l}.rnn.rnn.*``,
+    3H gate rows; deepspeech2/encoder.py:24-33, gru.py:6-15); 3H-row tensors under the LSTM names are no layout the
+    reference writes."""
     keys = sd.keys()
     if family in ("conformer", "efficient_conformer") and any(k.endswith("conv_module.norm.running_mean") for k in keys):
         raise UnsupportedConfig("unsupported config: cnn_module_norm='batch_norm' (this build implements the shipped "
@@ -130,7 +133,12 @@ def check_supported(sd: Dict[str, torch.Tensor], family: str = "conformer") -> N
     if family == "deepspeech2":
         hh = sd.get("encoder.rnns.0.rnn.weight_hh_l0")
         if hh is not None and hh.shape[0] != 4 * hh.shape[1]:          # GRU: 3 gates, LSTM: 4
-            raise UnsupportedConfig("unsupported config: use_gru=True (this build implements the shipped LSTM recurrences)")
+            raise UnsupportedConfig(f"unsupported layout: {hh.shape[0]}-row recurrent weights under the LSTM key names "
+                                    "(use_gru=True checkpoints keep their GRU under encoder.rnns.{l}.rnn.rnn.*)")
+        hh = sd.get("encoder.rnns.0.rnn.rnn.weight_hh_l0")
+        if hh is not None and hh.shape[0] != 3 * hh.shape[1]:
+            raise UnsupportedConfig(f"unsupported layout: {hh.shape[0]}-row recurrent weights under the GRU key names "
+                                    "(use_gru=True: 3 gates)")
         return
     u = sd.get("encoder.encoders.0.self_attn.pos_bias_u")
     if u is not None:

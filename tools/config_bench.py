@@ -5,7 +5,8 @@ per-GPU shard of every BASELINE.json config that is not the headline — one JSO
     config 5  conformer.yml (streaming-trained), 64 utterances of 1-30 s per GPU (512 over 8), ctc_beam_search (no LM)
     config 4lm / 4plm / 5lm  the same beam-search configs with a synthetic character 5-gram ARPA LM (alpha 2.2, beta 4.3, the
               shipped configs' values; a few million n-grams, generated into a temporary directory on first use)
-    plus      squeezeformer.yml / deepspeech2.yml whole-utterance, 32 x 10 s, ctc_greedy
+    plus      squeezeformer.yml / deepspeech2.yml whole-utterance, 32 x 10 s, ctc_greedy; deepspeech2gru the same with
+              encoder_conf.use_gru: True (GRU recurrences)
 Numbers printed here are dev measurements (CUDA-synchronised wall clock around the public engine call), not bench values."""
 import json
 import os
@@ -104,7 +105,7 @@ def greedy_oracle(mod, sd, cfg, batched=True):
     return f
 
 
-from oracle import conformer as oc, deepspeech2 as ods, efficient_conformer as oe, squeezeformer as osq  # noqa: E402
+from oracle import conformer as oc, deepspeech2 as ods, deepspeech2_gru as odg, efficient_conformer as oe, squeezeformer as osq  # noqa: E402
 
 tens = [synth.noise_audio(1000 + i, 160000) for i in range(32)]
 rng = np.random.default_rng(0)
@@ -176,3 +177,8 @@ sdn = synth.deepspeech2_state_dict(0)
 e = DeepSpeech2Engine(sdn, streaming=True)
 run("deepspeech2 deepspeech2.yml 32x10s ctc_greedy (whole utterance)", e, tens, lambda w: e.transcribe(w),
     oracle=greedy_oracle(ods, synth.to_torch(sdn), ods.DS2Config()), sample=(0,))
+del e
+sdn = synth.deepspeech2_state_dict(0, use_gru=True)
+e = DeepSpeech2Engine(sdn, streaming=True)
+run("deepspeech2gru deepspeech2.yml use_gru=True 32x10s ctc_greedy (whole utterance)", e, tens, lambda w: e.transcribe(w),
+    oracle=greedy_oracle(odg, synth.to_torch(sdn), ods.DS2Config()), sample=(0,))
