@@ -14,18 +14,29 @@
 //            correction Hh.W2l + Hl.W2h accumulated per k16 step over all of F; then + b2, then x + alpha * v.
 //
 // Structure (persistent over 64-row blocks; 2 consumer warpgroups + 1 TMA producer warpgroup, setmaxnreg 232 / 40):
-//   per hidden chunk j (128 columns):
+//   per hidden chunk (128 columns):
 //     phase A  warpgroup w computes hidden columns [64 w, +64) of the chunk: m64n64k16 over K = 256 (X and W1 K-blocks streamed
-//              through the ring), bias + SiLU + split in registers, st.shared into the H buffer (64 x 128 pair, K-major with the
-//              64-byte swizzle TMA uses, so gmma_desc_sw64 describes it)
-//     barrier  named barrier over both consumer warpgroups, after fence.proxy.async (generic stores -> wgmma reads)
+//              through the ring)
+//     epilogue bias + SiLU + split in registers, st.shared into one of two H buffers (64 x 128 pair, K-major with the 64-byte
+//              swizzle TMA uses, so gmma_desc_sw64 describes it), then fence.proxy.async (generic stores -> wgmma reads)
+//     barrier  named barrier over both consumer warpgroups: the H chunk is complete
 //     phase B  warpgroup w multiplies the whole H chunk by W2 rows [128 w, +128): m64n128k16, 4 W2 K-blocks from the ring
-//   The K-blocks of a row block are issued as one in-order stream A(0), B(0), A(1), B(1), ... ; a warpgroup waits for its MMAs
-//   only once per chunk, after A(j + 1) (wait_group 0), and before that per K-block with wait_group 1 to release ring stages.
-//   Shared memory: ring 4 x 32 KB | H 32 KB | running sum 64 x 256 fp32 = 64 KB | mbarriers  (= 224 KB + alignment)
+//   The K-blocks of a row block are issued in the order A(0), A(1), B(0), A(2), B(1), ..., A(nch - 1), B(nch - 2), B(nch - 1):
+//   A(j + 1) runs before B(j), so while the tensor cores run B(j) on H[j & 1] the warpgroup stores the epilogue of chunk j + 1
+//   into H[(j + 1) & 1], a quarter of it after each of B(j)'s K-blocks.  After each K-block's commit a warpgroup waits for the
+//   previous one (wait_group 1) and releases its ring stage; wgmma groups retire in order, so B(j) is complete once A(j + 2)'s
+//   first K-block is issued and waited past: that is where the main product of a 256-chunk goes into the running sum and
+//   where the row block's output is written, with no wait of their own.  One barrier per chunk: H(j + 1) is complete in both
+//   warpgroups, and both have finished B(j), so H[j & 1] is free for chunk j + 2.  After the barrier a warpgroup waits for
+//   everything (wait_group 0), so that the barrier overlaps A(j + 2)'s last K-block: ptxas serializes every wgmma of the
+//   kernel (C7514 / C7518) when MMAs are in flight across the chunk loop's back-edge.
+//   The second H buffer costs the ring its fourth stage, too few to hide HBM latency when the weights are cold, so each CTA
+//   first prefetches its share of the weights into L2 (cp.async.bulk.prefetch).
+//   Shared memory: ring 3 x 32 KB | H 2 x 32 KB | running sum 64 x 256 fp32 = 64 KB | mbarriers  (= 224 KB + alignment)
 //   Registers per consumer thread: 32 + 32 (phase A) + 64 + 64 (phase B) accumulators.
 #include <cuda.h>
 #include <cuda_fp16.h>
+#include <stdlib.h>
 #include <string.h>
 
 #include "tc_common.cuh"
@@ -38,15 +49,15 @@ constexpr int FM = 64;                         // rows per CTA (row block)
 constexpr int FD = 256;                        // model width d (K of w_1, N of w_2)
 constexpr int FHC = 128;                       // hidden columns per chunk
 constexpr int FBK = 32;                        // K per ring stage (one 64-byte swizzle row of halves)
-constexpr int F_STAGES = 4;
+constexpr int F_STAGES = 3;
 constexpr int F_STAGE_BYTES = 32768;           // phase A: Xh, Xl (4 KB each) + W1h, W1l (8 KB each); phase B: W2h, W2l (16 KB each)
-constexpr int F_H_BYTES = FM * FHC * 2 * 2;    // hidden chunk as (h, l): [K-block][h / l] 64 x 32 tiles of 4 KB
+constexpr int F_H_BYTES = FM * FHC * 2 * 2;    // one H buffer, a hidden chunk as (h, l): [K-block][h / l] 64 x 32 tiles of 4 KB
 constexpr int F_SUM_BYTES = FM * FD * 4;       // running fp32 sum of the finished 256-chunks (each thread: its own elements)
 constexpr int F_THREADS = 384;
 constexpr int F_PRODUCER_REGS = 40, F_CONSUMER_REGS = 232;
 constexpr uint32_t F_TX_A = 2 * FM * FBK * 2 + 2 * FHC * FBK * 2;   // 24 KB
 constexpr uint32_t F_TX_B = 2 * FD * FBK * 2;                       // 32 KB
-constexpr size_t kFfnSmem = F_STAGES * F_STAGE_BYTES + F_H_BYTES + F_SUM_BYTES + 1024 + 256;
+constexpr size_t kFfnSmem = F_STAGES * F_STAGE_BYTES + 2 * F_H_BYTES + F_SUM_BYTES + 1024 + 256;
 static_assert(kFfnSmem <= 232448, "ffn_tc shared memory exceeds the 227 KB per-CTA limit of sm_90");
 static_assert(F_PRODUCER_REGS * 128 + F_CONSUMER_REGS * 256 <= 65536, "register file of the SM");
 
@@ -57,13 +68,19 @@ struct FfnMaps {
 };
 
 struct FfnParams {
+    const void* w[4];         // W1h, W1l, W2h, W2l: F x 256 halves each, contiguous
     const float* b1;
     const float* b2;
     float* x;
     int64_t ldx;
     int M, F;
     float alpha;
+    int flags;                // profiling switches, read only by ffn_tc_kernel<true>
 };
+
+// Profiling switches (MASR_FFN_FLAGS, tools/ffn_bound_probe.py; the outputs are garbage under them): no TMA loads (the
+// producer arrives on the full barrier and the MMAs run on stale stages), no MMAs, no hidden epilogue (store_hidden skipped)
+constexpr int FFN_NO_LOADS = 1, FFN_NO_MMA = 2, FFN_NO_EPILOGUE = 4;
 
 // D[64x64] (+)= A[64x16] . B[64x16]^T, both operands K-major in shared memory; scale_d == 0 overwrites D
 __device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
@@ -84,62 +101,79 @@ __device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t da, 
 
 __device__ __forceinline__ void bar_consumers() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
+template <bool PROBE>
 __global__ void __launch_bounds__(F_THREADS, 1) ffn_tc_kernel(const __grid_constant__ FfnMaps maps, FfnParams p) {
+    const bool no_loads = PROBE && (p.flags & FFN_NO_LOADS), no_mma = PROBE && (p.flags & FFN_NO_MMA);
+    const bool no_epilogue = PROBE && (p.flags & FFN_NO_EPILOGUE);
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* hbuf = smem + F_STAGES * F_STAGE_BYTES;
-    uint8_t* sum = hbuf + F_H_BYTES;
+    uint8_t* hbuf = smem + F_STAGES * F_STAGE_BYTES;          // chunk g in H[g & 1] = hbuf + (g & 1) * F_H_BYTES
+    uint8_t* sum = hbuf + 2 * F_H_BYTES;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(sum + F_SUM_BYTES);
     uint64_t* empty_bar = full_bar + F_STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nrb = (p.M + FM - 1) / FM;
-    const int nch = p.F / FHC;                 // hidden chunks (even: F % 256 == 0)
+    const int nch = p.F / FHC;                 // hidden chunks per row block (even: F % 256 == 0)
+    // chunk g % nch of row block blockIdx.x + (g / nch) gridDim.x
 
     if (warp == 8 && lane == 0) {
         tma_prefetch_desc(&maps.xh); tma_prefetch_desc(&maps.xl); tma_prefetch_desc(&maps.w1h);
         tma_prefetch_desc(&maps.w1l); tma_prefetch_desc(&maps.w2h); tma_prefetch_desc(&maps.w2l);
         for (int s = 0; s < F_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        // Every CTA reads all of the weights, chunk by chunk, and they come cold from HBM in a model step.  Each CTA
+        // prefetches its 1 / gridDim share of them into L2 at once (no kernel writes them, so before griddepcontrol.wait),
+        // so that the first CTA to reach a chunk does not wait for HBM with only the ring's few stages in flight.
+        const uint32_t wbytes = (uint32_t)p.F * FD * 2;
+        const uint32_t share = ((wbytes + gridDim.x - 1) / gridDim.x + 15) & ~15u;
+        const uint32_t off = share * blockIdx.x;
+        if (!no_loads && off < wbytes)
+            for (int t = 0; t < 4; ++t)
+                asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;"
+                             ::"l"(static_cast<const uint8_t*>(p.w[t]) + off), "r"(min(share, wbytes - off)) : "memory");
     }
     __syncthreads();
     pdl_wait();
     pdl_launch_dependents();
 
     if (warp >= 8) {
-        // ---- TMA producer: the K-blocks of every row block in the consumers' order A(0), B(0), A(1), ..., B(nch - 1) ----
+        // ---- TMA producer: per row block, the K-blocks in the consumers' order A(0), A(1), B(0), A(2), B(1), ..., B(nch - 1) ----
         setmaxnreg_dec<F_PRODUCER_REGS>();
         if (warp == 8 && elect_one_sync()) {
             uint32_t kg = 0;
             auto acquire = [&](uint32_t tx) {
                 const uint32_t s = kg % F_STAGES;
                 mbar_wait(&empty_bar[s], ((kg / F_STAGES) & 1) ^ 1);
-                mbar_expect_tx(&full_bar[s], tx);
+                if (no_loads) mbar_arrive(&full_bar[s]);
+                else mbar_expect_tx(&full_bar[s], tx);
                 ++kg;
                 return s;
             };
+            auto load_a = [&](int m0, int j) {          // A(j): X rows m0.., W1 rows 128 j ..
+                const int n0 = j * FHC;
+#pragma unroll 1
+                for (int kb = 0; kb < FD / FBK; ++kb) {
+                    const uint32_t s = acquire(F_TX_A);
+                    if (no_loads) continue;
+                    uint8_t* st = smem + s * F_STAGE_BYTES;
+                    tma_load_2d(&maps.xh, &full_bar[s], st, kb * FBK, m0);
+                    tma_load_2d(&maps.xl, &full_bar[s], st + 4096, kb * FBK, m0);
+                    tma_load_2d(&maps.w1h, &full_bar[s], st + 8192, kb * FBK, n0);
+                    tma_load_2d(&maps.w1l, &full_bar[s], st + 16384, kb * FBK, n0);
+                }
+            };
             for (int rb = blockIdx.x; rb < nrb; rb += gridDim.x) {
-                const int m0 = rb * FM;
-                for (int j = -1; j < nch; ++j) {
-                    if (j >= 0) {
+                load_a(rb * FM, 0);
+                for (int j = 0; j < nch; ++j) {
+                    if (j + 1 < nch) load_a(rb * FM, j + 1);
 #pragma unroll 1
-                        for (int kb = 0; kb < FHC / FBK; ++kb) {          // B(j): W2 [256 rows, hidden 128 j + 32 kb ..]
-                            const uint32_t s = acquire(F_TX_B);
-                            uint8_t* st = smem + s * F_STAGE_BYTES;
-                            tma_load_2d(&maps.w2h, &full_bar[s], st, j * FHC + kb * FBK, 0);
-                            tma_load_2d(&maps.w2l, &full_bar[s], st + F_STAGE_BYTES / 2, j * FHC + kb * FBK, 0);
-                        }
-                    }
-                    if (j + 1 < nch) {
-#pragma unroll 1
-                        for (int kb = 0; kb < FD / FBK; ++kb) {           // A(j + 1): X rows m0.., W1 rows 128 (j + 1)..
-                            const uint32_t s = acquire(F_TX_A);
-                            uint8_t* st = smem + s * F_STAGE_BYTES;
-                            tma_load_2d(&maps.xh, &full_bar[s], st, kb * FBK, m0);
-                            tma_load_2d(&maps.xl, &full_bar[s], st + 4096, kb * FBK, m0);
-                            tma_load_2d(&maps.w1h, &full_bar[s], st + 8192, kb * FBK, (j + 1) * FHC);
-                            tma_load_2d(&maps.w1l, &full_bar[s], st + 16384, kb * FBK, (j + 1) * FHC);
-                        }
+                    for (int kb = 0; kb < FHC / FBK; ++kb) {    // B(j): W2 [256 rows, hidden 128 j + 32 kb ..]
+                        const uint32_t s = acquire(F_TX_B);
+                        if (no_loads) continue;
+                        uint8_t* st = smem + s * F_STAGE_BYTES;
+                        tma_load_2d(&maps.w2h, &full_bar[s], st, j * FHC + kb * FBK, 0);
+                        tma_load_2d(&maps.w2l, &full_bar[s], st + F_STAGE_BYTES / 2, j * FHC + kb * FBK, 0);
                     }
                 }
             }
@@ -173,9 +207,9 @@ __global__ void __launch_bounds__(F_THREADS, 1) ffn_tc_kernel(const __grid_const
             if (pend >= 0) release((uint32_t)pend);
             pend = (int)s;
         };
-        auto phase_a = [&]() {
+        auto phase_a = [&](int kb_begin, int kb_end) {             // K-blocks [kb_begin, kb_end) of an A chunk
 #pragma unroll 1
-            for (int kb = 0; kb < FD / FBK; ++kb) {
+            for (int kb = kb_begin; kb < kb_end; ++kb) {
                 const uint32_t s = next_stage();
                 const uint32_t sa = smem_u32(smem + s * F_STAGE_BYTES);
                 const uint64_t dXh = gmma_desc_sw64(sa), dXl = gmma_desc_sw64(sa + 4096);
@@ -184,6 +218,7 @@ __global__ void __launch_bounds__(F_THREADS, 1) ffn_tc_kernel(const __grid_const
                 wgmma_fence();
 #pragma unroll
                 for (int ks = 0; ks < FBK / 16; ++ks) {
+                    if (no_mma) break;
                     const uint64_t adv = (uint64_t)(ks * 2);
                     const uint32_t first = (kb | ks) ? 1u : 0u;
                     wgmma_m64n64k16_ss(acc1, dXh + adv, dWh + adv, first);
@@ -194,41 +229,44 @@ __global__ void __launch_bounds__(F_THREADS, 1) ffn_tc_kernel(const __grid_const
                 retire(s);
             }
         };
-        auto phase_b = [&](int j) {
-#pragma unroll 1
-            for (int kb = 0; kb < FHC / FBK; ++kb) {
-                const uint32_t s = next_stage();
-                const uint32_t sa = smem_u32(smem + s * F_STAGE_BYTES);
-                const uint64_t dWh = gmma_desc_sw64(sa + wg * 8192), dWl = gmma_desc_sw64(sa + F_STAGE_BYTES / 2 + wg * 8192);
-                const uint64_t dHh = gmma_desc_sw64(h_base + kb * 8192), dHl = gmma_desc_sw64(h_base + kb * 8192 + 4096);
-                reg_fence(acc2); reg_fence(cor2);
-                wgmma_fence();
+        // K-block kb of B for hidden chunk j (of its row block), H chunk at hb
+        auto phase_b = [&](int j, uint32_t hb, int kb) {
+            const uint32_t s = next_stage();
+            const uint32_t sa = smem_u32(smem + s * F_STAGE_BYTES);
+            const uint64_t dWh = gmma_desc_sw64(sa + wg * 8192), dWl = gmma_desc_sw64(sa + F_STAGE_BYTES / 2 + wg * 8192);
+            const uint64_t dHh = gmma_desc_sw64(hb + kb * 8192), dHl = gmma_desc_sw64(hb + kb * 8192 + 4096);
+            reg_fence(acc2); reg_fence(cor2);
+            wgmma_fence();
 #pragma unroll
-                for (int ks = 0; ks < FBK / 16; ++ks) {
-                    const uint64_t adv = (uint64_t)(ks * 2);
-                    wgmma_m64n128k16_ss(acc2, dHh + adv, dWh + adv, ((j & 1) | kb | ks) ? 1u : 0u);   // fresh per 256-chunk
-                    wgmma_m64n128k16_ss(cor2, dHh + adv, dWl + adv, (j | kb | ks) ? 1u : 0u);         // over all of F
-                    wgmma_m64n128k16_ss(cor2, dHl + adv, dWh + adv, 1u);
-                }
-                wgmma_commit();
-                retire(s);
+            for (int ks = 0; ks < FBK / 16; ++ks) {
+                if (no_mma) break;
+                const uint64_t adv = (uint64_t)(ks * 2);
+                wgmma_m64n128k16_ss(acc2, dHh + adv, dWh + adv, ((j & 1) | kb | ks) ? 1u : 0u);   // fresh per 256-chunk
+                wgmma_m64n128k16_ss(cor2, dHh + adv, dWl + adv, (j | kb | ks) ? 1u : 0u);         // over all of F
+                wgmma_m64n128k16_ss(cor2, dHl + adv, dWh + adv, 1u);
             }
+            wgmma_commit();
+            retire(s);
         };
         // fragment of m64nN: this thread holds rows 16 wi + lane / 4 (+ 8) and columns 8 i + 2 q (+ 1)
         const int r_lo = 16 * wi + (lane >> 2);
-        // hidden chunk j: H <- split(SiLU(fmaf(cor1, 2^-11, acc1) + b1)).  Caller: both warpgroups are past their reads of H.
-        auto store_hidden = [&](int j) {
-            float2 bb[8];
-            const float* b = p.b1 + j * FHC + 64 * wg + 2 * q;
+        // b1 of column groups 2 sl, 2 sl + 1 of hidden chunk j (this warpgroup's 64 columns)
+        auto load_b1 = [&](int j, int sl, float2 (&bb)[2]) {
+            const float* b = p.b1 + j * FHC + 64 * wg + 16 * sl + 2 * q;
+            bb[0] = __ldg(reinterpret_cast<const float2*>(b));
+            bb[1] = __ldg(reinterpret_cast<const float2*>(b + 8));
+        };
+        // slice sl (column groups 2 sl, 2 sl + 1) of a hidden chunk: H at hb <- split(SiLU(fmaf(cor1, 2^-11, acc1) + b1)).
+        // Caller: A of the chunk has completed, and both warpgroups are past their reads of the buffer at hb.
+        auto store_hidden = [&](uint32_t hb, int sl, const float2 (&bb)[2]) {
+            if (no_epilogue) return;
 #pragma unroll
-            for (int i = 0; i < 8; ++i) bb[i] = __ldg(reinterpret_cast<const float2*>(b + 8 * i));
-#pragma unroll
-            for (int i = 0; i < 8; ++i)
+            for (int i = 2 * sl; i < 2 * sl + 2; ++i)
 #pragma unroll
                 for (int hh = 0; hh < 2; ++hh) {
                     float v0 = fmaf(cor1[4 * i + 2 * hh], kLoInv, acc1[4 * i + 2 * hh]);
                     float v1 = fmaf(cor1[4 * i + 2 * hh + 1], kLoInv, acc1[4 * i + 2 * hh + 1]);
-                    v0 += bb[i].x; v1 += bb[i].y;
+                    v0 += bb[i - 2 * sl].x; v1 += bb[i - 2 * sl].y;
                     // SiLU exactly as tc_gemm.cu's MASR_EPI_BIAS_SILU epilogue
                     float e0, e1;
                     mul2(e0, e1, v0, v1, -1.4426950408889634f, -1.4426950408889634f);
@@ -239,12 +277,13 @@ __global__ void __launch_bounds__(F_THREADS, 1) ffn_tc_kernel(const __grid_const
                     __half2 h2, l2;
                     split_f16x2(v0, v1, h2, l2);
                     const int r = r_lo + 8 * hh, c = 64 * wg + 8 * i + 2 * q;     // chunk column c: K-block c / 32
-                    const uint32_t a = h_base + (c >> 5) * 8192 + r * 64 + ((((c & 31) >> 3) ^ ((r >> 1) & 3)) << 4) + (c & 7) * 2;
+                    const uint32_t a = hb + (c >> 5) * 8192 + r * 64 + ((((c & 31) >> 3) ^ ((r >> 1) & 3)) << 4) + (c & 7) * 2;
                     asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(*reinterpret_cast<uint32_t*>(&h2)) : "memory");
                     asm volatile("st.shared.b32 [%0], %1;" ::"r"(a + 4096), "r"(*reinterpret_cast<uint32_t*>(&l2)) : "memory");
                 }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic stores -> visible to wgmma (async proxy)
         };
+        // generic stores of H -> visible to wgmma (async proxy)
+        auto fence_h = [&]() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); };
         auto drain = [&]() {
             wgmma_wait<0>();
             reg_fence(acc1); reg_fence(cor1); reg_fence(acc2); reg_fence(cor2);
@@ -252,41 +291,24 @@ __global__ void __launch_bounds__(F_THREADS, 1) ffn_tc_kernel(const __grid_const
             pend = -1;
         };
 
-        for (int rb = blockIdx.x; rb < nrb; rb += gridDim.x) {
-            const int m0 = rb * FM;
-            phase_a();
-            drain();
-            bar_consumers();                     // both warpgroups are done with the previous row block's H
-            store_hidden(0);
-            bar_consumers();                     // H(0) complete
-#pragma unroll 1
-            for (int j = 0; j < nch; ++j) {
-                phase_b(j);
-                if (j + 1 < nch) phase_a();
-                drain();
-                // end of a 256-chunk that is not the last: add the main product into the running sum (acc2 is only read)
-                if ((j & 1) && j + 1 < nch) {
+        // end of a 256-chunk j that is not the last: add the main product into the running sum (acc2 is only read)
+        auto add_sum = [&](int j) {
 #pragma unroll
-                    for (int i = 0; i < 16; ++i)
+            for (int i = 0; i < 16; ++i)
 #pragma unroll
-                        for (int hh = 0; hh < 2; ++hh) {
-                            float x0 = acc2[4 * i + 2 * hh], x1 = acc2[4 * i + 2 * hh + 1];
-                            const uint32_t a = sum_base + (i * 2 + hh) * 1024;
-                            if (j > 1) {
-                                float s0, s1;
-                                asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(s0), "=f"(s1) : "r"(a) : "memory");
-                                x0 = s0 + x0; x1 = s1 + x1;
-                            }
-                            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(x0), "f"(x1) : "memory");
-                        }
+                for (int hh = 0; hh < 2; ++hh) {
+                    float x0 = acc2[4 * i + 2 * hh], x1 = acc2[4 * i + 2 * hh + 1];
+                    const uint32_t a = sum_base + (i * 2 + hh) * 1024;
+                    if (j > 1) {
+                        float s0, s1;
+                        asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(s0), "=f"(s1) : "r"(a) : "memory");
+                        x0 = s0 + x0; x1 = s1 + x1;
+                    }
+                    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(x0), "f"(x1) : "memory");
                 }
-                if (j + 1 < nch) {
-                    bar_consumers();             // both warpgroups' B(j) have retired: H is free
-                    store_hidden(j + 1);
-                    bar_consumers();             // H(j + 1) complete
-                }
-            }
-            // x <- x + alpha * ((running sum + last chunk) + 2^-11 * correction + b2), rows < M
+        };
+        // x <- x + alpha * ((running sum + last chunk) + 2^-11 * correction + b2) for the row block at m0, rows < M
+        auto write_out = [&](int m0) {
             const float* b2 = p.b2 + 128 * wg + 2 * q;
 #pragma unroll
             for (int i = 0; i < 16; ++i) {
@@ -311,6 +333,47 @@ __global__ void __launch_bounds__(F_THREADS, 1) ffn_tc_kernel(const __grid_const
                         *xp = make_float2(x0, x1);
                     }
                 }
+            }
+        };
+
+#pragma unroll 1
+        for (int rb = blockIdx.x; rb < nrb; rb += gridDim.x) {
+            // prologue: A(0), its epilogue into H[0], A(1) (nch >= 2).  The previous row block's last chunks have drained,
+            // and the barrier below is passed by both warpgroups before either writes H[1] again.
+            phase_a(0, FD / FBK);
+            drain();
+#pragma unroll
+            for (int sl = 0; sl < 4; ++sl) {
+                float2 bb[2];
+                load_b1(0, sl, bb);
+                store_hidden(h_base, sl, bb);
+            }
+            fence_h();
+            phase_a(0, FD / FBK);
+            drain();
+            bar_consumers();                                         // H(0) complete
+            // A warpgroup drains once per chunk, after the barrier, so that the barrier wait overlaps A(j + 2)'s last K-block.
+            // ptxas serializes every wgmma of the kernel (C7514 / C7518) when MMAs are in flight across the back-edge.
+#pragma unroll 1
+            for (int j = 0; j < nch; ++j) {
+                // here A(j + 1) has been issued (j + 1 < nch) and H(j) is complete in H[j & 1]
+                const bool next = j + 1 < nch, a2 = j + 2 < nch;
+                const uint32_t hb = h_base + (j & 1) * F_H_BYTES, hn = h_base + ((j + 1) & 1) * F_H_BYTES;
+#pragma unroll
+                for (int kb = 0; kb < FHC / FBK; ++kb) {
+                    float2 bb[2];
+                    if (next) load_b1(j + 1, kb, bb);
+                    phase_b(j, hb, kb);
+                    if (next) store_hidden(hn, kb, bb);              // a quarter of H(j + 1) while B(j)'s K-block kb runs
+                }
+                if (next) fence_h();
+                if (a2) phase_a(0, 1);                               // A(j + 2)'s first K-block; B(j) has retired
+                else drain();
+                if ((j & 1) && j + 1 < nch) add_sum(j);
+                if (j == nch - 1) write_out(rb * FM);
+                if (a2) phase_a(1, FD / FBK);
+                if (next) bar_consumers();                           // H(j + 1) complete; H[j & 1] no longer read
+                drain();                                             // nothing in flight across the loop's back-edge
             }
         }
     }
@@ -366,15 +429,21 @@ extern "C" int masr_ffn_tc_f16x2(const void* Ah, const void* Al, int64_t lda, co
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) dev = 0;
+    void (*const kernels[2])(FfnMaps, FfnParams) = {ffn_tc_kernel<false>, ffn_tc_kernel<true>};
     if (!g_ffn_attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(ffn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFfnSmem);
-        if (e != cudaSuccess) { set_last_error("ffn_tc smem attr: %s", cudaGetErrorString(e)); return (int)e; }
+        for (auto k : kernels) {
+            cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFfnSmem);
+            if (e != cudaSuccess) { set_last_error("ffn_tc smem attr: %s", cudaGetErrorString(e)); return (int)e; }
+        }
         g_ffn_attr_set[dev] = true;
     }
     int sms = 0;
     if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
     const int nrb = (M + FM - 1) / FM;
-    FfnParams p{b1, b2, x, ldx, M, F, alpha};
-    launch_pdl(ffn_tc_kernel, dim3(nrb < sms ? nrb : sms), dim3(F_THREADS), kFfnSmem, (cudaStream_t)stream, maps, p);
+    const char* env = getenv("MASR_FFN_FLAGS");   // profiling switches only (FFN_NO_*); unset or 0 in normal use
+    const int flags = env ? atoi(env) : 0;
+    FfnParams p{{W1h, W1l, W2h, W2l}, b1, b2, x, ldx, M, F, alpha, flags};
+    const dim3 grid(nrb < sms ? nrb : sms);
+    launch_pdl(kernels[flags ? 1 : 0], grid, dim3(F_THREADS), kFfnSmem, (cudaStream_t)stream, maps, p);
     return check_launch("ffn_tc_kernel");
 }
