@@ -87,8 +87,9 @@ int masr_wave_gain_f32(const float* wave, const int64_t* offsets, int B, int64_t
 /* AudioSegment.to('int16') + torchaudio.compliance.kaldi.fbank(num_mel_bins=80, frame_length=25,
  * frame_shift=10, dither=0, sample_frequency=16000) (audio.py:244-254,549-574;
  * audio_featurizer.py:120-138; torchaudio kaldi.py:514-645).  gain may be NULL (no dB normalisation).
- * feats: [B, Fmax, 80] raw log-mel, rows >= the utterance's frame count are zero;
- * num_frames[b] = 1 + (n_b - 400) / 160 (0 if n_b < 400), may be NULL. */
+ * feats: [B, Fmax, 80] raw log-mel, rows >= the utterance's frame count are zero (an utterance with more than Fmax
+ * frames gets its first Fmax); num_frames[b] = 1 + (n_b - 400) / 160 (0 if n_b < 400), written for every b whatever
+ * Fmax (also 0), may be NULL.  With Fmax == 0 no sample is read and no feature written: wave and feats may be NULL. */
 int masr_fbank_f32(const float* wave, const int64_t* offsets, const float* gain, int B, int Fmax, float* feats,
                    int* num_frames, void* stream);
 

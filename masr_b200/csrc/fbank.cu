@@ -9,7 +9,7 @@
 //
 // Kernels
 //   wave_sumsq_kernel   per-utterance sum of squares, fixed-order double partials (deterministic)
-//   wave_gain_kernel    mean square -> gain factor (float32 chain as numpy does it), error flag if the
+//   wave_gain_kernel    mean square -> gain factor (float32 chain, as numpy's up to the last bit), error flag if the
 //                       required gain exceeds 300 dB (the reference raises ValueError, audio.py:302)
 //   fbank_kernel        one warp per frame: quantise 400 samples on the fly, DC removal, pre-emphasis,
 //                       povey window, 512-point real FFT (as a 256-point complex FFT in shared memory),
@@ -138,8 +138,9 @@ __global__ void wave_gain_kernel(const int64_t* __restrict__ offs, const double*
     for (int c = 0; c < chunks; ++c) s += partial[(int64_t)b * max_chunks + c];
     float ms = n > 0 ? (float)(s / (double)n) : 0.f;       // np.mean -> float32
     if (ms == 0.f) ms = 1.f;                               // audio.py:526-527
-    float rms_db = 10.f * (float)log10((double)ms);        // float32 scalar chain (audio.py:529)
-    float g = target_db - rms_db;
+    // required gain target_db - 10 log10(ms) (audio.py:301,529), rounded once by a fused multiply-add.  numpy rounds
+    // rms_db to float32 first, from a float32 log10 that is not always correctly rounded: g can differ in its last bit.
+    float g = fmaf(-10.f, (float)log10((double)ms), target_db);
     int bad = g > max_gain_db;
     if (bad) g = max_gain_db;
     float e = g / 20.f;
@@ -370,8 +371,12 @@ extern "C" int masr_wave_gain_f32(const float* wave, const int64_t* offsets, int
 
 extern "C" int masr_fbank_f32(const float* wave, const int64_t* offsets, const float* gain, int B, int Fmax,
                               float* feats, int* num_frames, void* stream) {
-    if (B == 0 || Fmax == 0) return MASR_OK;
-    MASR_REQUIRE(wave && offsets && feats, "masr_fbank_f32: null pointer");
+    if (B == 0) return MASR_OK;
+    MASR_REQUIRE(B > 0 && Fmax >= 0, "masr_fbank_f32: bad argument");
+    // with Fmax == 0 no sample is read and no feature written, so wave and feats may be NULL (zero-byte buffers of a
+    // batch of sub-frame chunks have no address); only num_frames is written
+    MASR_REQUIRE(offsets && (Fmax == 0 || (wave && feats)), "masr_fbank_f32: null pointer");
+    if (Fmax == 0 && !num_frames) return MASR_OK;
     {
         std::lock_guard<std::mutex> lk(g_tab_mu);
         int dev = 0;
@@ -384,7 +389,8 @@ extern "C" int masr_fbank_f32(const float* wave, const int64_t* offsets, const f
         }
     }
     const int frames_per_block = kWarpsPerBlock * kFramesPerWarp;
-    dim3 grid((Fmax + frames_per_block - 1) / frames_per_block, B);
+    // at least one CTA column: it writes num_frames even when Fmax == 0 (its warps leave the frame loop at once)
+    dim3 grid(max(1, (Fmax + frames_per_block - 1) / frames_per_block), B);
     fbank_kernel<<<grid, kWarpsPerBlock * 32, 0, (cudaStream_t)stream>>>(wave, offsets, gain, feats, num_frames, Fmax);
     return check_launch("fbank_kernel");
 }

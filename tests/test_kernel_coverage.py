@@ -11,9 +11,6 @@ HEADER = os.path.join(ROOT, "include", "masr_b200.h")
 # entry point -> why no test names it as a string
 COVERED_INDIRECTLY = {
     "masr_abi_version": "called as a ctypes attribute in test_abi.py::test_abi_version_and_error_string",
-    "masr_fbank_workspace_bytes": "host-only size query behind ConformerEngine.fbank (test_gpu_parity.py)",
-    "masr_wave_gain_f32": "through ConformerEngine.fbank in test_gpu_parity.py (gain and the GAIN_EXCEEDED status)",
-    "masr_fbank_f32": "through ConformerEngine.fbank in test_gpu_parity.py, against the oracle's kaldi fbank",
     "masr_lm_load_arpa": "through CharLM in test_lm.py and test_gpu_lm.py, including every rejected file",
     "masr_lm_info": "through CharLM in test_lm.py and test_gpu_lm.py",
     "masr_lm_export": "through CharLM in test_lm.py and test_gpu_lm.py",
