@@ -180,7 +180,9 @@ int masr_ctc_head_argmax_tc_f16x2(const void* Ah, const void* Al, int64_t lda, c
 /* Conv2dSubsampling4's first conv (as masr_conv1_cmvn_relu_f32) written as fp16 (h,l) pairs in four
  * (t,f)-parity planes [4][B][(F1max+1)/2][20][C], and its second conv + ReLU (subsampling.py:83-84) as a
  * tensor-core implicit GEMM over those planes: the stride-2 window of tap (kh,kw) is a dense TMA box of plane
- * (kh&1, kw&1).  Wh/Wl: split of the [C, 3,3,C]-permuted weight.  Output rows ((b*T2 + t)*19 + f) x C. */
+ * (kh&1, kw&1).  Wh/Wl: split of the [C, 3,3,C]-permuted weight.  Output rows ((b*T2 + t)*19 + f) x C.
+ * masr_conv2_tc_f16x2: C = 256 or 512 (C / 32 K-blocks per tap; the main product is summed in 256-K chunks, so a tap at
+ * C = 512 is two chunks); masr_conv1_cmvn_relu_planes_f16: any C that is a multiple of 8. */
 int masr_conv1_cmvn_relu_planes_f16(const float* feats, const float* mean, const float* istd, const float* w1,
                                     const float* b1, void* planes_h, void* planes_l, int B, int Fmax, int idim,
                                     int F1max, int W1, int C, void* stream);
@@ -194,14 +196,15 @@ int masr_split_f16(const float* x, void* h, void* l, int64_t n, void* stream);
 int masr_layernorm_f32(const float* x, int64_t ldx, const float* gamma, const float* beta, float* y, int64_t ldy,
                        int M, int D, float eps, void* stream);
 
-/* LayerNorm writing the fp16 (h, l) operand pair of masr_gemm_tc_f16x2 instead of fp32. */
+/* LayerNorm writing the fp16 (h, l) operand pair of masr_gemm_tc_f16x2 instead of fp32.  D = 256, 1024 or 2048 (a 512-wide
+ * row goes through masr_layernorm_f32 + masr_split_f16, which write the same pair). */
 int masr_layernorm_split_f16(const float* x, int64_t ldx, const float* gamma, const float* beta, void* yh, void* yl,
                              int64_t ldy, int M, int D, float eps, void* stream);
 
 /* Two LayerNorms back to back in one pass: y1 = LN(x; gamma1, beta1) as fp32 (row pitch ldx; may alias x), then
  * LN(y1; gamma2, beta2) as fp32 y2 (optional) and as the fp16 pair (row pitch ldy) — `norm_final` of one encoder block
  * followed by the next block's `norm_ff_macaron`, or by `after_norm` after the last block (conformer/encoder.py:161,106,342).
- * Bit-identical to masr_layernorm_f32 followed by masr_layernorm_split_f16. */
+ * Bit-identical to masr_layernorm_f32 followed by masr_layernorm_split_f16.  D = 256 or 512. */
 int masr_layernorm2_split_f16(const float* x, int64_t ldx, const float* gamma1, const float* beta1, float* y1,
                               const float* gamma2, const float* beta2, float* y2, void* yh, void* yl, int64_t ldy, int M,
                               int D, float eps, void* stream);
@@ -264,14 +267,15 @@ int masr_relpos_attention_tc5(const float* Q, int64_t ldq, int64_t q_bstride, co
 /* ConvolutionModule middle (masr/model_utils/conformer/convolution.py:121-126): depthwise Conv1d(k)
  * -> LayerNorm(C) -> SiLU.  y[b,t,:] for t < out_rows from g[b, t - lpad + k, :], k < kernel_size;
  * g rows < 0 read pad_vec (NULL = 0), rows >= in_lens[b] read 0.  w [C,k] (reference [C,1,k]).
- * Output: fp32 y and/or the fp16 (yh, yl) pair (either may be NULL). */
+ * Output: fp32 y and/or the fp16 (yh, yl) pair (either may be NULL).  C = 256 or 512, kernel_size 7 / 15 / 31. */
 int masr_dwconv_ln_silu_f32(const float* g, int64_t ldg, int64_t g_bstride, const float* w, const float* bias,
                             const float* ln_gamma, const float* ln_beta, const float* pad_vec, float* y, void* yh,
                             void* yl, int64_t ldy, int64_t y_bstride, const int* in_lens, int B, int C,
                             int kernel_size, int lpad, int out_rows, float eps, void* stream);
 
 /* masr_dwconv_ln_silu_f32 with a time stride (1 or 2): y[t] reads g[t*stride - lpad + k] — the strided depthwise conv of
- * the EfficientConformer's block 3 (masr/model_utils/efficient_conformer/convolution.py:40-48, encoder.py:160-175). */
+ * the EfficientConformer's block 3 (masr/model_utils/efficient_conformer/convolution.py:40-48, encoder.py:160-175).
+ * Stride 2: C = 256 and kernel_size 15 only. */
 int masr_dwconv_ln_silu_strided_f32(const float* g, int64_t ldg, int64_t g_bstride, const float* w, const float* bias,
                                     const float* ln_gamma, const float* ln_beta, const float* pad_vec, float* y, void* yh,
                                     void* yl, int64_t ldy, int64_t y_bstride, const int* in_lens, int B, int C,

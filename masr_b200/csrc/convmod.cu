@@ -17,7 +17,7 @@
 
 namespace masr {
 
-// Layout: one warp owns TW = 4 consecutive output frames and all 256 channels (8 per lane: channels 4*lane..+3 and
+// 256 channels (dwconv_ln_silu_wide_kernel below: 512).  Layout: one warp owns TW = 4 consecutive output frames and all 256 channels (8 per lane: channels 4*lane..+3 and
 // 128 + 4*lane..+3, so every row access is two coalesced 512-byte warp loads); a CTA = 4 warps = 16 consecutive frames, whose
 // halo rows hit L1.  The tap weights sit transposed in shared memory ([k][c], 128-bit reads).  The LayerNorm over the channels
 // of a frame is then a pure warp reduction (two-pass: mean, centred variance) — the first version (thread per channel) needed
@@ -134,6 +134,146 @@ __global__ void __launch_bounds__(DW_WARPS * 32) dwconv_ln_silu_kernel(const flo
     }
 }
 
+// The same kernel for the wide model (C = 512): stride 1, LayerNorm, 4 frames
+// per warp.  A lane owns V = C / 128 float4 per frame (channels 128 i + 4 lane..+3), i.e. 4 V TW = 64 accumulator registers at
+// C = 512.  The per-lane partial sums of the LayerNorm statistics are combined pairwise over the 128-channel groups,
+// (g0 + g1) + (g2 + g3), the order the 256-channel kernel uses for its two groups.  The 256-channel kernel above is kept as a
+// separate function: written through this template its instantiations schedule differently (90 to 120 registers against
+// 112 to 116), and the model size every measurement of this project was taken on should not change with this one.
+// The [KS][C] weight tile is static shared memory up to the 48 KB static limit and dynamic shared memory above it (k = 31 at
+// C = 512: 62 KB, opt-in attribute set by the wrapper; three CTAs still fit an SM).
+constexpr int DW_STATIC_SMEM_MAX = 48 * 1024;
+__host__ __device__ constexpr bool dw_dynamic_smem(int ks, int c) { return ks * c * (int)sizeof(float) > DW_STATIC_SMEM_MAX; }
+
+template <int KS, int C>
+__global__ void __launch_bounds__(DW_WARPS * 32) dwconv_ln_silu_wide_kernel(const float* __restrict__ g, int64_t ldg,
+                                                             int64_t g_bstride, const float* __restrict__ w,
+                                                             const float* __restrict__ bias,
+                                                             const float* __restrict__ ln_g,
+                                                             const float* __restrict__ ln_b,
+                                                             const float* __restrict__ pad_vec, float* __restrict__ y,
+                                                             __half* __restrict__ yh, __half* __restrict__ yl, int64_t ldy, int64_t y_bstride,
+                                                             const int* __restrict__ in_lens, int lpad, int out_rows,
+                                                             float eps) {
+    static_assert(C == 512, "four 128-channel groups per lane (the pairwise sums below are written for V = 4)");
+    constexpr int TW = DW_TW;
+    constexpr int V = C / 128;                               // float4 per lane and frame
+    constexpr int ROWS = TW - 1 + KS;                        // input rows one warp touches
+    constexpr bool DYN = dw_dynamic_smem(KS, C);
+    extern __shared__ __align__(16) float s_w_dyn[];
+    __shared__ __align__(16) float s_w_static[DYN ? 4 : KS * C];
+    float* const s_w = DYN ? s_w_dyn : s_w_static;           // tap-major weights [KS][C]
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int b = blockIdx.y;
+    const int t0 = (blockIdx.x * DW_WARPS + warp) * TW;      // first output frame of this warp
+    for (int idx = threadIdx.x; idx < KS * C; idx += DW_WARPS * 32) {
+        const int k = idx / C, c = idx - k * C;              // reference layout [C, 1, k]; conflict-free shared stores
+        s_w[idx] = __ldg(w + c * KS + k);
+    }
+    pdl_wait();
+    pdl_launch_dependents();
+    __syncthreads();
+    if (t0 >= out_rows) return;                              // warp-uniform (after the only barrier)
+    const int in_len = in_lens[b];
+    const int c0 = lane * 4;                                 // group i: channels 128 i + c0 .. + 3
+    float4 pv[V], a[V][TW];
+#pragma unroll
+    for (int i = 0; i < V; ++i) {
+        const float4 bs = ldg_f4(bias + 128 * i + c0);
+        pv[i] = pad_vec ? ldg_f4(pad_vec + 128 * i + c0) : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+        for (int j = 0; j < TW; ++j) a[i][j] = bs;
+    }
+    const float* gb = g + (int64_t)b * g_bstride * ldg;
+#pragma unroll
+    for (int r = 0; r < ROWS; ++r) {
+        const int tau = t0 - lpad + r;
+        float4 v[V];
+#pragma unroll
+        for (int i = 0; i < V; ++i) {
+            if (tau < 0) v[i] = pv[i];
+            else if (tau >= in_len) v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+            else v[i] = ldg_f4(gb + (int64_t)tau * ldg + 128 * i + c0);
+        }
+#pragma unroll
+        for (int j = 0; j < TW; ++j) {
+            const int k = r - j;
+            if (k >= 0 && k < KS) {
+#pragma unroll
+                for (int i = 0; i < V; ++i) {
+                    const float4 wk = *reinterpret_cast<const float4*>(&s_w[k * C + 128 * i + c0]);
+                    a[i][j].x = fmaf(wk.x, v[i].x, a[i][j].x); a[i][j].y = fmaf(wk.y, v[i].y, a[i][j].y);
+                    a[i][j].z = fmaf(wk.z, v[i].z, a[i][j].z); a[i][j].w = fmaf(wk.w, v[i].w, a[i][j].w);
+                }
+            }
+        }
+    }
+    // LayerNorm over the C channels of each frame: two-pass statistics, warp-wide
+    float mean[TW], rstd[TW];
+#pragma unroll
+    for (int j = 0; j < TW; ++j) {
+        float part[V];
+#pragma unroll
+        for (int i = 0; i < V; ++i) part[i] = (a[i][j].x + a[i][j].y) + (a[i][j].z + a[i][j].w);
+        mean[j] = warp_sum((part[0] + part[1]) + (part[2] + part[3])) * (1.0f / C);
+    }
+#pragma unroll
+    for (int j = 0; j < TW; ++j) {
+        float part[V];
+#pragma unroll
+        for (int i = 0; i < V; ++i) {
+            const float d0 = a[i][j].x - mean[j], d1 = a[i][j].y - mean[j], d2 = a[i][j].z - mean[j], d3 = a[i][j].w - mean[j];
+            part[i] = (d0 * d0 + d1 * d1) + (d2 * d2 + d3 * d3);
+        }
+        rstd[j] = rsqrtf(warp_sum((part[0] + part[1]) + (part[2] + part[3])) * (1.0f / C) + eps);
+    }
+#pragma unroll
+    for (int j = 0; j < TW; ++j) {
+        const int t = t0 + j;
+        if (t >= out_rows) break;                            // warp-uniform
+        const int64_t ro = ((int64_t)b * y_bstride + t) * ldy;
+#pragma unroll
+        for (int i = 0; i < V; ++i) {
+            const int c = 128 * i + c0;
+            const float4 gg = ldg_f4(ln_g + c), bb = ldg_f4(ln_b + c);
+            float4 o;
+            o.x = fast_silu((a[i][j].x - mean[j]) * rstd[j] * gg.x + bb.x); o.y = fast_silu((a[i][j].y - mean[j]) * rstd[j] * gg.y + bb.y);
+            o.z = fast_silu((a[i][j].z - mean[j]) * rstd[j] * gg.z + bb.z); o.w = fast_silu((a[i][j].w - mean[j]) * rstd[j] * gg.w + bb.w);
+            if (y) *reinterpret_cast<float4*>(y + ro + c) = o;
+            if (yh) {
+                const float ov[4] = {o.x, o.y, o.z, o.w};
+                __half hh[4], ll[4];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    hh[e] = __float2half_rn(ov[e]);
+                    ll[e] = __float2half_rn((ov[e] - __half2float(hh[e])) * 2048.0f);
+                }
+                *reinterpret_cast<uint2*>(yh + ro + c) = *reinterpret_cast<const uint2*>(hh);
+                *reinterpret_cast<uint2*>(yl + ro + c) = *reinterpret_cast<const uint2*>(ll);
+            }
+        }
+    }
+}
+
+// Launch of the wide kernel; the instantiation whose weight tile is dynamic shared memory gets the opt-in attribute once per device.
+template <int KS, int C, typename... Args>
+static int launch_dw_wide(dim3 grid, cudaStream_t st, Args... args) {
+    constexpr size_t dyn = dw_dynamic_smem(KS, C) ? KS * C * sizeof(float) : 0;
+    if (dyn) {
+        static bool set[64] = {false};
+        int dev = 0;
+        cudaGetDevice(&dev);
+        if (dev < 0 || dev >= 64) dev = 0;
+        if (!set[dev]) {
+            cudaError_t e = cudaFuncSetAttribute(dwconv_ln_silu_wide_kernel<KS, C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
+            if (e != cudaSuccess) { set_last_error("dwconv_ln_silu smem attr: %s", cudaGetErrorString(e)); return (int)e; }
+            set[dev] = true;
+        }
+    }
+    launch_pdl(dwconv_ln_silu_wide_kernel<KS, C>, grid, dim3(DW_WARPS * 32), dyn, st, args...);
+    return check_launch("dwconv_ln_silu_wide_kernel");
+}
+
 }  // namespace masr
 
 using namespace masr;
@@ -154,9 +294,26 @@ extern "C" int masr_dwconv_ln_silu_strided_f32(const float* g, int64_t ldg, int6
                                                int lpad, int stride, int out_rows, float eps, void* stream) {
     if (B == 0 || out_rows == 0) return MASR_OK;
     MASR_REQUIRE(g && w && bias && ln_gamma && ln_beta && (y || (yh && yl)) && in_lens, "masr_dwconv_ln_silu_f32: null pointer");
-    MASR_REQUIRE(C == 256, "masr_dwconv_ln_silu_f32: C=%d unsupported (this build: 256)", C);
+    MASR_REQUIRE(C == 256 || (C == 512 && stride == 1),
+                 "masr_dwconv_ln_silu_f32: C=%d unsupported (this build: 256, and 512 at stride 1)", C);
     MASR_REQUIRE(ldg % 4 == 0 && ldy % 4 == 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0,
                  "masr_dwconv_ln_silu_f32: rows must be 16-byte aligned (ldg, ldy multiples of 4)");
+    if (C == 512) {
+        dim3 wgrid((out_rows + DW_TW * DW_WARPS - 1) / (DW_TW * DW_WARPS), B);
+        cudaStream_t wst = (cudaStream_t)stream;
+#define MASR_DW_WIDE(KS)                                                                                                        \
+    return launch_dw_wide<KS, 512>(wgrid, wst, g, ldg, g_bstride, w, bias, ln_gamma, ln_beta, pad_vec, y, (__half*)yh, (__half*)yl, \
+                                   ldy, y_bstride, in_lens, lpad, out_rows, eps)
+        switch (kernel_size) {
+            case 7: MASR_DW_WIDE(7);
+            case 15: MASR_DW_WIDE(15);
+            case 31: MASR_DW_WIDE(31);
+            default:
+                set_last_error("masr_dwconv_ln_silu_f32: unsupported kernel size %d (7/15/31)", kernel_size);
+                return MASR_ERR_INVALID_ARGUMENT;
+        }
+#undef MASR_DW_WIDE
+    }
     const int tw = dw_tw();
     const int TT = tw * DW_WARPS;
     dim3 grid((out_rows + TT - 1) / TT, B);

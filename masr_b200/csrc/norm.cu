@@ -1,4 +1,4 @@
-// Row LayerNorm over the model dimension (d = 256): one warp per row, 128-bit loads, two-pass
+// Row LayerNorm over the model dimension (d = 256 or 512): one warp per row, 128-bit loads, two-pass
 // statistics in registers (mean, then centred variance) — the numerically safe form.
 //
 // Replaces `torch.nn.LayerNorm(size, eps=1e-5)` at encoder.py:64-72,115,122,141,153,161,342 and
@@ -150,9 +150,13 @@ extern "C" int masr_layernorm2_split_f16(const float* x, int64_t ldx, const floa
     if (M == 0) return MASR_OK;
     MASR_REQUIRE(x && gamma1 && beta1 && y1 && gamma2 && beta2 && yh && yl, "masr_layernorm2_split_f16: null pointer");
     MASR_REQUIRE(ldx % 4 == 0 && ldy % 4 == 0, "masr_layernorm2_split_f16: leading dimensions must be multiples of 4");
-    MASR_REQUIRE(D == 256, "masr_layernorm2_split_f16: unsupported width D=%d (256)", D);
-    launch_pdl(layernorm2_kernel<256>, dim3((M + 7) / 8), dim3(256), 0, (cudaStream_t)stream, x, ldx, gamma1, beta1, y1, gamma2,
-               beta2, y2, (__half*)yh, (__half*)yl, ldy, M, eps);
+    MASR_REQUIRE(D == 256 || D == 512, "masr_layernorm2_split_f16: unsupported width D=%d (256/512)", D);
+    if (D == 256)
+        launch_pdl(layernorm2_kernel<256>, dim3((M + 7) / 8), dim3(256), 0, (cudaStream_t)stream, x, ldx, gamma1, beta1, y1, gamma2,
+                   beta2, y2, (__half*)yh, (__half*)yl, ldy, M, eps);
+    else
+        launch_pdl(layernorm2_kernel<512>, dim3((M + 7) / 8), dim3(256), 0, (cudaStream_t)stream, x, ldx, gamma1, beta1, y1, gamma2,
+                   beta2, y2, (__half*)yh, (__half*)yl, ldy, M, eps);
     return check_launch("layernorm2_kernel");
 }
 

@@ -575,6 +575,7 @@ tc_gemm_kernel(const __grid_constant__ TcMaps maps, TcParams p, int num_tiles, i
             constexpr uint32_t a_bytes = CONV ? CONV_ROWS * TBK * 2 : TILE_BYTES;
             constexpr uint32_t tx_bytes = 2 * a_bytes + 2 * TILE_BYTES;
             uint32_t kg = 0;
+            const int kb_tap = CONV ? p.N / TBK : 1;   // CONV: K-blocks per tap (K = 9 C, N = C: 8 at C = 256, 16 = two chunks at 512)
             if (lnp) mbar_wait(&ln_bar[0], 0);      // the consumer warps have written this CTA's A rows (LayerNorm prologue)
             for (int tile = tile_begin; tile < tile_end; tile += tile_stride) {
                 int n0, m0, t0, b;
@@ -589,7 +590,7 @@ tc_gemm_kernel(const __grid_constant__ TcMaps maps, TcParams p, int num_tiles, i
                     }
                     mbar_expect_tx(&full_bar[s], tx_bytes);
                     if (CONV) {
-                        const int tap = kb / CHUNK_KB, cj = kb % CHUNK_KB;   // K index = tap*256 + cj*32  (C = 256)
+                        const int tap = kb / kb_tap, cj = kb - tap * kb_tap;   // K index = tap*C + cj*32
                         const int kh = tap / 3, kw = tap - kh * 3;
                         const int plane = (kh & 1) * 2 + (kw & 1);
                         tma_load_4d(&maps.a[2 * plane], &full_bar[s], st, cj * TBK, kw >> 1, t0 + (kh >> 1), b);
@@ -997,7 +998,7 @@ extern "C" int masr_conv2_tc_f16x2(const void* c1h, const void* c1l, const void*
                                    float* out, void* outh, void* outl, int B, int F1, int T2, int C, void* stream) {
     if (B == 0 || T2 == 0) return MASR_OK;
     MASR_REQUIRE(c1h && c1l && Wh && Wl && (out || (outh && outl)), "masr_conv2_tc_f16x2: null pointer");
-    MASR_REQUIRE(C == 256, "masr_conv2_tc_f16x2: C=%d unsupported (this build: 256)", C);
+    MASR_REQUIRE(C == 256 || C == 512, "masr_conv2_tc_f16x2: C=%d unsupported (this build: 256/512)", C);
     const int TH = (F1 + 1) / 2;
     TcMaps maps;
     memset(&maps, 0, sizeof(maps));

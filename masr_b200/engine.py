@@ -111,6 +111,7 @@ class ConformerEngine:
         self.d2h_bytes = 0
         self.last_gain = None
         self.prof: Optional[Dict[str, list]] = None      # tag -> [(start_event, end_event)], see profile()
+        self._ln_tmp: Optional[torch.Tensor] = None      # see _ln_split
         self.graph_tail_hook = None                      # callable(ws) appended to the captured device step (see _graph_for)
         self._precompute_pos()
         self._tcw = {}
@@ -263,8 +264,16 @@ class ConformerEngine:
         self._tc(yp, d, W, bias, M, N, d, epi, C=C, Cp=Cp, ldc=ldc, tag=tag)
 
     def _ln_split(self, x, gb, yp, M):
-        self._k("layernorm", "masr_layernorm_split_f16", _p(x), self.d, _p(gb[0]), _p(gb[1]), _p(yp[0]), _p(yp[1]),
-                self.d, M, self.d, 1e-5)
+        """yp <- pair(LN(x; gb)).  d = 256: one launch.  d = 512: masr_layernorm_split_f16 has no 512-wide form, so the row goes
+        through masr_layernorm_f32 into `self._ln_tmp` (an fp32 [M, d] scratch of the running step, set by its driver) and
+        masr_split_f16 — the same rounding steps, hence the same pair, in two launches."""
+        if self.d == 256:
+            self._k("layernorm", "masr_layernorm_split_f16", _p(x), self.d, _p(gb[0]), _p(gb[1]), _p(yp[0]), _p(yp[1]),
+                    self.d, M, self.d, 1e-5)
+            return
+        tmp = self._ln_tmp
+        self._ln(x, gb, tmp, M)
+        self._k("layernorm", "masr_split_f16", _p(tmp), _p(yp[0]), _p(yp[1]), M * self.d)
 
     # ------------------------------------------------------------------------------------------
     def _stream(self):
@@ -539,6 +548,7 @@ class ConformerEngine:
         w, d, tw = self.w, self.d, self._tcw
         x, g, qkv = ws["x"], ws["g"], ws["qkv"]
         t0p, t1p, c1p, c2p = ws["t0p"], ws["t1p"], ws["c1p"], ws["c2p"]
+        self._ln_tmp = ws["t1"]                       # fp32 scratch of _ln_split at d = 512 (not otherwise used on this path)
         # the FFN modules: one fused launch each (masr_ffn_tc_f16x2), or w_1 + w_2 through the hidden pair
         ffn_fused = self._ffn_fused()
         hidp = None if ffn_fused else self._hidp(ws)
@@ -1379,6 +1389,9 @@ class EfficientConformerEngine(ConformerEngine):
                 L.ptab = torch.empty(pe2.shape[0], self.d, device=self.device, dtype=torch.float32)
                 self._gemm(pe2, self.d, L.wpos, None, L.ptab, self.d, pe2.shape[0], self.d, self.d)
         torch.cuda.synchronize(self.device)
+
+    def _pack(self, sd, max_len):
+        return pack_conformer(sd, self.device, max_len, family="efficient_conformer")
 
     def final_len(self, t: int) -> int:
         return (t + 1) // 2

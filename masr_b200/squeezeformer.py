@@ -14,7 +14,7 @@ import torch
 
 from ._lib import EPI_BIAS, EPI_BIAS_GLU, EPI_BIAS_SILU, EPI_RESIDUAL
 from .engine import ConformerEngine, _p, subsampled_len
-from .weights import sinusoid_table
+from .weights import check_supported, sinusoid_table
 
 
 @dataclass
@@ -80,6 +80,7 @@ class SqueezeWeights:
 
 def pack_squeezeformer(sd: Dict[str, torch.Tensor], device, max_len: int = 5000, bn_eps: float = 1e-5) -> SqueezeWeights:
     dev = torch.device(device)
+    check_supported(sd, "squeezeformer")
 
     def D(t):
         return t.contiguous().to(dev)

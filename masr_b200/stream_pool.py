@@ -210,6 +210,7 @@ class ConformerStreamPool(_PoolBase):
         M = S * C
         F1 = (CHUNK_FRAMES - 1) // 2
         x, t0, t0p, t1p, hidp, qkv, qkvp, g, xcp = b["x"], b["t0"], b["t0p"], b["t1p"], b["hidp"], b["qkv"], b["qkvp"], b["g"], b["xcp"]
+        eng._ln_tmp = t0                              # scratch of eng._ln_split at d = 512: t0 is live only from norm_conv to its copy into xcat
         eng._k("conv1", "masr_conv1_cmvn_relu_planes_f16", _p(feats), _p(w.cmvn_mean), _p(w.cmvn_istd), _p(w.conv1_w), _p(w.conv1_b),
                _p(b["c1p"][0]), _p(b["c1p"][1]), S, CHUNK_FRAMES, w.idim, F1, eng.w1_cols, d)
         eng._k("conv2", "masr_conv2_tc_f16x2", _p(b["c1p"][0]), _p(b["c1p"][1]), _p(tw["conv2"][0]), _p(tw["conv2"][1]), _p(w.conv2_b),

@@ -120,7 +120,7 @@ def check_supported(sd: Dict[str, torch.Tensor], family: str = "conformer") -> N
     (the packers read architecture from tensor names and shapes): ``cnn_module_norm='batch_norm'`` in a Conformer /
     EfficientConformer (convolution.py:60-63: same ``conv_module.norm.weight`` key as the LayerNorm variant, plus running
     statistics), ``input_layer`` conv2d6 / conv2d8 (subsampling.py:115-236: extra ``embed.conv.4``), attention heads that
-    are not 64 wide.  A DeepSpeech2 checkpoint is an LSTM one (``encoder.rnns.{l}.rnn.*``, 4H gate rows) or a GRU one
+    are not 64 wide, model widths without kernels (Conformer: 256 and 512; Squeezeformer, EfficientConformer: 256).  A DeepSpeech2 checkpoint is an LSTM one (``encoder.rnns.{l}.rnn.*``, 4H gate rows) or a GRU one
     (``use_gru: True``: the reference's ``GRU`` wrapper nests ``nn.GRU`` one level deeper, ``encoder.rnns.{l}.rnn.rnn.*``,
     3H gate rows; deepspeech2/encoder.py:24-33, gru.py:6-15); 3H-row tensors under the LSTM names are no layout the
     reference writes."""
@@ -140,17 +140,24 @@ def check_supported(sd: Dict[str, torch.Tensor], family: str = "conformer") -> N
             raise UnsupportedConfig(f"unsupported layout: {hh.shape[0]}-row recurrent weights under the GRU key names "
                                     "(use_gru=True: 3 gates)")
         return
+    dn = sd.get("encoder.after_norm.weight", sd.get("encoder.preln.weight"))
     u = sd.get("encoder.encoders.0.self_attn.pos_bias_u")
-    if u is not None:
-        d = sd["encoder.after_norm.weight"].shape[0]
+    if u is not None and dn is not None:
+        d = dn.shape[0]
         if d % u.shape[0] or d // u.shape[0] != 64:
             raise UnsupportedConfig(f"unsupported config: attention heads of width {d / u.shape[0]:g} (this build: d_k = 64, "
                                     "e.g. output_size 256 / attention_heads 4)")
+    if dn is not None:
+        d = dn.shape[0]
+        widths = (256, 512) if family == "conformer" else (256,)
+        if d not in widths:
+            raise UnsupportedConfig(f"unsupported config: output_size {d} for {family} (this build has kernels for "
+                                    f"output_size {' and '.join(str(x) for x in widths)})")
 
 
-def pack_conformer(sd: Dict[str, torch.Tensor], device, max_len: int = 5000) -> ConformerWeights:
+def pack_conformer(sd: Dict[str, torch.Tensor], device, max_len: int = 5000, family: str = "conformer") -> ConformerWeights:
     dev = torch.device(device)
-    check_supported(sd, "conformer")
+    check_supported(sd, family)
 
     def D(t):
         return t.contiguous().to(dev)
