@@ -479,6 +479,75 @@ int masr_ctc_prefix_beam_lm_pool(const int* cand_id, const float* cand_logp, con
                                  int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int* fresh, int* out_tok,
                                  int64_t tok_stride, int* out_n, float* out_score, float* out_approx, void* stream);
 
+/* ---- word n-gram LM fusion (ARPA) with the lexicon constraint -------------------------------------------
+ * The external Scorer for a WORD-based LM (English models: configs/english_example.yml): the LM scores a word once, when
+ * the <space> after it is emitted, and every hypothesis is limited to words of a lexicon built from the LM's unigrams
+ * (the library's OpenFST dictionary).  PARITY UNPINNED (library absent): semantics per oracle/word_lm.py (DESIGN.md §2).
+ *
+ * Word ids are 24 bits (lexicon words 0 .. dict_size-1 in unigram file order, <s> = dict_size, </s> = dict_size + 1),
+ * packed 24 bits each into the 4-word key, so orders 1..5 and at most 2^24 - 1 declared unigrams are accepted.
+ * The lexicon: every unigram except <s>, </s>, <unk> whose code points are each a model token, as a trie over token ids
+ * (node 0 = root, nodes in insertion order); its arcs in CSR form, ascending token within a node. */
+typedef struct masr_word_lm_tables {
+    const uint32_t* keys;     /* device: 4 words per slot (n word ids, 24 bits each from bit 0)                 */
+    const float* vals;        /* device: 2 floats per slot: ln p, ln backoff                                    */
+    const int* lex_off;       /* device [nodes + 1]: first arc of each lexicon node                             */
+    const int* lex_tok;       /* device [arcs]: token of each arc                                               */
+    const int* lex_next;      /* device [arcs]: node each arc leads to                                          */
+    const int* lex_word;      /* device [nodes]: word id ending at the node, -1 if none                         */
+    int order;                /* N, 1..5                                                                        */
+    int bos, eos;             /* word ids of <s>, </s>                                                          */
+    int vocab;                /* V                                                                              */
+    int space;                /* token id of <space>                                                            */
+    int root;                 /* lexicon root node (0)                                                          */
+    int nodes;                /* lexicon nodes                                                                  */
+    int dict_size;            /* lexicon words                                                                  */
+    int64_t off[8];           /* off[n]: first slot of the order-n table (n = 1..order)                         */
+    int64_t mask[8];          /* mask[n]: slots of the order-n table - 1 (a power of two - 1)                   */
+} masr_word_lm_tables;
+
+/* info_host[32] written by masr_word_lm_info: the masr_lm_info layout (KEY_WORDS, READ, KEPT, ... of the word tables;
+ * CHAR_BASED = 0, DICT_SIZE = lexicon words) plus these */
+enum { MASR_WORD_LM_INFO_NODES = 27, MASR_WORD_LM_INFO_ARCS = 28, MASR_WORD_LM_INFO_SPACE = 29 };
+
+/* Parse a word-based plain-text ARPA file against the vocabulary (as masr_lm_load_arpa).  Rejects, besides every case
+ * masr_lm_load_arpa rejects: a character-based file, a vocabulary without "<space>", an order above 5 and more than
+ * 2^24 - 1 declared unigrams.  n-grams with a word outside the lexicon (other than <s>, </s>) are dropped. */
+int masr_word_lm_load_arpa(const char* path_host, const char* vocab_host, int V, void** handle_host);
+int masr_word_lm_info(const void* handle_host, int64_t* info_host);
+/* copy the tables and the lexicon (sizes from masr_word_lm_info) into host buffers and fill layout_host (all but the
+ * six pointers); the handle is released with masr_lm_free */
+int masr_word_lm_export(const void* handle_host, uint32_t* keys_host, float* vals_host, int* lex_off_host, int* lex_tok_host,
+                        int* lex_next_host, int* lex_word_host, masr_word_lm_tables* layout_host);
+/* Q queries of lnP(word | window) over word ids: ctx [Q, order-1] (oldest first) and word [Q]; -1 = out of vocabulary */
+int masr_word_lm_score_f32(const masr_word_lm_tables* lm_host, const int* ctx, const int* word, int Q, float* out, void* stream);
+
+/* masr_ctc_prefix_beam_lm with a word LM: an extension by <space> adds alpha * lnP(word just completed | the N-1 words
+ * before it) + beta, any other extension adds nothing; extensions the lexicon rejects contribute nothing (after <space>,
+ * a prefix's first attempt in candidate order is rejected and resets it to the lexicon root, once).  After the last frame
+ * every non-empty prefix not ending in <space> gets alpha * lnP(its last word | h) + beta (-1000 for lnP of a partial
+ * word) on the side; the best of those adjusted scores is reported (out_score) with its approx_ctc (out_approx).
+ * The word-LM forms also keep one flag per trie node in trie_tok[trie_cap/5, 2*trie_cap/5) of each utterance.
+ * Same workspace as masr_ctc_prefix_beam; the streaming and pool forms size their state with
+ * masr_ctc_prefix_beam_wordlm_state_size and are otherwise as masr_ctc_prefix_beam_lm_stream / _lm_pool. */
+int masr_ctc_prefix_beam_wordlm(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
+                                int64_t bstride, const int* lens, int B, int beam_size, int blank,
+                                const masr_word_lm_tables* lm_host, float alpha, float beta, float* pool, int* trie_parent,
+                                int* trie_tok, int64_t trie_cap, int* out_tok, int64_t tok_stride, int* out_n, float* out_score,
+                                float* out_approx, void* stream);
+int masr_ctc_prefix_beam_wordlm_state_size(int64_t* ints_per_utt, int64_t* floats_per_utt);
+int masr_ctc_prefix_beam_wordlm_stream(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
+                                       int64_t bstride, const int* lens, int B, int beam_size, int blank,
+                                       const masr_word_lm_tables* lm_host, float alpha, float beta, float* pool,
+                                       int* trie_parent, int* trie_tok, int64_t trie_cap, int* state_i, float* state_f,
+                                       int resume, int* out_tok, int64_t tok_stride, int* out_n, float* out_score,
+                                       float* out_approx, void* stream);
+int masr_ctc_prefix_beam_wordlm_pool(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
+                                     int64_t bstride, const int* lens, int B, int beam_size, int blank,
+                                     const masr_word_lm_tables* lm_host, float alpha, float beta, float* pool, int* trie_parent,
+                                     int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int* fresh, int* out_tok,
+                                     int64_t tok_stride, int* out_n, float* out_score, float* out_approx, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

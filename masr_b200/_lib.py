@@ -26,8 +26,19 @@ class LmTables(C.Structure):
 
 
 _lmp = C.POINTER(LmTables)
+
+
+class WordLmTables(C.Structure):
+    """``masr_word_lm_tables`` of include/masr_b200.h."""
+    _fields_ = [("keys", _vp), ("vals", _vp), ("lex_off", _vp), ("lex_tok", _vp), ("lex_next", _vp), ("lex_word", _vp),
+                ("order", _i), ("bos", _i), ("eos", _i), ("vocab", _i), ("space", _i), ("root", _i), ("nodes", _i),
+                ("dict_size", _i), ("off", _i64 * 8), ("mask", _i64 * 8)]
+
+
+_wlmp = C.POINTER(WordLmTables)
 LM_INFO_ORDER, LM_INFO_CHAR_BASED, LM_INFO_DICT_SIZE, LM_INFO_VOCAB, LM_INFO_KEY_WORDS, LM_INFO_VAL_FLOATS = range(6)
 LM_INFO_READ, LM_INFO_KEPT, LM_INFO_SLOTS, LM_INFO_TABLE_BYTES = 8, 14, 20, 26
+WORD_LM_INFO_NODES, WORD_LM_INFO_ARCS, WORD_LM_INFO_SPACE = 27, 28, 29
 
 # name -> argtypes, exactly the declarations of include/masr_b200.h
 SIGNATURES = {
@@ -104,6 +115,17 @@ SIGNATURES = {
                                   _vp],
     "masr_ctc_prefix_beam_lm_pool": [_vp, _vp, _vp, _vp, _i64, _vp, _i, _i, _i, _lmp, _f, _f, _vp, _vp, _vp, _i64, _vp, _vp, _vp,
                                      _vp, _i64, _vp, _vp, _vp, _vp],
+    "masr_word_lm_load_arpa": [_vp, _vp, _i, C.POINTER(_vp)],
+    "masr_word_lm_info": [_vp, C.POINTER(_i64)],
+    "masr_word_lm_export": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _wlmp],
+    "masr_word_lm_score_f32": [_wlmp, _vp, _vp, _i, _vp, _vp],
+    "masr_ctc_prefix_beam_wordlm": [_vp, _vp, _vp, _vp, _i64, _vp, _i, _i, _i, _wlmp, _f, _f, _vp, _vp, _vp, _i64, _vp, _i64, _vp,
+                                    _vp, _vp, _vp],
+    "masr_ctc_prefix_beam_wordlm_state_size": [C.POINTER(_i64), C.POINTER(_i64)],
+    "masr_ctc_prefix_beam_wordlm_stream": [_vp, _vp, _vp, _vp, _i64, _vp, _i, _i, _i, _wlmp, _f, _f, _vp, _vp, _vp, _i64, _vp, _vp,
+                                           _i, _vp, _i64, _vp, _vp, _vp, _vp],
+    "masr_ctc_prefix_beam_wordlm_pool": [_vp, _vp, _vp, _vp, _i64, _vp, _i, _i, _i, _wlmp, _f, _f, _vp, _vp, _vp, _i64, _vp, _vp,
+                                         _vp, _vp, _i64, _vp, _vp, _vp, _vp],
 }
 
 

@@ -179,19 +179,34 @@ struct BeamSharedLm : BeamShared {
     uint16_t ctx[BEAM_CAP][LM_CTX], s_ctx[BEAM_CAP][LM_CTX];
 };
 
+// The word-LM instantiation: each beam entry carries its window of the N-1 completed words before its current word and
+// its lexicon state (a lexicon node, LEX_AFTER_SPACE, or the root 0 after a reset); k0 = the candidate of this frame whose
+// attempt resets an entry in LEX_AFTER_SPACE (-1: none).
+struct BeamSharedWord : BeamShared {
+    uint32_t wctx[BEAM_CAP][WLM_CTX], s_wctx[BEAM_CAP][WLM_CTX];
+    int lex[BEAM_CAP], s_lex[BEAM_CAP], k0[BEAM_CAP];
+};
+
+enum : int { BEAM_PLAIN = 0, BEAM_CHAR_LM = 1, BEAM_WORD_LM = 2 };
+template <int MODE> struct BeamSmem { using type = BeamShared; };
+template <> struct BeamSmem<BEAM_CHAR_LM> { using type = BeamSharedLm; };
+template <> struct BeamSmem<BEAM_WORD_LM> { using type = BeamSharedWord; };
+
 struct LmSearch {
     masr_lm_tables lm;
     const float* blank_lp;                       // ln p_blank per frame, rows as cand_cnt
     float alpha, beta;
     float* out_approx;                           // [B]
+    masr_word_lm_tables wlm;                     // BEAM_WORD_LM
 };
 
 constexpr int LM_STATE_INTS = 3 * BEAM_CAP + 2 + BEAM_CAP * LM_CTX / 2;   // + the windows, two ids per int
+constexpr int WLM_STATE_INTS = 3 * BEAM_CAP + 2 + BEAM_CAP * (WLM_CTX + 1);   // + the word windows and lexicon states
 
 // pool layout: [0, BEAM_CAP) existing prefixes (rank order), then BEAM_CAP + i*K + k children of (rank i, candidate k);
 // K = this frame's candidate count (usually a handful, cutoff_prob 0.99), so the pool the selection scans is 512 + beam*K
 // entries, not 512 + beam*40
-template <bool LM, bool POOL = false>
+template <int MODE, bool POOL = false>
 __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
     const int* __restrict__ cand_id, const float* __restrict__ cand_logp, const int* __restrict__ cand_cnt, int64_t bstride,
     const int* __restrict__ lens, int beam, int blank, float* __restrict__ pool_all, int* __restrict__ trie_parent,
@@ -210,7 +225,12 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
     // when it marks a slot fresh (one memset of the slot's hash range instead of hcap stores by one CTA, which would hold up
     // every other slot of the launch).  A slot with no frames this launch (lens[b] == 0) returns at once: its state, trie
     // and outputs stay byte for byte as they were.
-    using Shared = typename std::conditional<LM, BeamSharedLm, BeamShared>::type;
+    // WORD (per oracle/word_lm.py): only an extension by <space> gets the LM term, (base + alpha lnP(word | h)) + beta;
+    // the lexicon rejects extensions (pool entry -inf); an entry in LEX_AFTER_SPACE loses its first attempt of a frame
+    // and is reset to the root, a flag kept with its trie node (tflag) so the reset persists if the node drops out of the
+    // beam and comes back; after the last frame a read-out term is added on the side to pick and report the best entry.
+    constexpr bool LM = MODE != BEAM_PLAIN, CHAR = MODE == BEAM_CHAR_LM, WORD = MODE == BEAM_WORD_LM;
+    using Shared = typename BeamSmem<MODE>::type;
     extern __shared__ __align__(16) uint8_t smem_beam[];
     Shared& S = *reinterpret_cast<Shared*>(smem_beam);
     const int b = blockIdx.x, tid = threadIdx.x;
@@ -226,8 +246,9 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
     const int64_t node_cap = trie_cap / 5;
     const uint32_t hcap = (uint32_t)(trie_cap - node_cap);
     int* thash = tpar + node_cap;
+    int* tflag = ttok + node_cap;                                   // WORD: per node, 1 = reset after <space>
     int nbeam = 1, nnodes = 1;
-    int* st_i = state_i ? state_i + (int64_t)b * (LM ? LM_STATE_INTS : 3 * BEAM_CAP + 2) : nullptr;
+    int* st_i = state_i ? state_i + (int64_t)b * (WORD ? WLM_STATE_INTS : LM ? LM_STATE_INTS : 3 * BEAM_CAP + 2) : nullptr;
     float* st_f = state_f ? state_f + (int64_t)b * (3 * BEAM_CAP) : nullptr;
     bool cont;
     if constexpr (POOL) cont = fresh[b] == 0;
@@ -238,7 +259,13 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
         if (tid < nbeam) {
             S.node[tid] = st_i[tid]; S.par[tid] = st_i[BEAM_CAP + tid]; S.last[tid] = st_i[2 * BEAM_CAP + tid];
             S.pb[tid] = st_f[tid]; S.pnb[tid] = st_f[BEAM_CAP + tid]; S.score[tid] = st_f[2 * BEAM_CAP + tid];
-            if constexpr (LM) {
+            if constexpr (WORD) {
+                const int* w = st_i + 3 * BEAM_CAP + 2 + tid * (WLM_CTX + 1);
+#pragma unroll
+                for (int j = 0; j < WLM_CTX; ++j) S.wctx[tid][j] = (uint32_t)w[j];
+                S.lex[tid] = w[WLM_CTX];
+            }
+            if constexpr (CHAR) {
                 const int* w = st_i + 3 * BEAM_CAP + 2 + tid * (LM_CTX / 2);
 #pragma unroll
                 for (int j = 0; j < LM_CTX / 2; ++j) {
@@ -254,7 +281,13 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
         if (tid == 0) {
             S.node[0] = 0; S.par[0] = -1; S.last[0] = -1; S.pb[0] = 0.f; S.pnb[0] = -INFINITY; S.score[0] = 0.f;
             tpar[0] = -1; ttok[0] = -1;
-            if constexpr (LM) {
+            if constexpr (WORD) {
+#pragma unroll
+                for (int j = 0; j < WLM_CTX; ++j) S.wctx[0][j] = (uint32_t)lms.wlm.bos;
+                S.lex[0] = 0;
+                tflag[0] = 0;
+            }
+            if constexpr (CHAR) {
 #pragma unroll
                 for (int j = 0; j < LM_CTX; ++j) S.ctx[0][j] = (uint16_t)lms.lm.bos;
             }
@@ -283,14 +316,19 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
             while (atomicCAS(&S.hkey[h], -1, S.node[tid]) != -1) h = (h + 1) & (2 * BEAM_CAP - 1);
             S.hval[h] = tid;
             float nb = -INFINITY, nnb = -INFINITY;
+            int k0 = -1;                                           // first attempt (non-blank, past the cut)
             for (int k = 0; k < K; ++k) {
                 if constexpr (LM) {
                     if (__fadd_rn(S.clp[k], S.score[tid]) < cut) continue;
                 }
                 if (S.cid[k] == blank) nb = logaddexp_f(nb, S.score[tid] + S.clp[k]);
-                else if (S.cid[k] == S.last[tid]) nnb = logaddexp_f(nnb, S.pnb[tid] + S.clp[k]);
+                else {
+                    if (k0 < 0) k0 = k;
+                    if (S.cid[k] == S.last[tid]) nnb = logaddexp_f(nnb, S.pnb[tid] + S.clp[k]);
+                }
             }
             S.nb[tid] = nb; S.nnb[tid] = nnb;
+            if constexpr (WORD) S.k0[tid] = S.lex[tid] == LEX_AFTER_SPACE ? k0 : -1;
         }
         __syncthreads();
         // extensions: child (rank i, candidate k)
@@ -304,7 +342,22 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
             float add;
             if (c == S.last[i]) add = S.pb[i] == -INFINITY ? -INFINITY : S.pb[i] + S.clp[k];
             else add = S.score[i] + S.clp[k];
-            if constexpr (LM) {
+            if constexpr (WORD) {                  // the attempt: lexicon acceptance (repeats with p_b = -inf count)
+                int st = S.lex[i];
+                if (st == LEX_AFTER_SPACE) {
+                    if (k == S.k0[i]) continue;                        // rejected; the entry is reset below
+                    st = 0;                                            // later attempts of this frame: from the root
+                }
+                if (c == lms.wlm.space) {
+                    const int wid = st > 0 ? __ldg(lms.wlm.lex_word + st) : -1;
+                    if (wid < 0) continue;
+                    if (add != -INFINITY)
+                        add = __fadd_rn(__fadd_rn(add, __fmul_rn(lms.alpha, wlm_lnp(lms.wlm, S.wctx[i], (uint32_t)wid))), lms.beta);
+                } else if (lex_child(lms.wlm, st, c) < 0) {
+                    continue;
+                }
+            }
+            if constexpr (CHAR) {
                 if (add != -INFINITY) {
                     const float lnp = lm_lnp(lms.lm, S.ctx[i], lm_word(lms.lm, c));
                     add = __fadd_rn(__fadd_rn(add, __fmul_rn(lms.alpha, lnp)), lms.beta);
@@ -313,6 +366,12 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
             pool[BEAM_CAP + i * K + k] = add;
         }
         __syncthreads();
+        if constexpr (WORD) {                      // the reset of an entry's first attempt after <space>: once, with its node
+            if (tid < nbeam && S.k0[tid] >= 0) {
+                S.lex[tid] = 0;
+                if (S.node[tid] < node_cap) tflag[S.node[tid]] = 1;
+            }
+        }
         // children that already exist as beam entries: fold their contribution into that entry (one pair per entry)
         if (tid < nbeam && S.par[tid] >= 0) {
             uint32_t h = ((uint32_t)S.par[tid] * 2654435761u) & (2 * BEAM_CAP - 1);
@@ -448,7 +507,12 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
                 S.s_node[tid] = S.node[src]; S.s_par[tid] = S.par[src]; S.s_last[tid] = S.last[src];
                 S.s_pb[tid] = S.nb[src]; S.s_pnb[tid] = S.nnb[src];
                 S.s_src[tid] = -1;
-                if constexpr (LM) {
+                if constexpr (WORD) {
+#pragma unroll
+                    for (int j = 0; j < WLM_CTX; ++j) S.s_wctx[tid][j] = S.wctx[src][j];
+                    S.s_lex[tid] = S.lex[src];
+                }
+                if constexpr (CHAR) {
 #pragma unroll
                     for (int j = 0; j < LM_CTX; ++j) S.s_ctx[tid][j] = S.ctx[src][j];
                 }
@@ -457,7 +521,20 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
                 S.s_node[tid] = -1; S.s_par[tid] = S.node[i]; S.s_last[tid] = S.cid[k];
                 S.s_pb[tid] = -INFINITY; S.s_pnb[tid] = pool[src];
                 S.s_src[tid] = 1;
-                if constexpr (LM) {                   // window of l+c = window of l shifted by one + c
+                if constexpr (WORD) {                 // <space>: the completed word enters the window; a letter: a lexicon arc
+                    const int st = S.lex[i], c = S.cid[k];
+                    const int n1 = lms.wlm.order - 1;
+                    if (c == lms.wlm.space) {
+                        for (int j = 0; j + 1 < n1; ++j) S.s_wctx[tid][j] = S.wctx[i][j + 1];
+                        if (n1 > 0) S.s_wctx[tid][n1 - 1] = (uint32_t)__ldg(lms.wlm.lex_word + st);
+                        S.s_lex[tid] = LEX_AFTER_SPACE;
+                    } else {
+#pragma unroll
+                        for (int j = 0; j < WLM_CTX; ++j) S.s_wctx[tid][j] = S.wctx[i][j];
+                        S.s_lex[tid] = lex_child(lms.wlm, st, c);
+                    }
+                }
+                if constexpr (CHAR) {                 // window of l+c = window of l shifted by one + c
                     const int n1 = lms.lm.order - 1;
                     for (int j = 0; j + 1 < n1; ++j) S.s_ctx[tid][j] = S.ctx[i][j + 1];
                     if (n1 > 0) S.s_ctx[tid][n1 - 1] = lm_word(lms.lm, S.cid[k]);
@@ -479,6 +556,9 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
             }
             S.s_node[tid] = found;
             need_new = found < 0;
+            if constexpr (WORD) {                     // a prefix that comes back keeps its reset
+                if (found >= 0 && found < node_cap && tflag[found]) S.s_lex[tid] = 0;
+            }
         }
         int new_total;
         {
@@ -497,6 +577,7 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
             if (id < node_cap) {
                 const int par = S.s_par[tid], tok = S.s_last[tid];
                 tpar[id] = par; ttok[id] = tok;
+                if constexpr (WORD) tflag[id] = 0;
                 uint32_t h = (((uint32_t)par * 2654435761u) ^ ((uint32_t)tok * 40503u)) % hcap;
                 while (atomicCAS(&thash[h], -1, id) != -1) h = h + 1 == hcap ? 0 : h + 1;
             }
@@ -506,7 +587,12 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
         if (tid < n_sel) {
             S.node[tid] = S.s_node[tid]; S.par[tid] = S.s_par[tid]; S.last[tid] = S.s_last[tid];
             S.pb[tid] = S.s_pb[tid]; S.pnb[tid] = S.s_pnb[tid]; S.score[tid] = S.r_score[tid];
-            if constexpr (LM) {
+            if constexpr (WORD) {
+#pragma unroll
+                for (int j = 0; j < WLM_CTX; ++j) S.wctx[tid][j] = S.s_wctx[tid][j];
+                S.lex[tid] = S.s_lex[tid];
+            }
+            if constexpr (CHAR) {
 #pragma unroll
                 for (int j = 0; j < LM_CTX; ++j) S.ctx[tid][j] = S.s_ctx[tid][j];
             }
@@ -519,7 +605,13 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
         if (tid < nbeam) {
             st_i[tid] = S.node[tid]; st_i[BEAM_CAP + tid] = S.par[tid]; st_i[2 * BEAM_CAP + tid] = S.last[tid];
             st_f[tid] = S.pb[tid]; st_f[BEAM_CAP + tid] = S.pnb[tid]; st_f[2 * BEAM_CAP + tid] = S.score[tid];
-            if constexpr (LM) {
+            if constexpr (WORD) {
+                int* w = st_i + 3 * BEAM_CAP + 2 + tid * (WLM_CTX + 1);
+#pragma unroll
+                for (int j = 0; j < WLM_CTX; ++j) w[j] = (int)S.wctx[tid][j];
+                w[WLM_CTX] = S.lex[tid];
+            }
+            if constexpr (CHAR) {
                 int* w = st_i + 3 * BEAM_CAP + 2 + tid * (LM_CTX / 2);
 #pragma unroll
                 for (int j = 0; j < LM_CTX / 2; ++j) w[j] = (int)((unsigned)S.ctx[tid][2 * j] | ((unsigned)S.ctx[tid][2 * j + 1] << 16));
@@ -527,12 +619,46 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
         }
         if (tid == 0) { st_i[3 * BEAM_CAP] = nbeam; st_i[3 * BEAM_CAP + 1] = nnodes; }
     }
+    // the entry to report: rank 0, or (WORD) the best after the read-out term, which is computed on the side (the state
+    // saved above never sees it): alpha lnP(last word | h) + beta for every non-empty entry not ending in <space>
+    int best = 0;
+    float best_sc = nbeam > 0 ? S.score[0] : -INFINITY;
+    if constexpr (WORD) {
+        float a = -INFINITY;
+        int ai = 0x7fffffff;
+        if (tid < nbeam) {
+            a = S.score[tid];
+            ai = tid;
+            if (S.par[tid] >= 0 && S.last[tid] != lms.wlm.space) {
+                const int st = S.lex[tid];
+                const int wid = st > 0 ? __ldg(lms.wlm.lex_word + st) : -1;
+                const float lnp = wlm_lnp(lms.wlm, S.wctx[tid], wid < 0 ? WLM_OOV : (uint32_t)wid);
+                a = __fadd_rn(a, __fadd_rn(__fmul_rn(lms.alpha, lnp), lms.beta));
+            }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float oa = __shfl_xor_sync(0xffffffffu, a, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, ai, o);
+            if (oa > a || (oa == a && oi < ai)) { a = oa; ai = oi; }
+        }
+        __syncthreads();                                   // (s_score / scan are free again)
+        if ((tid & 31) == 0) { S.s_score[tid >> 5] = a; S.scan[tid >> 5] = ai; }
+        __syncthreads();
+        if (tid == 0 && nbeam > 0) {
+            a = S.s_score[0]; ai = S.scan[0];
+            for (int w = 1; w < BEAM_THREADS / 32; ++w)
+                if (S.s_score[w] > a || (S.s_score[w] == a && S.scan[w] < ai)) { a = S.s_score[w]; ai = S.scan[w]; }
+            best = ai;
+            best_sc = a;
+        }
+    }
     if (tid == 0) {
         int n = 0;
         float sc = -INFINITY;
         if (nbeam > 0) {
-            sc = S.score[0];
-            int node = S.node[0];
+            sc = best_sc;
+            int node = S.node[best];
             int len = 0;
             for (int x = node; x > 0 && x < node_cap; x = tpar[x]) ++len;
             n = len;
@@ -541,7 +667,40 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
         }
         out_n[b] = n;
         out_score[b] = sc;
-        if constexpr (LM) {
+        if constexpr (WORD) {
+            // approx_ctc: score' - len * beta - alpha * lnP(sentence) over the words split on <space> (a trailing partial
+            // word is one; a partial that is not a word end is out of vocabulary)
+            float apx = sc;
+            if (nbeam > 0) {
+                const masr_word_lm_tables& lm = lms.wlm;
+                const int n1 = lm.order - 1;
+                uint32_t win[WLM_CTX];
+#pragma unroll
+                for (int j = 0; j < WLM_CTX; ++j) win[j] = (uint32_t)lm.bos;
+                float s = 0.f;
+                int nw = 0, ln = 0;
+                for (int p = 0; p <= n; ++p) {
+                    const int tok = p < n ? out_tok[(int64_t)b * tok_stride + p] : lm.space;
+                    if (tok != lm.space) {
+                        ln = ln >= 0 ? lex_child(lm, ln, tok) : -1;
+                        continue;
+                    }
+                    if (ln == 0) continue;                              // (no letters since the last <space>)
+                    const int wid = ln > 0 ? __ldg(lm.lex_word + ln) : -1;
+                    const uint32_t w = wid < 0 ? WLM_OOV : (uint32_t)wid;
+                    s = __fadd_rn(s, wlm_lnp(lm, win, w));
+                    for (int j = 0; j + 1 < n1; ++j) win[j] = win[j + 1];
+                    if (n1 > 0) win[n1 - 1] = w;
+                    ++nw;
+                    ln = 0;
+                }
+                if (nw == 0) s = wlm_lnp(lm, win, (uint32_t)lm.bos);
+                s = __fadd_rn(s, wlm_lnp(lm, win, (uint32_t)lm.eos));
+                apx = __fsub_rn(__fsub_rn(sc, __fmul_rn((float)n, lms.beta)), __fmul_rn(lms.alpha, s));
+            }
+            lms.out_approx[b] = apx;
+        }
+        if constexpr (CHAR) {
             // approx_ctc: score - len * beta - alpha * lnP(sentence), sentence = <s>^(N-1) tokens </s> (<s>^N </s> if empty)
             float apx = sc;
             if (nbeam > 0) {
@@ -613,11 +772,11 @@ extern "C" int masr_ctc_prefix_beam(const int* cand_id, const float* cand_logp, 
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) dev = 0;
     if (!attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BeamShared));
+        cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<BEAM_PLAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BeamShared));
         if (e != cudaSuccess) { set_last_error("prefix_beam smem attr: %s", cudaGetErrorString(e)); return (int)e; }
         attr_set[dev] = true;
     }
-    prefix_beam_kernel<false><<<B, BEAM_THREADS, sizeof(BeamShared), (cudaStream_t)stream>>>(
+    prefix_beam_kernel<BEAM_PLAIN><<<B, BEAM_THREADS, sizeof(BeamShared), (cudaStream_t)stream>>>(
         cand_id, cand_logp, cand_cnt, bstride, lens, beam_size, blank, pool, trie_parent, trie_tok, trie_cap, out_tok, tok_stride,
         out_n, out_score, nullptr, nullptr, 0, LmSearch{}, nullptr);
     return check_launch("prefix_beam_kernel");
@@ -643,9 +802,9 @@ extern "C" int masr_ctc_prefix_beam_stream(const int* cand_id, const float* cand
     MASR_REQUIRE(cand_id && cand_logp && cand_cnt && lens && pool && trie_parent && trie_tok && out_tok && out_n && out_score &&
                  state_i && state_f, "masr_ctc_prefix_beam_stream: null pointer");
     MASR_REQUIRE(beam_size >= 1 && beam_size <= BEAM_CAP, "masr_ctc_prefix_beam_stream: beam_size=%d out of range (1..%d)", beam_size, BEAM_CAP);
-    cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BeamShared));
+    cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<BEAM_PLAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BeamShared));
     if (e != cudaSuccess) { set_last_error("prefix_beam smem attr: %s", cudaGetErrorString(e)); return (int)e; }
-    prefix_beam_kernel<false><<<B, BEAM_THREADS, sizeof(BeamShared), (cudaStream_t)stream>>>(
+    prefix_beam_kernel<BEAM_PLAIN><<<B, BEAM_THREADS, sizeof(BeamShared), (cudaStream_t)stream>>>(
         cand_id, cand_logp, cand_cnt, bstride, lens, beam_size, blank, pool, trie_parent, trie_tok, trie_cap, out_tok, tok_stride,
         out_n, out_score, state_i, state_f, resume, LmSearch{}, nullptr);
     return check_launch("prefix_beam_kernel<stream>");
@@ -657,15 +816,15 @@ extern "C" int masr_ctc_prefix_beam_stream(const int* cand_id, const float* cand
 // before its next launch.  Slots with lens[b] == 0 are left untouched (state, trie and outputs).  Every argument that varies
 // between launches is device data, so the launch can be captured once into a CUDA graph and replayed.
 // The function attribute is set once per device (not while a graph is being captured).
-template <bool LM>
+template <int MODE>
 static int pool_smem_attr() {
-    using Shared = typename std::conditional<LM, BeamSharedLm, BeamShared>::type;
+    using Shared = typename BeamSmem<MODE>::type;
     static bool done[64] = {};
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) dev = 0;
     if (!done[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<LM, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Shared));
+        cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<MODE, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Shared));
         if (e != cudaSuccess) { set_last_error("prefix_beam<pool> smem attr: %s", cudaGetErrorString(e)); return (int)e; }
         done[dev] = true;
     }
@@ -680,9 +839,9 @@ extern "C" int masr_ctc_prefix_beam_pool(const int* cand_id, const float* cand_l
     MASR_REQUIRE(cand_id && cand_logp && cand_cnt && lens && pool && trie_parent && trie_tok && out_tok && out_n && out_score &&
                  state_i && state_f && fresh, "masr_ctc_prefix_beam_pool: null pointer");
     MASR_REQUIRE(beam_size >= 1 && beam_size <= BEAM_CAP, "masr_ctc_prefix_beam_pool: beam_size=%d out of range (1..%d)", beam_size, BEAM_CAP);
-    const int rc = pool_smem_attr<false>();
+    const int rc = pool_smem_attr<BEAM_PLAIN>();
     if (rc) return rc;
-    prefix_beam_kernel<false, true><<<B, BEAM_THREADS, sizeof(BeamShared), (cudaStream_t)stream>>>(
+    prefix_beam_kernel<BEAM_PLAIN, true><<<B, BEAM_THREADS, sizeof(BeamShared), (cudaStream_t)stream>>>(
         cand_id, cand_logp, cand_cnt, bstride, lens, beam_size, blank, pool, trie_parent, trie_tok, trie_cap, out_tok, tok_stride,
         out_n, out_score, state_i, state_f, 0, LmSearch{}, fresh);
     return check_launch("prefix_beam_kernel<pool>");
@@ -702,14 +861,14 @@ static int launch_beam_lm(const char* what, const int* cand_id, const float* can
     MASR_REQUIRE(beam_size >= 1 && beam_size <= BEAM_CAP, "%s: beam_size=%d out of range (1..%d)", what, beam_size, BEAM_CAP);
     if constexpr (POOL) {
         MASR_REQUIRE(state_i && state_f && fresh, "%s: null pointer", what);
-        const int rc = pool_smem_attr<true>();
+        const int rc = pool_smem_attr<BEAM_CHAR_LM>();
         if (rc) return rc;
     } else {
-        cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BeamSharedLm));
+        cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<BEAM_CHAR_LM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BeamSharedLm));
         if (e != cudaSuccess) { set_last_error("prefix_beam<lm> smem attr: %s", cudaGetErrorString(e)); return (int)e; }
     }
     const LmSearch lms{*lm, blank_logp, alpha, beta, out_approx};
-    prefix_beam_kernel<true, POOL><<<B, BEAM_THREADS, sizeof(BeamSharedLm), stream>>>(
+    prefix_beam_kernel<BEAM_CHAR_LM, POOL><<<B, BEAM_THREADS, sizeof(BeamSharedLm), stream>>>(
         cand_id, cand_logp, cand_cnt, bstride, lens, beam_size, blank, pool, trie_parent, trie_tok, trie_cap, out_tok, tok_stride,
         out_n, out_score, state_i, state_f, resume, lms, fresh);
     return check_launch(what);
@@ -754,4 +913,84 @@ extern "C" int masr_ctc_prefix_beam_lm_pool(const int* cand_id, const float* can
     return launch_beam_lm<true>("masr_ctc_prefix_beam_lm_pool", cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size,
                                 blank, lm_host, alpha, beta, pool, trie_parent, trie_tok, trie_cap, state_i, state_f, 0, out_tok,
                                 tok_stride, out_n, out_score, out_approx, (cudaStream_t)stream, fresh);
+}
+
+// ---- with a word LM and its lexicon (oracle/word_lm.py) ----
+template <bool POOL = false>
+static int launch_beam_wordlm(const char* what, const int* cand_id, const float* cand_logp, const int* cand_cnt,
+                              const float* blank_logp, int64_t bstride, const int* lens, int B, int beam_size, int blank,
+                              const masr_word_lm_tables* lm, float alpha, float beta, float* pool, int* trie_parent,
+                              int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int resume, int* out_tok,
+                              int64_t tok_stride, int* out_n, float* out_score, float* out_approx, cudaStream_t stream,
+                              int* fresh = nullptr) {
+    MASR_REQUIRE(cand_id && cand_logp && cand_cnt && blank_logp && lens && pool && trie_parent && trie_tok && out_tok && out_n &&
+                 out_score && out_approx && lm, "%s: null pointer", what);
+    MASR_REQUIRE(lm->keys && lm->vals && lm->lex_off && lm->lex_word && lm->nodes >= 1 && (lm->lex_tok || lm->nodes == 1) &&
+                 (lm->lex_next || lm->nodes == 1), "%s: word LM tables not set", what);
+    MASR_REQUIRE(lm->order >= 1 && lm->order <= WLM_MAX_ORDER, "%s: word LM order %d out of range (1..%d)", what, lm->order,
+                 WLM_MAX_ORDER);
+    MASR_REQUIRE(lm->space >= 0 && lm->space != blank, "%s: <space> token %d invalid", what, lm->space);
+    MASR_REQUIRE(beam_size >= 1 && beam_size <= BEAM_CAP, "%s: beam_size=%d out of range (1..%d)", what, beam_size, BEAM_CAP);
+    if constexpr (POOL) {
+        MASR_REQUIRE(state_i && state_f && fresh, "%s: null pointer", what);
+        const int rc = pool_smem_attr<BEAM_WORD_LM>();
+        if (rc) return rc;
+    } else {
+        cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<BEAM_WORD_LM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)sizeof(BeamSharedWord));
+        if (e != cudaSuccess) { set_last_error("prefix_beam<wordlm> smem attr: %s", cudaGetErrorString(e)); return (int)e; }
+    }
+    LmSearch lms{};
+    lms.blank_lp = blank_logp;
+    lms.alpha = alpha;
+    lms.beta = beta;
+    lms.out_approx = out_approx;
+    lms.wlm = *lm;
+    prefix_beam_kernel<BEAM_WORD_LM, POOL><<<B, BEAM_THREADS, sizeof(BeamSharedWord), stream>>>(
+        cand_id, cand_logp, cand_cnt, bstride, lens, beam_size, blank, pool, trie_parent, trie_tok, trie_cap, out_tok, tok_stride,
+        out_n, out_score, state_i, state_f, resume, lms, fresh);
+    return check_launch(what);
+}
+
+extern "C" int masr_ctc_prefix_beam_wordlm(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
+                                           int64_t bstride, const int* lens, int B, int beam_size, int blank,
+                                           const masr_word_lm_tables* lm_host, float alpha, float beta, float* pool,
+                                           int* trie_parent, int* trie_tok, int64_t trie_cap, int* out_tok, int64_t tok_stride,
+                                           int* out_n, float* out_score, float* out_approx, void* stream) {
+    if (B == 0) return MASR_OK;
+    return launch_beam_wordlm("masr_ctc_prefix_beam_wordlm", cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size,
+                              blank, lm_host, alpha, beta, pool, trie_parent, trie_tok, trie_cap, nullptr, nullptr, 0, out_tok,
+                              tok_stride, out_n, out_score, out_approx, (cudaStream_t)stream);
+}
+
+extern "C" int masr_ctc_prefix_beam_wordlm_state_size(int64_t* ints_per_utt, int64_t* floats_per_utt) {
+    MASR_REQUIRE(ints_per_utt && floats_per_utt, "masr_ctc_prefix_beam_wordlm_state_size: null pointer");
+    *ints_per_utt = WLM_STATE_INTS;
+    *floats_per_utt = 3 * BEAM_CAP;
+    return MASR_OK;
+}
+
+extern "C" int masr_ctc_prefix_beam_wordlm_stream(const int* cand_id, const float* cand_logp, const int* cand_cnt,
+                                                  const float* blank_logp, int64_t bstride, const int* lens, int B, int beam_size,
+                                                  int blank, const masr_word_lm_tables* lm_host, float alpha, float beta,
+                                                  float* pool, int* trie_parent, int* trie_tok, int64_t trie_cap, int* state_i,
+                                                  float* state_f, int resume, int* out_tok, int64_t tok_stride, int* out_n,
+                                                  float* out_score, float* out_approx, void* stream) {
+    if (B == 0) return MASR_OK;
+    MASR_REQUIRE(state_i && state_f, "masr_ctc_prefix_beam_wordlm_stream: null pointer");
+    return launch_beam_wordlm("masr_ctc_prefix_beam_wordlm_stream", cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B,
+                              beam_size, blank, lm_host, alpha, beta, pool, trie_parent, trie_tok, trie_cap, state_i, state_f,
+                              resume, out_tok, tok_stride, out_n, out_score, out_approx, (cudaStream_t)stream);
+}
+
+extern "C" int masr_ctc_prefix_beam_wordlm_pool(const int* cand_id, const float* cand_logp, const int* cand_cnt,
+                                                const float* blank_logp, int64_t bstride, const int* lens, int B, int beam_size,
+                                                int blank, const masr_word_lm_tables* lm_host, float alpha, float beta, float* pool,
+                                                int* trie_parent, int* trie_tok, int64_t trie_cap, int* state_i, float* state_f,
+                                                int* fresh, int* out_tok, int64_t tok_stride, int* out_n, float* out_score,
+                                                float* out_approx, void* stream) {
+    if (B == 0) return MASR_OK;
+    return launch_beam_wordlm<true>("masr_ctc_prefix_beam_wordlm_pool", cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B,
+                                    beam_size, blank, lm_host, alpha, beta, pool, trie_parent, trie_tok, trie_cap, state_i,
+                                    state_f, 0, out_tok, tok_stride, out_n, out_score, out_approx, (cudaStream_t)stream, fresh);
 }

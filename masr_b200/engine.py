@@ -658,9 +658,10 @@ class ConformerEngine:
                  cutoff_prob: float = 0.99, cutoff_top_n: int = 40, lm=None, alpha: float = 0.0, beta: float = 0.0):
         """`ctc_beam_search_decoding(probs, vocab, beam_size, cutoff_prob, cutoff_top_n, scorer, blank_id=0)` of the
         reference's external decoder (masr/decoders/swig_wrapper.py:35-64) for a whole batch on the GPU -> device tensors
-        (tokens [B,T], count [B], log-score [B]).  ``lm`` (a masr_b200.lm.CharLM, or None): shallow fusion with weight
-        ``alpha`` and insertion bonus ``beta``; the log-score is then the reference's approx_ctc (the fused score with the
-        LM terms taken out again; the fused score is in ws["beam_score"]).  Parity unpinned (DESIGN.md)."""
+        (tokens [B,T], count [B], log-score [B]).  ``lm`` (a masr_b200.lm.CharLM or WordLM, or None): shallow fusion with
+        weight ``alpha`` and insertion bonus ``beta`` (a WordLM scores per word and constrains the words to its lexicon); the
+        log-score is then the reference's approx_ctc (the fused score with the LM terms taken out again; the fused score is
+        in ws["beam_score"]).  Parity unpinned (DESIGN.md)."""
         B = len(out_lens)
         M = B * T
         dev = self.device
@@ -685,7 +686,7 @@ class ConformerEngine:
                 ws["beam_approx"] = torch.zeros_like(ws["beam_score"])
             self._k("ctc_topk", "masr_ctc_topk_blank_f32", _p(logits), self.Vpad, M, self.V, int(cutoff_top_n), float(cutoff_prob),
                     0, _p(ws["cand_id"]), _p(ws["cand_lp"]), _p(ws["cand_n"]), _p(ws["blank_lp"]))
-            self._k("prefix_beam", "masr_ctc_prefix_beam_lm", _p(ws["cand_id"]), _p(ws["cand_lp"]), _p(ws["cand_n"]),
+            self._k("prefix_beam", lm.BEAM, _p(ws["cand_id"]), _p(ws["cand_lp"]), _p(ws["cand_n"]),
                     _p(ws["blank_lp"]), T, _p(ws["tlens"]), B, int(beam_size), 0, _lib.C.byref(lm.tables(dev)), float(alpha),
                     float(beta), _p(ws["beam_pool"]), _p(ws["trie_par"]), _p(ws["trie_tok"]), ws["trie_cap"], _p(ws["beam_tok"]),
                     ws["beam_tok"].shape[1], _p(ws["beam_n"]), _p(ws["beam_score"]), _p(ws["beam_approx"]))
@@ -727,6 +728,7 @@ class ConformerEngine:
         call."""
         dev = self.device
         lm_t = _lib.C.byref(lm.tables(dev)) if lm is not None else None
+        lm_beam = lm.BEAM if lm is not None else None
         main = torch.cuda.current_stream(dev)
         if getattr(self, "_beam_stream", None) is None:
             self._beam_stream = torch.cuda.Stream(device=dev)
@@ -795,7 +797,7 @@ class ConformerEngine:
                                     _p(slot["tlens"]), B, int(beam_size), 0, _p(slot["pool"]), _p(slot["trie_par"]), _p(slot["trie_tok"]),
                                     slot["trie_cap"], _p(slot["tok"]), slot["tok"].shape[1], _p(slot["n"]), _p(slot["sc"]))
                         else:                      # the reported score is approx_ctc (see ctc_beam)
-                            self._k("prefix_beam", "masr_ctc_prefix_beam_lm", _p(slot["cand_id"]), _p(slot["cand_lp"]),
+                            self._k("prefix_beam", lm_beam, _p(slot["cand_id"]), _p(slot["cand_lp"]),
                                     _p(slot["cand_n"]), _p(slot["blank_lp"]), T, _p(slot["tlens"]), B, int(beam_size), 0, lm_t,
                                     float(alpha), float(beta), _p(slot["pool"]), _p(slot["trie_par"]), _p(slot["trie_tok"]),
                                     slot["trie_cap"], _p(slot["tok"]), slot["tok"].shape[1], _p(slot["n"]), _p(slot["fused"]),
@@ -1292,8 +1294,9 @@ class StreamBeam:
     """Streaming CTC prefix beam search of ONE stream on the GPU — ``BeamSearchDecoder.decode_chunk / reset_decoder``
     (masr/decoders/beam_search_decoder.py:75-96, called at masr/predict.py:322,353): the beam, the prefix trie and its hash
     stay on the device between chunks (masr_ctc_prefix_beam_stream), so after every chunk the best prefix equals the
-    whole-utterance search over all frames seen so far.  ``lm`` / ``alpha`` / ``beta``: shallow fusion of a character LM as
-    in ConformerEngine.ctc_beam (each beam entry's LM window is part of the device state); the score is then approx_ctc.
+    whole-utterance search over all frames seen so far.  ``lm`` / ``alpha`` / ``beta``: shallow fusion of a character or
+    word LM as in ConformerEngine.ctc_beam (each beam entry's LM window, and with a word LM its lexicon state, is part of
+    the device state); the score is then approx_ctc.
     Parity unpinned (DESIGN.md)."""
 
     def __init__(self, eng: "ConformerEngine", beam_size: int = 300, cutoff_prob: float = 0.99, cutoff_top_n: int = 40,
@@ -1304,7 +1307,7 @@ class StreamBeam:
         dev, C = eng.device, _lib.C
         pool_n, trie_n, si, sf = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_int64(0)
         call("masr_ctc_prefix_beam_workspace", 1, self.max_frames, C.byref(pool_n), C.byref(trie_n))
-        call("masr_ctc_prefix_beam_lm_state_size" if lm is not None else "masr_ctc_prefix_beam_state_size", C.byref(si), C.byref(sf))
+        call(lm.BEAM + "_state_size" if lm is not None else "masr_ctc_prefix_beam_state_size", C.byref(si), C.byref(sf))
         i32, f32 = torch.int32, torch.float32
         self.cand_id = torch.empty(self.max_chunk, 40, device=dev, dtype=i32)
         self.cand_lp = torch.empty(self.max_chunk, 40, device=dev, dtype=f32)
@@ -1345,7 +1348,7 @@ class StreamBeam:
         self.lens.fill_(rows)
         n_view = self.out[1:2].view(torch.int32)
         if lm:
-            eng._k("prefix_beam", "masr_ctc_prefix_beam_lm_stream", _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n),
+            eng._k("prefix_beam", self.lm.BEAM + "_stream", _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n),
                    _p(self.blank_lp), self.max_chunk, _p(self.lens), 1, self.beam, 0, self.lm_t, self.alpha, self.beta,
                    _p(self.pool), _p(self.trie_par), _p(self.trie_tok), self.trie_cap, _p(self.state_i), _p(self.state_f),
                    1 if self.frames else 0, _p(self.out_tok), self.out_tok.shape[1], _p(n_view), _p(self.fused), _p(self.out[0:1]))

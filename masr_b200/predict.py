@@ -106,9 +106,10 @@ class MASRPredictor:
         self.lm = None
         if self.configs.decoder == 'ctc_beam_search':
             # GPU prefix beam search: whole-utterance calls (engine.ctc_beam) and streaming (engine.StreamBeam =
-            # BeamSearchDecoder.decode_chunk / reset_decoder).  With a character-based ARPA file at language_model_path the
-            # LM is fused into the search (the reference's Scorer, beam_search_decoder.py:28-37) and the score is
-            # approx_ctc; otherwise the search runs without LM and reports the beam's log score.
+            # BeamSearchDecoder.decode_chunk / reset_decoder).  With an ARPA file at language_model_path the LM (character-based,
+            # or word-based with its lexicon when the vocabulary has <space>) is fused into the search (the reference's
+            # Scorer, beam_search_decoder.py:28-37) and the score is approx_ctc; otherwise the search runs without LM and
+            # reports the beam's log score.
             bc = dict(self.configs.get('ctc_beam_search_decoder_conf', {}) or {})
             self._beam_conf = {'beam_size': int(bc.get('beam_size', 300)), 'cutoff_prob': float(bc.get('cutoff_prob', 0.99)),
                                'cutoff_top_n': int(bc.get('cutoff_top_n', 40))}
@@ -144,9 +145,10 @@ class MASRPredictor:
 
     # ---------------------------------------------------------------------------------------------
     def _load_lm(self, bc):
-        """The CharLM at ``language_model_path`` when that is a character-based ARPA file (judged by content, not by
-        extension), loaded once; else None with a warning that names the reason."""
-        from .lm import CharLM, sniff
+        """The LM at ``language_model_path`` when that is a plain-text ARPA file (judged by content, not by extension),
+        loaded once: a CharLM for a character-based file, a WordLM (lexicon-constrained, scored per word) for a word-based
+        one when the vocabulary has ``<space>``; else None with a warning that names the reason."""
+        from .lm import CharLM, WordLM, sniff
         path = bc.get('language_model_path') or ''
         kind = sniff(path)
         reason = {'missing': f'language model {path!r} not found',
@@ -154,9 +156,13 @@ class MASRPredictor:
                   'unknown': f'{path!r} is not an ARPA file'}.get(kind)
         lm = None
         if reason is None:
-            lm = CharLM(path, self._text_featurizer.vocab_list)
+            vocab = self._text_featurizer.vocab_list
+            lm = CharLM(path, vocab)
             if not lm.is_character_based:
-                reason, lm = f'{path!r} is a word-based LM; only character-based LMs are supported', None
+                if '<space>' not in vocab:
+                    reason, lm = f'{path!r} is a word-based LM and the vocabulary has no <space> token', None
+                else:
+                    lm = WordLM(path, vocab)
         if lm is None:
             logger.warning(f'ctc_beam_search: {reason}: GPU prefix beam search without LM (alpha/beta ignored)')
             return None
@@ -360,7 +366,7 @@ class MASRPredictor:
 
     def create_stream_pool(self, n_slots: int, max_frames: int = 3000):
         """Additive: a ``StreamPool`` of ``n_slots`` concurrent streams over this predictor's model, decoding as the YAML
-        says — greedy, or the GPU prefix beam search with the character LM this predictor loaded (if any).  Each slot's
+        says — greedy, or the GPU prefix beam search with the character or word LM this predictor loaded (if any).  Each slot's
         ``push`` results equal ``predict_stream`` on that stream alone.  ``max_frames``: encoder frames one stream may reach
         before it must be reset (40 ms each; 3000 = 2 minutes)."""
         if not self.configs.streaming:

@@ -622,12 +622,12 @@ class PoolBeam:
     reference's ``BeamSearchDecoder.decode_chunk / reset_decoder`` per stream, beam_search_decoder.py:75-96).
 
     Each pool step adds two launches, captured into the step's CUDA graph with the encoder: the top-k candidates of all
-    ``S * OUT_ROWS`` CTC-head rows (``pool.b["logits"]``), then ``masr_ctc_prefix_beam[_lm]_pool`` with one CTA per slot
+    ``S * OUT_ROWS`` CTC-head rows (``pool.b["logits"]``), then ``masr_ctc_prefix_beam[_lm|_wordlm]_pool`` with one CTA per slot
     over that slot's valid rows (the length row of the pool's device ``meta``).  Slots without frames in a step are not
     touched.  Per slot the beam, its trie and the trie's hash stay on the device, so after every step a slot's best
     prefix equals the whole-utterance search over its frames since the last ``reset`` — what ``predict_stream`` returns.
     The trie is sized by ``beam_size`` and the pool's frame capacity (at most ``beam_size`` new prefixes per frame), so
-    no stream the pool accepts can overflow it.  ``lm`` / ``alpha`` / ``beta``: character-LM shallow fusion as in
+    no stream the pool accepts can overflow it.  ``lm`` / ``alpha`` / ``beta``: character- or word-LM shallow fusion as in
     ``StreamBeam``; the reported score is then approx_ctc."""
 
     def __init__(self, pool, beam_size: int = 300, cutoff_prob: float = 0.99, cutoff_top_n: int = 40, lm=None,
@@ -647,7 +647,7 @@ class PoolBeam:
         self.frames = pool.cap * R // CHUNK_OUT + 1
         pool_n, trie_n, si, sf = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_int64(0)
         call("masr_ctc_prefix_beam_workspace", S, 1, C.byref(pool_n), C.byref(trie_n))
-        call("masr_ctc_prefix_beam_lm_state_size" if lm is not None else "masr_ctc_prefix_beam_state_size", C.byref(si), C.byref(sf))
+        call(lm.BEAM + "_state_size" if lm is not None else "masr_ctc_prefix_beam_state_size", C.byref(si), C.byref(sf))
         self.trie_cap = 5 * (self.frames * beam_size + 1)          # nodes + 4 hash slots per node; the kernel reads node_cap = cap / 5
         i32, f32 = torch.int32, torch.float32
         self.cand_id = torch.zeros(S * R, 40, device=dev, dtype=i32)
@@ -679,7 +679,7 @@ class PoolBeam:
         if self.lm is not None:
             eng._k("ctc_topk", "masr_ctc_topk_blank_f32", _p(logits), eng.Vpad, S * R, eng.V, self.top_n, self.cutoff, 0,
                    _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n), _p(self.blank_lp))
-            eng._k("prefix_beam", "masr_ctc_prefix_beam_lm_pool", _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n),
+            eng._k("prefix_beam", self.lm.BEAM + "_pool", _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n),
                    _p(self.blank_lp), R, self.lens, S, self.beam, 0, self.lm_t, self.alpha, self.beta,
                    _p(self.scratch), _p(self.trie_par), _p(self.trie_tok), self.trie_cap, _p(self.state_i), _p(self.state_f),
                    _p(self.fresh), _p(self.out_tok), self.frames, _p(n_view), _p(self.out[2]), _p(self.out[0]))
@@ -729,7 +729,7 @@ class StreamPool:
                  target_db: float = -20.0, max_frames: int = 3000, beam: Optional[dict] = None, use_graph: bool = True,
                  resample: bool = False):
         """``beam``: None decodes greedily (``ctc_greedy``); a dict ``{beam_size, cutoff_prob, cutoff_top_n, lm, alpha,
-        beta}`` (``MASRPredictor``'s ``ctc_beam_search`` settings; ``lm`` a ``CharLM`` or None) runs the streaming prefix
+        beta}`` (``MASRPredictor``'s ``ctc_beam_search`` settings; ``lm`` a ``CharLM``, ``WordLM`` or None) runs the streaming prefix
         beam search of every slot on the GPU (``PoolBeam``), and every result is the beam's, as ``predict_stream`` with
         ``decoder: ctc_beam_search`` returns it.  ``use_graph=False`` launches every step eagerly instead of replaying
         its CUDA graph (same results).  ``resample``: accept pushes at other sample rates (``push(..., sample_rate=)``) and

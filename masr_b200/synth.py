@@ -291,6 +291,14 @@ def character_lm_arpa(path: str, seed: int = 0, order: int = 3, n_chars: int = 6
         for _ in range(m - 1):
             s.append(int(succ[s[-1], rng.choice(branch, p=weights)]) if rng.random() < 0.85 else int(rng.integers(0, n_chars)))
         sents.append(["<s>"] + [chars[i] for i in s] + ["</s>"])
+    _write_backoff_arpa(path, sents, chars + ["</s>", "<unk>"], order, discount)
+    return chars
+
+
+def _write_backoff_arpa(path: str, sents, words, order: int, discount: float, extra_unigrams=()):
+    """An absolute-discounting backoff LM of ``sents`` (lists ``<s> .. </s>``) over the unigram set ``words``, written as
+    ARPA with lmplz conventions (see character_lm_arpa).  ``extra_unigrams``: words appended to the unigram section, each
+    with the probability of an unseen word (the unigram distribution then no longer sums to 1)."""
     counts: List[Dict[tuple, int]] = [dict() for _ in range(order + 1)]
     for s in sents:
         for n in range(1, order + 1):
@@ -299,7 +307,6 @@ def character_lm_arpa(path: str, seed: int = 0, order: int = 3, n_chars: int = 6
                 if g[-1] == "<s>":
                     continue
                 counts[n][g] = counts[n].get(g, 0) + 1
-    words = chars + ["</s>", "<unk>"]
     N = sum(counts[1].values())
     prob: List[Dict[tuple, float]] = [dict() for _ in range(order + 1)]
     for w in words:
@@ -320,7 +327,7 @@ def character_lm_arpa(path: str, seed: int = 0, order: int = 3, n_chars: int = 6
             backoff[h] = (discount * n1p / ch) / (1.0 - lower)
     os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
     grams = [None] + [sorted(prob[n]) for n in range(1, order + 1)]
-    grams[1] = [("<s>",)] + grams[1]
+    grams[1] = [("<s>",)] + grams[1] + [(w,) for w in extra_unigrams]
     with open(path, "w", encoding="utf-8") as f:
         f.write("\\data\\\n")
         for n in range(1, order + 1):
@@ -328,13 +335,67 @@ def character_lm_arpa(path: str, seed: int = 0, order: int = 3, n_chars: int = 6
         for n in range(1, order + 1):
             f.write(f"\n\\{n}-grams:\n")
             for g in grams[n]:
-                p = -99.0 if g == ("<s>",) else math.log10(prob[n][g])
+                p = -99.0 if g == ("<s>",) else math.log10(prob[n][g] if g in prob[n] else 1.0 / (N + len(words)))
                 line = f"{p:.8g}\t{' '.join(g)}"
                 if n < order and g in backoff:
                     line += f"\t{math.log10(backoff[g]):.8g}"
                 f.write(line + "\n")
         f.write("\n\\end\\\n")
-    return chars
+
+
+ENGLISH_LETTERS = "abcdefghijklmnopqrstuvwxyz'"
+
+
+def english_vocabulary() -> List[str]:
+    """``<blank>``, ``<unk>``, a-z, ``'``, ``<space>``: the vocabulary of an English character model (30 tokens; ' ' is
+    written as ``<space>``, as TextFeaturizer does)."""
+    return ["<blank>", "<unk>"] + list(ENGLISH_LETTERS) + ["<space>"]
+
+
+def _letters(i: int) -> str:
+    s = ""
+    while True:
+        s = ENGLISH_LETTERS[i % 26] + s
+        i = i // 26 - 1
+        if i < 0:
+            return s
+
+
+def word_lm_arpa(path: str, seed: int = 0, order: int = 3, n_words: int = 200, n_sentences: int = 600, max_len: int = 12,
+                 discount: float = 0.5, branch: int = 4, extra_unigrams: int = 0) -> List[str]:
+    """Write a word n-gram LM as ARPA with lmplz conventions (the model of character_lm_arpa over words) and return its
+    corpus words.  The words are random a-z / ' strings; a fifth of them also occur without their last letter, so some
+    words are prefixes of others; four are not spellable with ``english_vocabulary()`` (a digit, an upper-case letter,
+    an accented letter, a '-') and stay in the corpus, so their n-grams exist but no hypothesis can reach them.
+    ``extra_unigrams``: that many more spellable unigrams (unseen in the corpus; e.g. > 65536 for the 24-bit word ids)."""
+    rng = np.random.default_rng(seed)
+    words: List[str] = []
+    seen = set()
+    while len(words) < n_words:
+        w = "".join(ENGLISH_LETTERS[i] for i in rng.integers(0, 26, int(rng.integers(1, 8))))
+        if rng.random() < 0.05 and len(w) > 2:
+            w = w[:2] + "'" + w[2:]
+        if w not in seen:
+            seen.add(w)
+            words.append(w)
+    for w in list(words[:n_words // 5]):
+        if len(w) >= 2 and w[:-1] not in seen:
+            seen.add(w[:-1])
+            words.append(w[:-1])
+    words += ["abc1", "Hello", "café", "x-ray"]
+    n = len(words)
+    succ = rng.integers(0, n, (n, branch))
+    weights = rng.dirichlet(np.ones(branch))
+    sents = []
+    for _ in range(n_sentences):
+        m = int(rng.integers(1, max_len + 1))
+        s = [int(rng.integers(0, n))]
+        for _ in range(m - 1):
+            s.append(int(succ[s[-1], rng.choice(branch, p=weights)]) if rng.random() < 0.85 else int(rng.integers(0, n)))
+        sents.append(["<s>"] + [words[i] for i in s] + ["</s>"])
+    extra = [f"qq'{_letters(i)}" for i in range(extra_unigrams)]
+    _write_backoff_arpa(path, sents, words + ["</s>", "<unk>"], order, discount, extra)
+    return words
 
 
 def noise_audio(seed: int, num_samples: int, sigma: float = 0.1) -> np.ndarray:
