@@ -1,0 +1,108 @@
+"""The GPU CTC prefix beam search (csrc/beam.cu) from the host: its device buffers and its two launches, for each of its
+three forms — one-shot (a batch of whole utterances), streaming (one stream fed chunk by chunk) and pool (every slot of a
+stream pool, launched inside the pool's CUDA graph) — without an LM, with a character LM or with a word LM.  Which entry
+point, which argument order and which buffers go with a (form, LM kind) is decided here and nowhere else."""
+from __future__ import annotations
+
+import ctypes as C
+import weakref
+
+import torch
+
+from ._lib import call
+
+BK_MAX = 40                                  # candidates per frame: the largest cutoff_top_n the top-k kernel takes
+ONE_SHOT, STREAM, POOL = "", "_stream", "_pool"      # the forms, named by their entry points' suffix
+
+
+class BeamSearch:
+    """One search's device buffers on ``device``.  ``topk`` launches the top-k kernel and ``search`` the prefix beam kernel,
+    both through ``eng._k`` of the engine passed in: two calls, so that a caller can put an event between them and run
+    ``search`` on another stream.  The search keeps no reference to the engine and only a weak one to the LM (whoever
+    launches it keeps the LM alive: the caller, or StreamBeam / PoolBeam), so an engine that keeps a search for reuse is
+    still freed as soon as it is dropped, and so is an LM its caller drops.
+
+    ``form``: ONE_SHOT, STREAM or POOL.  ``slots``: utterances (one CTA each); ``rows``: CTC-head rows the top-k kernel
+    writes (``cand_id`` / ``cand_lp`` [rows, BK_MAX], ``cand_n`` and, with an LM, ``blank_lp`` [rows]); ``max_frames``: the
+    most frames one slot searches (since its start or reset), which sizes its trie and its row of ``out_tok``.  ``lm``:
+    None, a ``lm.CharLM`` or a ``lm.WordLM``, fused with weight ``alpha`` and insertion bonus ``beta``.
+    The trie per slot is ``masr_ctc_prefix_beam_workspace(1, max_frames)`` (ONE_SHOT, STREAM), or 5 (max_frames *
+    beam_size + 1) for POOL, whose kernel never clears a slot's hash: it starts empty here and whoever resets a slot empties
+    its range again.  STREAM and POOL keep the beam of every slot in ``state_i`` / ``state_f``; POOL starts slot b afresh
+    while ``fresh[b]`` != 0.
+    Results: ``out_tok`` [slots, max_frames] and ``out`` [3, slots] = (``score``, ``count`` as int32 bits, fused score):
+    ``score`` is what the search reports (approx_ctc with an LM), ``fused`` the score the beam was ranked by (``score``
+    itself without an LM)."""
+
+    def __init__(self, device, form: str, slots: int, rows: int, max_frames: int, beam_size: int = 300,
+                 cutoff_prob: float = 0.99, cutoff_top_n: int = 40, lm=None, alpha: float = 0.0, beta: float = 0.0):
+        self.device, self.form, self.slots, self.max_frames = torch.device(device), form, int(slots), int(max_frames)
+        self.beam, self.cutoff, self.top_n = int(beam_size), float(cutoff_prob), int(cutoff_top_n)
+        self._lm, self.alpha, self.beta = None if lm is None else weakref.ref(lm), float(alpha), float(beta)
+        base = "masr_ctc_prefix_beam" if lm is None else lm.BEAM
+        self.name = base + form
+        dev, i32, f32, S = self.device, torch.int32, torch.float32, self.slots
+        pool_n, trie_n = C.c_int64(0), C.c_int64(0)
+        call("masr_ctc_prefix_beam_workspace", S, self.max_frames, C.byref(pool_n), C.byref(trie_n))
+        self.trie_cap = 5 * (self.max_frames * self.beam + 1) if form == POOL else trie_n.value
+        self.cand_id = torch.zeros(rows, BK_MAX, device=dev, dtype=i32)
+        self.cand_lp = torch.zeros(rows, BK_MAX, device=dev, dtype=f32)
+        self.cand_n = torch.zeros(rows, device=dev, dtype=i32)
+        self.blank_lp = None if lm is None else torch.zeros(rows, device=dev, dtype=f32)
+        if lm is not None:
+            lm.tables(dev)                                 # (uploaded here, never inside a graph capture)
+        self.scratch = torch.empty(pool_n.value, device=dev, dtype=f32)
+        if form == POOL:
+            self.trie_par = torch.full((S * self.trie_cap,), -1, device=dev, dtype=i32)
+        else:
+            self.trie_par = torch.empty(S * self.trie_cap, device=dev, dtype=i32)
+        self.trie_tok = torch.empty(S * self.trie_cap, device=dev, dtype=i32)
+        self.state_i = self.state_f = None
+        if form != ONE_SHOT:
+            si, sf = C.c_int64(0), C.c_int64(0)
+            call(base + "_state_size", C.byref(si), C.byref(sf))
+            self.state_i = torch.zeros(S, si.value, device=dev, dtype=i32)
+            self.state_f = torch.zeros(S, sf.value, device=dev, dtype=f32)
+        self.fresh = torch.ones(S, device=dev, dtype=i32) if form == POOL else None
+        self.out_tok = torch.zeros(S, self.max_frames, device=dev, dtype=i32)
+        self.out = torch.zeros(3, S, device=dev, dtype=f32)
+        self.score, self.count = self.out[0], self.out[1].view(i32)
+        self.fused = self.out[0] if lm is None else self.out[2]
+
+    @property
+    def lm(self):
+        """The LM this search fuses (None without one, or once its owner has dropped it)."""
+        return None if self._lm is None else self._lm()
+
+    def fits(self, slots: int, frames: int, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta) -> bool:
+        """Whether this search has room for ``slots`` utterances of ``frames`` frames and was built with these settings."""
+        return (self.slots >= slots and self.max_frames >= frames and (self._lm is None) == (lm is None) and self.lm is lm
+                and (self.beam, self.cutoff, self.top_n, self.alpha, self.beta)
+                == (int(beam_size), float(cutoff_prob), int(cutoff_top_n), float(alpha), float(beta)))
+
+    def topk(self, eng, logits: torch.Tensor, ld: int, rows: int):
+        """The candidates (and with an LM ln p_blank) of ``rows`` CTC-head rows of ``logits`` (row stride ``ld``)."""
+        cands = (self.cand_id.data_ptr(), self.cand_lp.data_ptr(), self.cand_n.data_ptr())
+        head = (logits.data_ptr(), ld, rows, eng.V, self.top_n, self.cutoff)
+        if self._lm is None:
+            eng._k("ctc_topk", "masr_ctc_topk_f32", *head, *cands)
+        else:
+            eng._k("ctc_topk", "masr_ctc_topk_blank_f32", *head, 0, *cands, self.blank_lp.data_ptr())
+
+    def search(self, eng, lens: int, B: int, bstride: int, resume: int = 0):
+        """The prefix beam search of slots 0..B-1 over candidate rows b * bstride + t, t < lens[b] (``lens``: the address
+        of a device int32 [B]).  ``resume`` (STREAM): 0 starts the stream at the root, else it continues from its state.
+        Host arguments only, no allocation or synchronisation: a POOL search can be captured into a CUDA graph."""
+        cands = (self.cand_id.data_ptr(), self.cand_lp.data_ptr(), self.cand_n.data_ptr())
+        if self._lm is None:
+            blank, fusion, scores = (), (), (self.score.data_ptr(),)
+        else:                        # the kernel writes the fused score to out_score and approx_ctc to out_approx
+            blank, fusion = (self.blank_lp.data_ptr(),), (C.byref(self.lm.tables(self.device)), self.alpha, self.beta)
+            scores = (self.fused.data_ptr(), self.score.data_ptr())
+        state = ()
+        if self.form != ONE_SHOT:
+            state = (self.state_i.data_ptr(), self.state_f.data_ptr(),
+                     self.fresh.data_ptr() if self.form == POOL else int(resume))
+        eng._k("prefix_beam", self.name, *cands, *blank, bstride, lens, B, self.beam, 0, *fusion, self.scratch.data_ptr(),
+               self.trie_par.data_ptr(), self.trie_tok.data_ptr(), self.trie_cap, *state, self.out_tok.data_ptr(),
+               self.max_frames, self.count.data_ptr(), *scores)

@@ -759,130 +759,11 @@ extern "C" int masr_ctc_prefix_beam_workspace(int B, int Tmax, int64_t* pool_flo
     return MASR_OK;
 }
 
-extern "C" int masr_ctc_prefix_beam(const int* cand_id, const float* cand_logp, const int* cand_cnt, int64_t bstride,
-                                    const int* lens, int B, int beam_size, int blank, float* pool, int* trie_parent,
-                                    int* trie_tok, int64_t trie_cap, int* out_tok, int64_t tok_stride, int* out_n,
-                                    float* out_score, void* stream) {
-    if (B == 0) return MASR_OK;
-    MASR_REQUIRE(cand_id && cand_logp && cand_cnt && lens && pool && trie_parent && trie_tok && out_tok && out_n && out_score,
-                 "masr_ctc_prefix_beam: null pointer");
-    MASR_REQUIRE(beam_size >= 1 && beam_size <= BEAM_CAP, "masr_ctc_prefix_beam: beam_size=%d out of range (1..%d)", beam_size, BEAM_CAP);
-    static bool attr_set[64] = {false};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) dev = 0;
-    if (!attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<BEAM_PLAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BeamShared));
-        if (e != cudaSuccess) { set_last_error("prefix_beam smem attr: %s", cudaGetErrorString(e)); return (int)e; }
-        attr_set[dev] = true;
-    }
-    prefix_beam_kernel<BEAM_PLAIN><<<B, BEAM_THREADS, sizeof(BeamShared), (cudaStream_t)stream>>>(
-        cand_id, cand_logp, cand_cnt, bstride, lens, beam_size, blank, pool, trie_parent, trie_tok, trie_cap, out_tok, tok_stride,
-        out_n, out_score, nullptr, nullptr, 0, LmSearch{}, nullptr);
-    return check_launch("prefix_beam_kernel");
-}
-
 extern "C" int masr_ctc_prefix_beam_state_size(int64_t* ints_per_utt, int64_t* floats_per_utt) {
     MASR_REQUIRE(ints_per_utt && floats_per_utt, "masr_ctc_prefix_beam_state_size: null pointer");
     *ints_per_utt = 3 * BEAM_CAP + 2;
     *floats_per_utt = 3 * BEAM_CAP;
     return MASR_OK;
-}
-
-// Streaming form (beam_search_decoder.py:75-96: CTCBeamSearchDecoder.next() + decode(), reset_state()): the same search
-// fed chunk by chunk.  `lens[b]` = frames of THIS chunk (0 = no new frames for that stream), `resume` = 0 starts a new
-// utterance (reset_decoder), != 0 continues from `state_*`; trie_parent / trie_tok must be sized for the whole stream
-// (masr_ctc_prefix_beam_workspace with Tmax = the longest stream in frames) and persist between calls.  Outputs = the best
-// prefix and its score after the frames seen so far — identical to one masr_ctc_prefix_beam call over the concatenation.
-extern "C" int masr_ctc_prefix_beam_stream(const int* cand_id, const float* cand_logp, const int* cand_cnt, int64_t bstride,
-                                           const int* lens, int B, int beam_size, int blank, float* pool, int* trie_parent,
-                                           int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int resume,
-                                           int* out_tok, int64_t tok_stride, int* out_n, float* out_score, void* stream) {
-    if (B == 0) return MASR_OK;
-    MASR_REQUIRE(cand_id && cand_logp && cand_cnt && lens && pool && trie_parent && trie_tok && out_tok && out_n && out_score &&
-                 state_i && state_f, "masr_ctc_prefix_beam_stream: null pointer");
-    MASR_REQUIRE(beam_size >= 1 && beam_size <= BEAM_CAP, "masr_ctc_prefix_beam_stream: beam_size=%d out of range (1..%d)", beam_size, BEAM_CAP);
-    cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<BEAM_PLAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BeamShared));
-    if (e != cudaSuccess) { set_last_error("prefix_beam smem attr: %s", cudaGetErrorString(e)); return (int)e; }
-    prefix_beam_kernel<BEAM_PLAIN><<<B, BEAM_THREADS, sizeof(BeamShared), (cudaStream_t)stream>>>(
-        cand_id, cand_logp, cand_cnt, bstride, lens, beam_size, blank, pool, trie_parent, trie_tok, trie_cap, out_tok, tok_stride,
-        out_n, out_score, state_i, state_f, resume, LmSearch{}, nullptr);
-    return check_launch("prefix_beam_kernel<stream>");
-}
-
-// Pool form (a stream pool's slots, each starting and ending utterances on its own): as masr_ctc_prefix_beam_stream with
-// `fresh[b]` (device) in place of `resume`.  fresh[b] != 0 starts slot b at the root and is cleared by the kernel; the caller
-// marks a slot fresh AND resets its hash range [b*trie_cap + trie_cap/5, (b+1)*trie_cap) of trie_parent to -1 (0xFF bytes)
-// before its next launch.  Slots with lens[b] == 0 are left untouched (state, trie and outputs).  Every argument that varies
-// between launches is device data, so the launch can be captured once into a CUDA graph and replayed.
-// The function attribute is set once per device (not while a graph is being captured).
-template <int MODE>
-static int pool_smem_attr() {
-    using Shared = typename BeamSmem<MODE>::type;
-    static bool done[64] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) dev = 0;
-    if (!done[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<MODE, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Shared));
-        if (e != cudaSuccess) { set_last_error("prefix_beam<pool> smem attr: %s", cudaGetErrorString(e)); return (int)e; }
-        done[dev] = true;
-    }
-    return MASR_OK;
-}
-
-extern "C" int masr_ctc_prefix_beam_pool(const int* cand_id, const float* cand_logp, const int* cand_cnt, int64_t bstride,
-                                         const int* lens, int B, int beam_size, int blank, float* pool, int* trie_parent,
-                                         int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int* fresh,
-                                         int* out_tok, int64_t tok_stride, int* out_n, float* out_score, void* stream) {
-    if (B == 0) return MASR_OK;
-    MASR_REQUIRE(cand_id && cand_logp && cand_cnt && lens && pool && trie_parent && trie_tok && out_tok && out_n && out_score &&
-                 state_i && state_f && fresh, "masr_ctc_prefix_beam_pool: null pointer");
-    MASR_REQUIRE(beam_size >= 1 && beam_size <= BEAM_CAP, "masr_ctc_prefix_beam_pool: beam_size=%d out of range (1..%d)", beam_size, BEAM_CAP);
-    const int rc = pool_smem_attr<BEAM_PLAIN>();
-    if (rc) return rc;
-    prefix_beam_kernel<BEAM_PLAIN, true><<<B, BEAM_THREADS, sizeof(BeamShared), (cudaStream_t)stream>>>(
-        cand_id, cand_logp, cand_cnt, bstride, lens, beam_size, blank, pool, trie_parent, trie_tok, trie_cap, out_tok, tok_stride,
-        out_n, out_score, state_i, state_f, 0, LmSearch{}, fresh);
-    return check_launch("prefix_beam_kernel<pool>");
-}
-
-// ---- with the LM (BeamSearchDecoder with its Scorer: beam_search_decoder.py:29-32,47-56) ----
-template <bool POOL = false>
-static int launch_beam_lm(const char* what, const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
-                          int64_t bstride, const int* lens, int B, int beam_size, int blank, const masr_lm_tables* lm, float alpha,
-                          float beta, float* pool, int* trie_parent, int* trie_tok, int64_t trie_cap, int* state_i, float* state_f,
-                          int resume, int* out_tok, int64_t tok_stride, int* out_n, float* out_score, float* out_approx,
-                          cudaStream_t stream, int* fresh = nullptr) {
-    MASR_REQUIRE(cand_id && cand_logp && cand_cnt && blank_logp && lens && pool && trie_parent && trie_tok && out_tok && out_n &&
-                 out_score && out_approx && lm, "%s: null pointer", what);
-    MASR_REQUIRE(lm->keys && lm->vals && lm->tok2lm, "%s: LM tables not set", what);
-    MASR_REQUIRE(lm->order >= 1 && lm->order <= LM_MAX_ORDER, "%s: LM order %d out of range (1..%d)", what, lm->order, LM_MAX_ORDER);
-    MASR_REQUIRE(beam_size >= 1 && beam_size <= BEAM_CAP, "%s: beam_size=%d out of range (1..%d)", what, beam_size, BEAM_CAP);
-    if constexpr (POOL) {
-        MASR_REQUIRE(state_i && state_f && fresh, "%s: null pointer", what);
-        const int rc = pool_smem_attr<BEAM_CHAR_LM>();
-        if (rc) return rc;
-    } else {
-        cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<BEAM_CHAR_LM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BeamSharedLm));
-        if (e != cudaSuccess) { set_last_error("prefix_beam<lm> smem attr: %s", cudaGetErrorString(e)); return (int)e; }
-    }
-    const LmSearch lms{*lm, blank_logp, alpha, beta, out_approx};
-    prefix_beam_kernel<BEAM_CHAR_LM, POOL><<<B, BEAM_THREADS, sizeof(BeamSharedLm), stream>>>(
-        cand_id, cand_logp, cand_cnt, bstride, lens, beam_size, blank, pool, trie_parent, trie_tok, trie_cap, out_tok, tok_stride,
-        out_n, out_score, state_i, state_f, resume, lms, fresh);
-    return check_launch(what);
-}
-
-extern "C" int masr_ctc_prefix_beam_lm(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
-                                       int64_t bstride, const int* lens, int B, int beam_size, int blank, const masr_lm_tables* lm_host,
-                                       float alpha, float beta, float* pool, int* trie_parent, int* trie_tok, int64_t trie_cap,
-                                       int* out_tok, int64_t tok_stride, int* out_n, float* out_score, float* out_approx,
-                                       void* stream) {
-    if (B == 0) return MASR_OK;
-    return launch_beam_lm("masr_ctc_prefix_beam_lm", cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size, blank,
-                          lm_host, alpha, beta, pool, trie_parent, trie_tok, trie_cap, nullptr, nullptr, 0, out_tok, tok_stride,
-                          out_n, out_score, out_approx, (cudaStream_t)stream);
 }
 
 extern "C" int masr_ctc_prefix_beam_lm_state_size(int64_t* ints_per_utt, int64_t* floats_per_utt) {
@@ -892,16 +773,144 @@ extern "C" int masr_ctc_prefix_beam_lm_state_size(int64_t* ints_per_utt, int64_t
     return MASR_OK;
 }
 
+extern "C" int masr_ctc_prefix_beam_wordlm_state_size(int64_t* ints_per_utt, int64_t* floats_per_utt) {
+    MASR_REQUIRE(ints_per_utt && floats_per_utt, "masr_ctc_prefix_beam_wordlm_state_size: null pointer");
+    *ints_per_utt = WLM_STATE_INTS;
+    *floats_per_utt = 3 * BEAM_CAP;
+    return MASR_OK;
+}
+
+// ---- the nine launching entry points: {no LM, character LM (BeamSearchDecoder with its Scorer,
+// beam_search_decoder.py:29-32,47-56), word LM with its lexicon (oracle/word_lm.py)} x {one-shot, streaming, pool} ----
+//
+// Streaming form (beam_search_decoder.py:75-96: CTCBeamSearchDecoder.next() + decode(), reset_state()): the same search
+// fed chunk by chunk.  `lens[b]` = frames of THIS chunk (0 = no new frames for that stream), `resume` = 0 starts a new
+// utterance (reset_decoder), != 0 continues from `state_*`; trie_parent / trie_tok must be sized for the whole stream
+// (masr_ctc_prefix_beam_workspace with Tmax = the longest stream in frames) and persist between calls.  Outputs = the best
+// prefix and its score after the frames seen so far — identical to one one-shot call over the concatenation.
+//
+// Pool form (a stream pool's slots, each starting and ending utterances on its own): as the streaming form with
+// `fresh[b]` (device) in place of `resume`.  fresh[b] != 0 starts slot b at the root and is cleared by the kernel; the caller
+// marks a slot fresh AND resets its hash range [b*trie_cap + trie_cap/5, (b+1)*trie_cap) of trie_parent to -1 (0xFF bytes)
+// before its next launch.  Slots with lens[b] == 0 are left untouched (state, trie and outputs).  Every argument that varies
+// between launches is device data, so the launch can be captured once into a CUDA graph and replayed.
+
+// The arguments every form shares; blank_logp / out_approx (LM forms), state_i / state_f (streaming and pool forms) and
+// fresh (pool forms) are null where a form has none.
+struct BeamArgs {
+    const int* cand_id; const float* cand_logp; const int* cand_cnt; const float* blank_logp; int64_t bstride;
+    const int* lens; int B, beam_size, blank; float* pool; int* trie_parent; int* trie_tok; int64_t trie_cap;
+    int* state_i; float* state_f; int resume; int* fresh;
+    int* out_tok; int64_t tok_stride; int* out_n; float* out_score; float* out_approx;
+};
+
+static int check_tables(const char* what, const masr_lm_tables* lm, int) {
+    MASR_REQUIRE(lm->keys && lm->vals && lm->tok2lm, "%s: LM tables not set", what);
+    MASR_REQUIRE(lm->order >= 1 && lm->order <= LM_MAX_ORDER, "%s: LM order %d out of range (1..%d)", what, lm->order, LM_MAX_ORDER);
+    return MASR_OK;
+}
+
+static int check_tables(const char* what, const masr_word_lm_tables* lm, int blank) {
+    MASR_REQUIRE(lm->keys && lm->vals && lm->lex_off && lm->lex_word && lm->nodes >= 1 && (lm->lex_tok || lm->nodes == 1) &&
+                 (lm->lex_next || lm->nodes == 1), "%s: word LM tables not set", what);
+    MASR_REQUIRE(lm->order >= 1 && lm->order <= WLM_MAX_ORDER, "%s: word LM order %d out of range (1..%d)", what, lm->order,
+                 WLM_MAX_ORDER);
+    MASR_REQUIRE(lm->space >= 0 && lm->space != blank, "%s: <space> token %d invalid", what, lm->space);
+    return MASR_OK;
+}
+
+// The dynamic shared memory attribute of one instantiation, set once per device (never while a graph is being captured:
+// the pool forms are launched eagerly once before their capture).
+template <int MODE, bool POOL>
+static int smem_attr() {
+    static bool done[64] = {};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev < 0 || dev >= 64) dev = 0;
+    if (!done[dev]) {
+        cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<MODE, POOL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)sizeof(typename BeamSmem<MODE>::type));
+        if (e != cudaSuccess) { set_last_error("prefix_beam smem attr: %s", cudaGetErrorString(e)); return (int)e; }
+        done[dev] = true;
+    }
+    return MASR_OK;
+}
+
+// `stateful`: the streaming and pool forms, which need state_i / state_f.  `lm`: null without an LM.
+template <int MODE, bool POOL>
+static int launch_beam(const char* what, bool stateful, const BeamArgs& a,
+                       const std::conditional_t<MODE == BEAM_WORD_LM, masr_word_lm_tables, masr_lm_tables>* lm, float alpha,
+                       float beta, void* stream) {
+    constexpr bool LM = MODE != BEAM_PLAIN;
+    if (a.B == 0) return MASR_OK;
+    MASR_REQUIRE(a.cand_id && a.cand_logp && a.cand_cnt && a.lens && a.pool && a.trie_parent && a.trie_tok && a.out_tok &&
+                 a.out_n && a.out_score && (!LM || (a.blank_logp && a.out_approx && lm)) &&
+                 (!stateful || (a.state_i && a.state_f)) && (!POOL || a.fresh), "%s: null pointer", what);
+    LmSearch lms{};
+    if constexpr (LM) {
+        const int rc = check_tables(what, lm, a.blank);
+        if (rc) return rc;
+        if constexpr (MODE == BEAM_CHAR_LM) lms.lm = *lm;
+        else lms.wlm = *lm;
+    }
+    MASR_REQUIRE(a.beam_size >= 1 && a.beam_size <= BEAM_CAP, "%s: beam_size=%d out of range (1..%d)", what, a.beam_size, BEAM_CAP);
+    const int rc = smem_attr<MODE, POOL>();
+    if (rc) return rc;
+    lms.blank_lp = a.blank_logp;
+    lms.alpha = alpha;
+    lms.beta = beta;
+    lms.out_approx = a.out_approx;
+    prefix_beam_kernel<MODE, POOL><<<a.B, BEAM_THREADS, sizeof(typename BeamSmem<MODE>::type), (cudaStream_t)stream>>>(
+        a.cand_id, a.cand_logp, a.cand_cnt, a.bstride, a.lens, a.beam_size, a.blank, a.pool, a.trie_parent, a.trie_tok,
+        a.trie_cap, a.out_tok, a.tok_stride, a.out_n, a.out_score, a.state_i, a.state_f, a.resume, lms, a.fresh);
+    return check_launch(what);
+}
+
+extern "C" int masr_ctc_prefix_beam(const int* cand_id, const float* cand_logp, const int* cand_cnt, int64_t bstride,
+                                    const int* lens, int B, int beam_size, int blank, float* pool, int* trie_parent,
+                                    int* trie_tok, int64_t trie_cap, int* out_tok, int64_t tok_stride, int* out_n,
+                                    float* out_score, void* stream) {
+    return launch_beam<BEAM_PLAIN, false>("masr_ctc_prefix_beam", false,
+        {cand_id, cand_logp, cand_cnt, nullptr, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
+         nullptr, nullptr, 0, nullptr, out_tok, tok_stride, out_n, out_score, nullptr}, nullptr, 0.f, 0.f, stream);
+}
+
+extern "C" int masr_ctc_prefix_beam_stream(const int* cand_id, const float* cand_logp, const int* cand_cnt, int64_t bstride,
+                                           const int* lens, int B, int beam_size, int blank, float* pool, int* trie_parent,
+                                           int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int resume,
+                                           int* out_tok, int64_t tok_stride, int* out_n, float* out_score, void* stream) {
+    return launch_beam<BEAM_PLAIN, false>("masr_ctc_prefix_beam_stream", true,
+        {cand_id, cand_logp, cand_cnt, nullptr, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
+         state_i, state_f, resume, nullptr, out_tok, tok_stride, out_n, out_score, nullptr}, nullptr, 0.f, 0.f, stream);
+}
+
+extern "C" int masr_ctc_prefix_beam_pool(const int* cand_id, const float* cand_logp, const int* cand_cnt, int64_t bstride,
+                                         const int* lens, int B, int beam_size, int blank, float* pool, int* trie_parent,
+                                         int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int* fresh,
+                                         int* out_tok, int64_t tok_stride, int* out_n, float* out_score, void* stream) {
+    return launch_beam<BEAM_PLAIN, true>("masr_ctc_prefix_beam_pool", true,
+        {cand_id, cand_logp, cand_cnt, nullptr, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
+         state_i, state_f, 0, fresh, out_tok, tok_stride, out_n, out_score, nullptr}, nullptr, 0.f, 0.f, stream);
+}
+
+extern "C" int masr_ctc_prefix_beam_lm(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
+                                       int64_t bstride, const int* lens, int B, int beam_size, int blank, const masr_lm_tables* lm_host,
+                                       float alpha, float beta, float* pool, int* trie_parent, int* trie_tok, int64_t trie_cap,
+                                       int* out_tok, int64_t tok_stride, int* out_n, float* out_score, float* out_approx,
+                                       void* stream) {
+    return launch_beam<BEAM_CHAR_LM, false>("masr_ctc_prefix_beam_lm", false,
+        {cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
+         nullptr, nullptr, 0, nullptr, out_tok, tok_stride, out_n, out_score, out_approx}, lm_host, alpha, beta, stream);
+}
+
 extern "C" int masr_ctc_prefix_beam_lm_stream(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
                                               int64_t bstride, const int* lens, int B, int beam_size, int blank,
                                               const masr_lm_tables* lm_host, float alpha, float beta, float* pool, int* trie_parent,
                                               int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int resume, int* out_tok,
                                               int64_t tok_stride, int* out_n, float* out_score, float* out_approx, void* stream) {
-    if (B == 0) return MASR_OK;
-    MASR_REQUIRE(state_i && state_f, "masr_ctc_prefix_beam_lm_stream: null pointer");
-    return launch_beam_lm("masr_ctc_prefix_beam_lm_stream", cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size,
-                          blank, lm_host, alpha, beta, pool, trie_parent, trie_tok, trie_cap, state_i, state_f, resume, out_tok,
-                          tok_stride, out_n, out_score, out_approx, (cudaStream_t)stream);
+    return launch_beam<BEAM_CHAR_LM, false>("masr_ctc_prefix_beam_lm_stream", true,
+        {cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
+         state_i, state_f, resume, nullptr, out_tok, tok_stride, out_n, out_score, out_approx}, lm_host, alpha, beta, stream);
 }
 
 extern "C" int masr_ctc_prefix_beam_lm_pool(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
@@ -909,47 +918,9 @@ extern "C" int masr_ctc_prefix_beam_lm_pool(const int* cand_id, const float* can
                                             const masr_lm_tables* lm_host, float alpha, float beta, float* pool, int* trie_parent,
                                             int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int* fresh, int* out_tok,
                                             int64_t tok_stride, int* out_n, float* out_score, float* out_approx, void* stream) {
-    if (B == 0) return MASR_OK;
-    return launch_beam_lm<true>("masr_ctc_prefix_beam_lm_pool", cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size,
-                                blank, lm_host, alpha, beta, pool, trie_parent, trie_tok, trie_cap, state_i, state_f, 0, out_tok,
-                                tok_stride, out_n, out_score, out_approx, (cudaStream_t)stream, fresh);
-}
-
-// ---- with a word LM and its lexicon (oracle/word_lm.py) ----
-template <bool POOL = false>
-static int launch_beam_wordlm(const char* what, const int* cand_id, const float* cand_logp, const int* cand_cnt,
-                              const float* blank_logp, int64_t bstride, const int* lens, int B, int beam_size, int blank,
-                              const masr_word_lm_tables* lm, float alpha, float beta, float* pool, int* trie_parent,
-                              int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int resume, int* out_tok,
-                              int64_t tok_stride, int* out_n, float* out_score, float* out_approx, cudaStream_t stream,
-                              int* fresh = nullptr) {
-    MASR_REQUIRE(cand_id && cand_logp && cand_cnt && blank_logp && lens && pool && trie_parent && trie_tok && out_tok && out_n &&
-                 out_score && out_approx && lm, "%s: null pointer", what);
-    MASR_REQUIRE(lm->keys && lm->vals && lm->lex_off && lm->lex_word && lm->nodes >= 1 && (lm->lex_tok || lm->nodes == 1) &&
-                 (lm->lex_next || lm->nodes == 1), "%s: word LM tables not set", what);
-    MASR_REQUIRE(lm->order >= 1 && lm->order <= WLM_MAX_ORDER, "%s: word LM order %d out of range (1..%d)", what, lm->order,
-                 WLM_MAX_ORDER);
-    MASR_REQUIRE(lm->space >= 0 && lm->space != blank, "%s: <space> token %d invalid", what, lm->space);
-    MASR_REQUIRE(beam_size >= 1 && beam_size <= BEAM_CAP, "%s: beam_size=%d out of range (1..%d)", what, beam_size, BEAM_CAP);
-    if constexpr (POOL) {
-        MASR_REQUIRE(state_i && state_f && fresh, "%s: null pointer", what);
-        const int rc = pool_smem_attr<BEAM_WORD_LM>();
-        if (rc) return rc;
-    } else {
-        cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<BEAM_WORD_LM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)sizeof(BeamSharedWord));
-        if (e != cudaSuccess) { set_last_error("prefix_beam<wordlm> smem attr: %s", cudaGetErrorString(e)); return (int)e; }
-    }
-    LmSearch lms{};
-    lms.blank_lp = blank_logp;
-    lms.alpha = alpha;
-    lms.beta = beta;
-    lms.out_approx = out_approx;
-    lms.wlm = *lm;
-    prefix_beam_kernel<BEAM_WORD_LM, POOL><<<B, BEAM_THREADS, sizeof(BeamSharedWord), stream>>>(
-        cand_id, cand_logp, cand_cnt, bstride, lens, beam_size, blank, pool, trie_parent, trie_tok, trie_cap, out_tok, tok_stride,
-        out_n, out_score, state_i, state_f, resume, lms, fresh);
-    return check_launch(what);
+    return launch_beam<BEAM_CHAR_LM, true>("masr_ctc_prefix_beam_lm_pool", true,
+        {cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
+         state_i, state_f, 0, fresh, out_tok, tok_stride, out_n, out_score, out_approx}, lm_host, alpha, beta, stream);
 }
 
 extern "C" int masr_ctc_prefix_beam_wordlm(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
@@ -957,17 +928,9 @@ extern "C" int masr_ctc_prefix_beam_wordlm(const int* cand_id, const float* cand
                                            const masr_word_lm_tables* lm_host, float alpha, float beta, float* pool,
                                            int* trie_parent, int* trie_tok, int64_t trie_cap, int* out_tok, int64_t tok_stride,
                                            int* out_n, float* out_score, float* out_approx, void* stream) {
-    if (B == 0) return MASR_OK;
-    return launch_beam_wordlm("masr_ctc_prefix_beam_wordlm", cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size,
-                              blank, lm_host, alpha, beta, pool, trie_parent, trie_tok, trie_cap, nullptr, nullptr, 0, out_tok,
-                              tok_stride, out_n, out_score, out_approx, (cudaStream_t)stream);
-}
-
-extern "C" int masr_ctc_prefix_beam_wordlm_state_size(int64_t* ints_per_utt, int64_t* floats_per_utt) {
-    MASR_REQUIRE(ints_per_utt && floats_per_utt, "masr_ctc_prefix_beam_wordlm_state_size: null pointer");
-    *ints_per_utt = WLM_STATE_INTS;
-    *floats_per_utt = 3 * BEAM_CAP;
-    return MASR_OK;
+    return launch_beam<BEAM_WORD_LM, false>("masr_ctc_prefix_beam_wordlm", false,
+        {cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
+         nullptr, nullptr, 0, nullptr, out_tok, tok_stride, out_n, out_score, out_approx}, lm_host, alpha, beta, stream);
 }
 
 extern "C" int masr_ctc_prefix_beam_wordlm_stream(const int* cand_id, const float* cand_logp, const int* cand_cnt,
@@ -976,11 +939,9 @@ extern "C" int masr_ctc_prefix_beam_wordlm_stream(const int* cand_id, const floa
                                                   float* pool, int* trie_parent, int* trie_tok, int64_t trie_cap, int* state_i,
                                                   float* state_f, int resume, int* out_tok, int64_t tok_stride, int* out_n,
                                                   float* out_score, float* out_approx, void* stream) {
-    if (B == 0) return MASR_OK;
-    MASR_REQUIRE(state_i && state_f, "masr_ctc_prefix_beam_wordlm_stream: null pointer");
-    return launch_beam_wordlm("masr_ctc_prefix_beam_wordlm_stream", cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B,
-                              beam_size, blank, lm_host, alpha, beta, pool, trie_parent, trie_tok, trie_cap, state_i, state_f,
-                              resume, out_tok, tok_stride, out_n, out_score, out_approx, (cudaStream_t)stream);
+    return launch_beam<BEAM_WORD_LM, false>("masr_ctc_prefix_beam_wordlm_stream", true,
+        {cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
+         state_i, state_f, resume, nullptr, out_tok, tok_stride, out_n, out_score, out_approx}, lm_host, alpha, beta, stream);
 }
 
 extern "C" int masr_ctc_prefix_beam_wordlm_pool(const int* cand_id, const float* cand_logp, const int* cand_cnt,
@@ -989,8 +950,7 @@ extern "C" int masr_ctc_prefix_beam_wordlm_pool(const int* cand_id, const float*
                                                 int* trie_parent, int* trie_tok, int64_t trie_cap, int* state_i, float* state_f,
                                                 int* fresh, int* out_tok, int64_t tok_stride, int* out_n, float* out_score,
                                                 float* out_approx, void* stream) {
-    if (B == 0) return MASR_OK;
-    return launch_beam_wordlm<true>("masr_ctc_prefix_beam_wordlm_pool", cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B,
-                                    beam_size, blank, lm_host, alpha, beta, pool, trie_parent, trie_tok, trie_cap, state_i,
-                                    state_f, 0, out_tok, tok_stride, out_n, out_score, out_approx, (cudaStream_t)stream, fresh);
+    return launch_beam<BEAM_WORD_LM, true>("masr_ctc_prefix_beam_wordlm_pool", true,
+        {cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
+         state_i, state_f, 0, fresh, out_tok, tok_stride, out_n, out_score, out_approx}, lm_host, alpha, beta, stream);
 }

@@ -21,6 +21,7 @@ import torch
 from . import _lib
 from . import resample as resampling
 from ._lib import EPI_BIAS, EPI_BIAS_GLU, EPI_BIAS_SCALE, EPI_BIAS_SILU, EPI_RESIDUAL, call
+from .beam import ONE_SHOT, STREAM, BeamSearch
 from .weights import ConformerWeights, load_state_dict, pack_conformer
 
 FRAME_LEN, FRAME_SHIFT, NUM_MEL = 400, 160, 80
@@ -653,7 +654,7 @@ class ConformerEngine:
                 _p(ws["tokens"]), ws["tokens"].shape[1], _p(ws["ntok"]), _p(ws["psum"]), _p(ws["pcount"]))
         return probs
 
-    # ---- CTC prefix beam search (optionally with a character LM) -------------------------------------
+    # ---- CTC prefix beam search (optionally with a character or word LM) ---------------------------------
     def ctc_beam(self, enc: torch.Tensor, out_lens: Sequence[int], T: int, ws, beam_size: int = 300,
                  cutoff_prob: float = 0.99, cutoff_top_n: int = 40, lm=None, alpha: float = 0.0, beta: float = 0.0):
         """`ctc_beam_search_decoding(probs, vocab, beam_size, cutoff_prob, cutoff_top_n, scorer, blank_id=0)` of the
@@ -661,53 +662,29 @@ class ConformerEngine:
         (tokens [B,T], count [B], log-score [B]).  ``lm`` (a masr_b200.lm.CharLM or WordLM, or None): shallow fusion with
         weight ``alpha`` and insertion bonus ``beta`` (a WordLM scores per word and constrains the words to its lexicon); the
         log-score is then the reference's approx_ctc (the fused score with the LM terms taken out again; the fused score is
-        in ws["beam_score"]).  Parity unpinned (DESIGN.md)."""
-        B = len(out_lens)
-        M = B * T
-        dev = self.device
+        in ws["beam_score"], and ln p_blank per row in ws["blank_lp"]).  Parity unpinned (DESIGN.md)."""
+        B, Tb = len(out_lens), max(1, T)
+        settings = (beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta)
         logits = self.ctc_logits(enc, ws)
-        if "cand_id" not in ws or ws["cand_id"].shape[0] < M:
-            ws["cand_id"] = torch.empty(M, 40, device=dev, dtype=torch.int32)
-            ws["cand_lp"] = torch.empty(M, 40, device=dev, dtype=torch.float32)
-            ws["cand_n"] = torch.empty(M, device=dev, dtype=torch.int32)
-            pool_n, trie_n = _lib.C.c_int64(0), _lib.C.c_int64(0)
-            call("masr_ctc_prefix_beam_workspace", B, T, _lib.C.byref(pool_n), _lib.C.byref(trie_n))
-            ws["beam_pool"] = torch.empty(pool_n.value, device=dev, dtype=torch.float32)
-            ws["trie_par"] = torch.empty(B * trie_n.value, device=dev, dtype=torch.int32)
-            ws["trie_tok"] = torch.empty(B * trie_n.value, device=dev, dtype=torch.int32)
-            ws["trie_cap"] = trie_n.value
-            ws["beam_tok"] = torch.zeros(B, max(1, T), device=dev, dtype=torch.int32)
-            ws["beam_n"] = torch.zeros(B, device=dev, dtype=torch.int32)
-            ws["beam_score"] = torch.zeros(B, device=dev, dtype=torch.float32)
-        if lm is not None:
-            if ws.get("blank_lp") is None or ws["blank_lp"].numel() < M:
-                ws["blank_lp"] = torch.empty(M, device=dev, dtype=torch.float32)
-            if ws.get("beam_approx") is None or ws["beam_approx"].numel() < ws["beam_score"].numel():
-                ws["beam_approx"] = torch.zeros_like(ws["beam_score"])
-            self._k("ctc_topk", "masr_ctc_topk_blank_f32", _p(logits), self.Vpad, M, self.V, int(cutoff_top_n), float(cutoff_prob),
-                    0, _p(ws["cand_id"]), _p(ws["cand_lp"]), _p(ws["cand_n"]), _p(ws["blank_lp"]))
-            self._k("prefix_beam", lm.BEAM, _p(ws["cand_id"]), _p(ws["cand_lp"]), _p(ws["cand_n"]),
-                    _p(ws["blank_lp"]), T, _p(ws["tlens"]), B, int(beam_size), 0, _lib.C.byref(lm.tables(dev)), float(alpha),
-                    float(beta), _p(ws["beam_pool"]), _p(ws["trie_par"]), _p(ws["trie_tok"]), ws["trie_cap"], _p(ws["beam_tok"]),
-                    ws["beam_tok"].shape[1], _p(ws["beam_n"]), _p(ws["beam_score"]), _p(ws["beam_approx"]))
-            self._last_beam = (ws, T, B)
-            return ws["beam_tok"], ws["beam_n"], ws["beam_approx"]
-        self._k("ctc_topk", "masr_ctc_topk_f32", _p(logits), self.Vpad, M, self.V, int(cutoff_top_n), float(cutoff_prob),
-                _p(ws["cand_id"]), _p(ws["cand_lp"]), _p(ws["cand_n"]))
-        self._k("prefix_beam", "masr_ctc_prefix_beam", _p(ws["cand_id"]), _p(ws["cand_lp"]), _p(ws["cand_n"]), T, _p(ws["tlens"]),
-                B, int(beam_size), 0, _p(ws["beam_pool"]), _p(ws["trie_par"]), _p(ws["trie_tok"]), ws["trie_cap"],
-                _p(ws["beam_tok"]), ws["beam_tok"].shape[1], _p(ws["beam_n"]), _p(ws["beam_score"]))
+        if "beam" not in ws or not ws["beam"].fits(B, Tb, *settings):
+            ws.pop("beam", None)                      # (the old buffers go back to the allocator before the new ones are taken)
+            ws["beam"] = BeamSearch(self.device, ONE_SHOT, B, B * Tb, Tb, *settings)
+        bs = ws["beam"]
+        ws["beam_score"], ws["blank_lp"] = bs.fused, bs.blank_lp
+        bs.topk(self, logits, self.Vpad, B * T)
+        bs.search(self, _p(ws["tlens"]), B, T)
         self._last_beam = (ws, T, B)
-        return ws["beam_tok"], ws["beam_n"], ws["beam_score"]
+        return bs.out_tok, bs.count, bs.score
 
     def last_beam_candidates(self):
         """The pruned per-frame candidate lists [(token id, float32 log-probability)] the last ``ctc_beam`` call searched
         over, per utterance and frame — what the top-k kernel handed to the prefix beam kernel (for parity tests: the CPU
         restatement run on the same candidates must return the same prefix and score bit for bit)."""
         ws, T, B = self._last_beam
-        n = ws["cand_n"][:B * T].cpu().numpy().reshape(B, T)
-        ids = ws["cand_id"][:B * T].cpu().numpy().reshape(B, T, -1)
-        lp = ws["cand_lp"][:B * T].cpu().numpy().reshape(B, T, -1)
+        bs = ws["beam"]
+        n = bs.cand_n[:B * T].cpu().numpy().reshape(B, T)
+        ids = bs.cand_id[:B * T].cpu().numpy().reshape(B, T, -1)
+        lp = bs.cand_lp[:B * T].cpu().numpy().reshape(B, T, -1)
         return [[[(int(ids[b, t, k]), np.float32(lp[b, t, k])) for k in range(int(n[b, t]))] for t in range(T)] for b in range(B)]
 
     def transcribe_beam(self, waves: Sequence[np.ndarray], beam_size: int = 300, cutoff_prob: float = 0.99,
@@ -727,8 +704,7 @@ class ConformerEngine:
         (two sets of candidate / trie / output buffers; the LM tables are shared read-only).  Same results as the blocking
         call."""
         dev = self.device
-        lm_t = _lib.C.byref(lm.tables(dev)) if lm is not None else None
-        lm_beam = lm.BEAM if lm is not None else None
+        settings = (beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta)
         main = torch.cuda.current_stream(dev)
         if getattr(self, "_beam_stream", None) is None:
             self._beam_stream = torch.cuda.Stream(device=dev)
@@ -760,53 +736,31 @@ class ConformerEngine:
                     main.wait_event(slot["done"])          # the slot's previous search (batch k-2) has consumed its buffers
                 feats, frames, status = self.fbank(waves, use_db_normalization, target_db, rates=rates)
                 enc, tl, T, ws = self.encode(feats, frames)
-                M = B * max(1, T)
-                if slot.get("M", 0) < M or slot.get("B", 0) < B or slot.get("T", 0) < T:
-                    pool_n, trie_n = _lib.C.c_int64(0), _lib.C.c_int64(0)
-                    call("masr_ctc_prefix_beam_workspace", B, max(1, T), _lib.C.byref(pool_n), _lib.C.byref(trie_n))
+                Tb = max(1, T)
+                if "beam" not in slot or not slot["beam"].fits(B, Tb, *settings):
+                    slot.clear()
                     i32, f32 = torch.int32, torch.float32
-                    slot.update(M=M, B=B, T=T, trie_cap=trie_n.value,
-                                cand_id=torch.empty(M, 40, device=dev, dtype=i32), cand_lp=torch.empty(M, 40, device=dev, dtype=f32),
-                                cand_n=torch.empty(M, device=dev, dtype=i32), pool=torch.empty(pool_n.value, device=dev, dtype=f32),
-                                trie_par=torch.empty(B * trie_n.value, device=dev, dtype=i32),
-                                trie_tok=torch.empty(B * trie_n.value, device=dev, dtype=i32),
-                                tok=torch.zeros(B, max(1, T), device=dev, dtype=i32), n=torch.zeros(B, device=dev, dtype=i32),
-                                sc=torch.zeros(B, device=dev, dtype=f32), tlens=torch.zeros(B, device=dev, dtype=i32),
-                                h_tok=torch.zeros(B, max(1, T), dtype=i32, pin_memory=True), h_n=torch.zeros(B, dtype=i32, pin_memory=True),
-                                h_sc=torch.zeros(B, dtype=f32, pin_memory=True), ready=torch.cuda.Event(), done=torch.cuda.Event(),
-                                blank_lp=torch.empty(M, device=dev, dtype=f32), fused=torch.zeros(B, device=dev, dtype=f32))
+                    slot.update(beam=BeamSearch(self.device, ONE_SHOT, B, B * Tb, Tb, *settings),
+                                tlens=torch.zeros(B, device=dev, dtype=i32), h_tok=torch.zeros(B, Tb, dtype=i32, pin_memory=True),
+                                h_n=torch.zeros(B, dtype=i32, pin_memory=True), h_sc=torch.zeros(B, dtype=f32, pin_memory=True),
+                                ready=torch.cuda.Event(), done=torch.cuda.Event())
+                bs = slot["beam"]
                 if T == 0:
                     slot["h_n"][:B].zero_()
                     slot["h_sc"][:B].zero_()
                     slot["done"].record(main)
-                    item = (slot, B)
                 else:
-                    logits = self.ctc_logits(enc, ws)
-                    if lm_t is None:
-                        self._k("ctc_topk", "masr_ctc_topk_f32", _p(logits), self.Vpad, B * T, self.V, int(cutoff_top_n),
-                                float(cutoff_prob), _p(slot["cand_id"]), _p(slot["cand_lp"]), _p(slot["cand_n"]))
-                    else:
-                        self._k("ctc_topk", "masr_ctc_topk_blank_f32", _p(logits), self.Vpad, B * T, self.V, int(cutoff_top_n),
-                                float(cutoff_prob), 0, _p(slot["cand_id"]), _p(slot["cand_lp"]), _p(slot["cand_n"]), _p(slot["blank_lp"]))
+                    bs.topk(self, self.ctc_logits(enc, ws), self.Vpad, B * T)
                     slot["tlens"][:B].copy_(ws["tlens"][:B])
                     slot["ready"].record(main)
                     side.wait_event(slot["ready"])
                     with torch.cuda.stream(side):
-                        if lm_t is None:
-                            self._k("prefix_beam", "masr_ctc_prefix_beam", _p(slot["cand_id"]), _p(slot["cand_lp"]), _p(slot["cand_n"]), T,
-                                    _p(slot["tlens"]), B, int(beam_size), 0, _p(slot["pool"]), _p(slot["trie_par"]), _p(slot["trie_tok"]),
-                                    slot["trie_cap"], _p(slot["tok"]), slot["tok"].shape[1], _p(slot["n"]), _p(slot["sc"]))
-                        else:                      # the reported score is approx_ctc (see ctc_beam)
-                            self._k("prefix_beam", lm_beam, _p(slot["cand_id"]), _p(slot["cand_lp"]),
-                                    _p(slot["cand_n"]), _p(slot["blank_lp"]), T, _p(slot["tlens"]), B, int(beam_size), 0, lm_t,
-                                    float(alpha), float(beta), _p(slot["pool"]), _p(slot["trie_par"]), _p(slot["trie_tok"]),
-                                    slot["trie_cap"], _p(slot["tok"]), slot["tok"].shape[1], _p(slot["n"]), _p(slot["fused"]),
-                                    _p(slot["sc"]))
-                        slot["h_tok"][:B, :slot["tok"].shape[1]].copy_(slot["tok"][:B], non_blocking=True)
-                        slot["h_n"][:B].copy_(slot["n"][:B], non_blocking=True)
-                        slot["h_sc"][:B].copy_(slot["sc"][:B], non_blocking=True)
+                        bs.search(self, _p(slot["tlens"]), B, T)
+                        slot["h_tok"][:B].copy_(bs.out_tok[:B], non_blocking=True)
+                        slot["h_n"][:B].copy_(bs.count[:B], non_blocking=True)
+                        slot["h_sc"][:B].copy_(bs.score[:B], non_blocking=True)
                         slot["done"].record(side)
-                    item = (slot, B)
+                item = (slot, B)
             if prev is not None:
                 yield finish(prev)
             prev = item
@@ -1290,10 +1244,10 @@ class ConformerStream:
         self.cache_start = 0
 
 
-class StreamBeam:
+class StreamBeam(BeamSearch):
     """Streaming CTC prefix beam search of ONE stream on the GPU — ``BeamSearchDecoder.decode_chunk / reset_decoder``
     (masr/decoders/beam_search_decoder.py:75-96, called at masr/predict.py:322,353): the beam, the prefix trie and its hash
-    stay on the device between chunks (masr_ctc_prefix_beam_stream), so after every chunk the best prefix equals the
+    stay on the device between chunks (the search's streaming form), so after every chunk the best prefix equals the
     whole-utterance search over all frames seen so far.  ``lm`` / ``alpha`` / ``beta``: shallow fusion of a character or
     word LM as in ConformerEngine.ctc_beam (each beam entry's LM window, and with a word LM its lexicon state, is part of
     the device state); the score is then approx_ctc.
@@ -1301,30 +1255,10 @@ class StreamBeam:
 
     def __init__(self, eng: "ConformerEngine", beam_size: int = 300, cutoff_prob: float = 0.99, cutoff_top_n: int = 40,
                  max_frames: int = 3000, max_chunk: int = 64, lm=None, alpha: float = 0.0, beta: float = 0.0):
-        self.eng, self.beam, self.cutoff, self.top_n = eng, int(beam_size), float(cutoff_prob), int(cutoff_top_n)
-        self.max_frames, self.max_chunk = int(max_frames), int(max_chunk)
-        self.lm, self.alpha, self.beta = lm, float(alpha), float(beta)
-        dev, C = eng.device, _lib.C
-        pool_n, trie_n, si, sf = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_int64(0)
-        call("masr_ctc_prefix_beam_workspace", 1, self.max_frames, C.byref(pool_n), C.byref(trie_n))
-        call(lm.BEAM + "_state_size" if lm is not None else "masr_ctc_prefix_beam_state_size", C.byref(si), C.byref(sf))
-        i32, f32 = torch.int32, torch.float32
-        self.cand_id = torch.empty(self.max_chunk, 40, device=dev, dtype=i32)
-        self.cand_lp = torch.empty(self.max_chunk, 40, device=dev, dtype=f32)
-        self.cand_n = torch.empty(self.max_chunk, device=dev, dtype=i32)
-        self.pool = torch.empty(pool_n.value, device=dev, dtype=f32)
-        self.trie_par = torch.empty(trie_n.value, device=dev, dtype=i32)
-        self.trie_tok = torch.empty(trie_n.value, device=dev, dtype=i32)
-        self.trie_cap = trie_n.value
-        self.state_i = torch.zeros(si.value, device=dev, dtype=i32)
-        self.state_f = torch.zeros(sf.value, device=dev, dtype=f32)
-        self.lens = torch.zeros(1, device=dev, dtype=i32)
-        self.out_tok = torch.zeros(1, self.max_frames, device=dev, dtype=i32)
-        self.out = torch.zeros(2, device=dev, dtype=f32)             # [score, count (int32 bits)]
-        if lm is not None:
-            self.blank_lp = torch.empty(self.max_chunk, device=dev, dtype=f32)
-            self.fused = torch.zeros(1, device=dev, dtype=f32)
-            self.lm_t = C.byref(lm.tables(dev))
+        super().__init__(eng.device, STREAM, 1, max_chunk, max_frames, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta)
+        self.eng, self._own_lm = eng, lm                         # (the search itself holds the LM only weakly)
+        self.max_chunk = int(max_chunk)
+        self.lens = torch.zeros(1, device=eng.device, dtype=torch.int32)
         self.frames = 0
 
     def reset(self):
@@ -1333,34 +1267,19 @@ class StreamBeam:
 
     def push(self, logits: torch.Tensor, rows: int):
         """CTC-head logits [>= rows, ld] of the new chunk's frames -> (token ids of the best prefix so far, its log score)."""
-        eng = self.eng
         if rows > self.max_chunk:
             raise ValueError(f"a chunk has at most {self.max_chunk} frames")
         if self.frames + rows > self.max_frames:
             raise AssertionError(f"stream longer than {self.max_frames} frames: create the StreamBeam with a larger max_frames")
-        lm = self.lm is not None
-        if rows > 0 and lm:
-            eng._k("ctc_topk", "masr_ctc_topk_blank_f32", _p(logits), logits.stride(0), rows, eng.V, self.top_n, self.cutoff, 0,
-                   _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n), _p(self.blank_lp))
-        elif rows > 0:
-            eng._k("ctc_topk", "masr_ctc_topk_f32", _p(logits), logits.stride(0), rows, eng.V, self.top_n, self.cutoff,
-                   _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n))
+        if rows > 0:
+            self.topk(self.eng, logits, logits.stride(0), rows)
         self.lens.fill_(rows)
-        n_view = self.out[1:2].view(torch.int32)
-        if lm:
-            eng._k("prefix_beam", self.lm.BEAM + "_stream", _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n),
-                   _p(self.blank_lp), self.max_chunk, _p(self.lens), 1, self.beam, 0, self.lm_t, self.alpha, self.beta,
-                   _p(self.pool), _p(self.trie_par), _p(self.trie_tok), self.trie_cap, _p(self.state_i), _p(self.state_f),
-                   1 if self.frames else 0, _p(self.out_tok), self.out_tok.shape[1], _p(n_view), _p(self.fused), _p(self.out[0:1]))
-        else:
-            eng._k("prefix_beam", "masr_ctc_prefix_beam_stream", _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n), self.max_chunk,
-                   _p(self.lens), 1, self.beam, 0, _p(self.pool), _p(self.trie_par), _p(self.trie_tok), self.trie_cap, _p(self.state_i),
-                   _p(self.state_f), 1 if self.frames else 0, _p(self.out_tok), self.out_tok.shape[1], _p(n_view), _p(self.out[0:1]))
+        self.search(self.eng, _p(self.lens), 1, self.max_chunk, resume=1 if self.frames else 0)
         self.frames += rows
-        oh = self.out.cpu()
-        n = int(oh[1:2].view(torch.int32).item())
+        oh = self.out[:2].cpu()                                     # [score, count (int32 bits)]
+        n = int(oh[1].view(torch.int32).item())
         toks = self.out_tok[0, :n].cpu().tolist() if n else []
-        eng.d2h_bytes += 8 + 4 * n
+        self.eng.d2h_bytes += 8 + 4 * n
         return toks, float(oh[0].item())
 
 

@@ -19,9 +19,9 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 import torch
 
-from . import _lib
-from ._lib import EPI_BIAS, EPI_BIAS_GLU, EPI_BIAS_SCALE, EPI_BIAS_SILU, EPI_RESIDUAL, call
+from ._lib import EPI_BIAS, EPI_BIAS_GLU, EPI_BIAS_SCALE, EPI_BIAS_SILU, EPI_RESIDUAL
 from .audio import pcm_bytes_to_float32, samples_to_float32
+from .beam import POOL, BeamSearch
 from .engine import ConformerEngine, _p, greedy_score, subsampled_len
 from .predict import CACHED_FEATURE_NUM, DECODING_WINDOW, FRAME_SHIFT, chunk_starts
 from .resample import MODEL_RATE, output_length
@@ -617,12 +617,12 @@ def make_pool(eng, n_slots: int, max_frames: int = 3000):
     raise NotImplementedError(f"no stream pool for {type(eng).__name__}")
 
 
-class PoolBeam:
+class PoolBeam(BeamSearch):
     """Streaming CTC prefix beam search of EVERY slot of a chunk-decoding pool (``engine.StreamBeam`` for many streams; the
     reference's ``BeamSearchDecoder.decode_chunk / reset_decoder`` per stream, beam_search_decoder.py:75-96).
 
     Each pool step adds two launches, captured into the step's CUDA graph with the encoder: the top-k candidates of all
-    ``S * OUT_ROWS`` CTC-head rows (``pool.b["logits"]``), then ``masr_ctc_prefix_beam[_lm|_wordlm]_pool`` with one CTA per slot
+    ``S * OUT_ROWS`` CTC-head rows (``pool.b["logits"]``), then the pool form of the prefix beam search with one CTA per slot
     over that slot's valid rows (the length row of the pool's device ``meta``).  Slots without frames in a step are not
     touched.  Per slot the beam, its trie and the trie's hash stay on the device, so after every step a slot's best
     prefix equals the whole-utterance search over its frames since the last ``reset`` — what ``predict_stream`` returns.
@@ -635,35 +635,15 @@ class PoolBeam:
         beam_size = int(beam_size)
         if not 1 <= beam_size <= 512:
             raise ValueError(f"beam_size={beam_size} out of range (1..512)")
-        self.beam, self.cutoff, self.top_n = beam_size, float(cutoff_prob), int(cutoff_top_n)
-        self.lm, self.alpha, self.beta = lm, float(alpha), float(beta)
-        eng, S, R = pool.eng, pool.S, pool.OUT_ROWS
-        dev, C = eng.device, _lib.C
+        S, R = pool.S, pool.OUT_ROWS
+        # beam frames one slot can reach: the pool's cap at its output rate (+1: the EfficientConformer halves an odd final chunk up)
+        frames = pool.cap * R // CHUNK_OUT + 1
+        super().__init__(pool.eng.device, POOL, S, S * R, frames, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta)
         # what the launches read from the pool (the pool holds this object: no reference back to it, so dropping a pool frees
         # its CUDA graph at once instead of in a later garbage collection, which may fall inside another pool's capture)
-        self.eng, self.S, self.R, self.logits = eng, S, R, pool.b["logits"]
+        self.eng, self.R, self.logits = pool.eng, R, pool.b["logits"]
+        self._own_lm = lm                                        # (the search itself holds the LM only weakly)
         self.lens = pool._m(pool.QLEN if R == CHUNK_OUT else pool.QLEN2)          # valid rows per slot (device meta row)
-        # beam frames one slot can reach: the pool's cap at its output rate (+1: the EfficientConformer halves an odd final chunk up)
-        self.frames = pool.cap * R // CHUNK_OUT + 1
-        pool_n, trie_n, si, sf = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_int64(0)
-        call("masr_ctc_prefix_beam_workspace", S, 1, C.byref(pool_n), C.byref(trie_n))
-        call(lm.BEAM + "_state_size" if lm is not None else "masr_ctc_prefix_beam_state_size", C.byref(si), C.byref(sf))
-        self.trie_cap = 5 * (self.frames * beam_size + 1)          # nodes + 4 hash slots per node; the kernel reads node_cap = cap / 5
-        i32, f32 = torch.int32, torch.float32
-        self.cand_id = torch.zeros(S * R, 40, device=dev, dtype=i32)
-        self.cand_lp = torch.zeros(S * R, 40, device=dev, dtype=f32)
-        self.cand_n = torch.zeros(S * R, device=dev, dtype=i32)
-        self.scratch = torch.empty(pool_n.value, device=dev, dtype=f32)
-        self.trie_par = torch.full((S * self.trie_cap,), -1, device=dev, dtype=i32)     # every slot's hash starts empty
-        self.trie_tok = torch.empty(S * self.trie_cap, device=dev, dtype=i32)
-        self.state_i = torch.zeros(S, si.value, device=dev, dtype=i32)
-        self.state_f = torch.zeros(S, sf.value, device=dev, dtype=f32)
-        self.fresh = torch.ones(S, device=dev, dtype=i32)
-        self.out_tok = torch.zeros(S, self.frames, device=dev, dtype=i32)
-        self.out = torch.zeros(3, S, device=dev, dtype=f32)         # [reported score, token count (int32 bits), fused score]
-        if lm is not None:
-            self.blank_lp = torch.zeros(S * R, device=dev, dtype=f32)
-            self.lm_t = C.byref(lm.tables(dev))
 
     def reset(self, slot: int):
         """``reset_decoder`` for one slot: start it at the root on its next frames (the kernel clears the flag) with an empty
@@ -674,21 +654,8 @@ class PoolBeam:
 
     def launch(self):
         """The two launches of one pool step (device inputs only: safe to capture and replay)."""
-        eng, S, R, logits = self.eng, self.S, self.R, self.logits
-        n_view = self.out[1].view(torch.int32)
-        if self.lm is not None:
-            eng._k("ctc_topk", "masr_ctc_topk_blank_f32", _p(logits), eng.Vpad, S * R, eng.V, self.top_n, self.cutoff, 0,
-                   _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n), _p(self.blank_lp))
-            eng._k("prefix_beam", self.lm.BEAM + "_pool", _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n),
-                   _p(self.blank_lp), R, self.lens, S, self.beam, 0, self.lm_t, self.alpha, self.beta,
-                   _p(self.scratch), _p(self.trie_par), _p(self.trie_tok), self.trie_cap, _p(self.state_i), _p(self.state_f),
-                   _p(self.fresh), _p(self.out_tok), self.frames, _p(n_view), _p(self.out[2]), _p(self.out[0]))
-        else:
-            eng._k("ctc_topk", "masr_ctc_topk_f32", _p(logits), eng.Vpad, S * R, eng.V, self.top_n, self.cutoff,
-                   _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n))
-            eng._k("prefix_beam", "masr_ctc_prefix_beam_pool", _p(self.cand_id), _p(self.cand_lp), _p(self.cand_n), R,
-                   self.lens, S, self.beam, 0, _p(self.scratch), _p(self.trie_par), _p(self.trie_tok), self.trie_cap,
-                   _p(self.state_i), _p(self.state_f), _p(self.fresh), _p(self.out_tok), self.frames, _p(n_view), _p(self.out[0]))
+        self.topk(self.eng, self.logits, self.eng.Vpad, self.slots * self.R)
+        self.search(self.eng, self.lens, self.slots, self.R)
 
     def results(self, slots: Sequence[int], frames: Sequence[int]) -> Dict[int, tuple]:
         """slot -> (token ids of its best prefix, score) after the last step: one D2H copy of every slot's count and score,
