@@ -133,42 +133,6 @@ int masr_ffn_tc_f16x2(const void* Ah, const void* Al, int64_t lda, const void* W
                       const void* W2h, const void* W2l, const float* b2, float* x, int64_t ldx, int M, int D, int F,
                       float alpha, void* stream);
 
-/* Sub-layer output projection (N = 256) + residual add + the LayerNorm(s) that follow it, in ONE tensor-core kernel:
- *   x_new = residual + alpha * (A.W^T + bias)
- *   gamma2 == NULL:  X <- x_new,                      (Yh, Yl) <- LN(x_new; gamma1, beta1)
- *                    (conformer/encoder.py:117 -> 122, 131 -> 141, 145 -> 153: the next sub-layer's pre-norm)
- *   gamma2 != NULL:  X <- LN(x_new; gamma1, beta1),   (Yh, Yl) <- LN(X; gamma2, beta2)
- *                    (encoder.py:155 -> 161 `norm_final` -> the next block's 106 `norm_ff_macaron`, or :342 `after_norm`)
- *   Y2 (optional): fp32 copy of what the pair holds.  X, Y2, Yh, Yl share the row pitch ldx; X may alias residual.
- * Launched as clusters of 2 CTAs (the two 128-column tiles of a row block); the row statistics (two-pass mean / centred
- * variance) cross the pair through distributed shared memory.  Same results as masr_gemm_tc_f16x2(MASR_EPI_RESIDUAL)
- * followed by masr_layernorm_split_f16 / masr_layernorm2_split_f16 up to the summation order of the statistics. */
-int masr_gemm_tc_residual_ln_f16x2(const void* Ah, const void* Al, int64_t lda, const void* Wh, const void* Wl,
-                                   const float* bias, const float* residual, int64_t ldr, float alpha, float* X,
-                                   const float* gamma1, const float* beta1, const float* gamma2, const float* beta2,
-                                   float* Y2, void* Yh, void* Yl, int64_t ldx, int M, int N, int K, float eps, void* stream);
-
-/* Post-norm form of the same cluster kernel (Squeezeformer blocks, squeezeformer/encoder.py:412-463):
- *   X <- LN(residual + alpha * (A.W^T + bias); gamma, beta)   becomes the stream,
- *   (Yh, Yl) <- ada_scale * X + ada_bias   (the next sub-module's adaptive scale, positionwise.py:57-58; NULL: the pair of X).
- * Replaces masr_gemm_tc_f16x2(MASR_EPI_RESIDUAL) + masr_layernorm_ada_split_f16 (used by the stream pools, where every launch
- * saved counts: a chunk step is latency-bound). */
-int masr_gemm_tc_residual_postln_f16x2(const void* Ah, const void* Al, int64_t lda, const void* Wh, const void* Wl,
-                                       const float* bias, const float* residual, int64_t ldr, float alpha, float* X,
-                                       const float* gamma, const float* beta, const float* ada_scale, const float* ada_bias,
-                                       void* Yh, void* Yl, int64_t ldx, int M, int N, int K, float eps, void* stream);
-
-/* LayerNorm + Linear in one launch (K = D = 256): C / (Ch, Cl) = epilogue(LN(x; gamma, beta) . W^T + bias) — the pre-norm
- * sub-layer inputs: norm_mha -> linear_q/k/v (encoder.py:122, attention.py:72-74), norm_conv -> pointwise_conv1 + GLU
- * (encoder.py:141, convolution.py:117-118), norm_ff / norm_ff_macaron -> w_1 + SiLU (encoder.py:153/106, positionwise.py:37).
- * Every CTA (pair) takes a contiguous range of output tiles and first normalises the rows of the <= 2 row blocks that range
- * touches into (Ah, Al) — an [M, 256] fp16 (h, l) scratch pair the caller provides; on return it holds LN(x) exactly as
- * masr_layernorm_split_f16 would have written it — then multiplies from it.  epilogue: MASR_EPI_BIAS .. MASR_EPI_BIAS_SCALE.
- * Same results as masr_layernorm_split_f16 + masr_gemm_tc_f16x2, one launch less. */
-int masr_gemm_tc_lnpre_f16x2(const float* x, int64_t ldx, const float* gamma, const float* beta, float eps, void* Ah, void* Al,
-                             int64_t lda, const void* Wh, const void* Wl, const float* bias, float* C, void* Ch, void* Cl,
-                             int64_t ldc, int M, int N, int K, int epilogue, float alpha, void* stream);
-
 /* CTC head without the [M, V] logits: ctc_lo Linear (loss/ctc.py:70) with a GEMM epilogue that keeps, per frame and per
  * 32-column group, (max logit, first argmax, sum exp(x - max)), then a combine kernel -> per-frame argmax id (first
  * maximum, ctc_greedy_decoder.py:21) and max-probability 1 / sum_j exp(x_j - max) (the softmax value of the argmax).

@@ -54,12 +54,6 @@ SIGNATURES = {
     "masr_gemm_f32": [_vp, _i64, _vp, _vp, _vp, _i64, _vp, _i64, _i, _i, _i, _i, _f, _vp],
     "masr_gemm_tc_f16x2": [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _f, _vp],
     "masr_ffn_tc_f16x2": [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _f, _vp],
-    "masr_gemm_tc_residual_ln_f16x2": [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64,
-                                       _i, _i, _i, _f, _vp],
-    "masr_gemm_tc_residual_postln_f16x2": [_vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64,
-                                           _i, _i, _i, _f, _vp],
-    "masr_gemm_tc_lnpre_f16x2": [_vp, _i64, _vp, _vp, _f, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _f,
-                                 _vp],
     "masr_ctc_head_argmax_tc_f16x2": [_vp, _vp, _i64, _vp, _vp, _vp, _i, _i, _i, _vp, _i64, _vp, _vp, _vp],
     "masr_split_f16": [_vp, _vp, _vp, _i64, _vp],
     "masr_conv1_cmvn_relu_planes_f16": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp],

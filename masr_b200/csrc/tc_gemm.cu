@@ -24,13 +24,10 @@
 //                passes of 32 rows -> fused bias/SiLU/ReLU/GLU/scale/residual -> row-contiguous 128-bit stores (fp32
 //                and/or the fp16 (h,l) pair the next GEMM consumes)
 //   warps 8..11  TMA producer (one elected thread): 4 boxes per K-block (Ah, Al, Wh, Wl; 32 halves = one 64-byte swizzle row)
-//   smem ring of 5 x 32 KB stages (BK = 32, 64-byte swizzle; 4 stages in the LayerNorm-epilogue variant) with full/empty
-//   mbarriers beside the 64 KB result tile; the producer runs up to 160 of K (128 with LNC) ahead, also into the next tile
-//   while the consumers run the epilogue.  Launched with programmatic dependent
-//   launch: the prologue overlaps the producer kernel's tail.
-// EPI_CTC_PARTIAL keeps per (row, 32 columns) softmax partials instead of logits (+ ctc_partial_combine_kernel);
-// the LNC variant (clusters of 2 CTAs) fuses the LayerNorm(s) that follow a residual projection, row statistics over DSMEM
-// (pre-norm LN / LN2 and the Squeezeformer's post-norm + adaptive scale).
+//   smem ring of 5 x 32 KB stages (BK = 32, 64-byte swizzle) with full/empty mbarriers beside the 64 KB result tile; the
+//   producer runs up to 160 of K ahead, also into the next tile while the consumers run the epilogue.  Launched with
+//   programmatic dependent launch: the prologue overlaps the producer kernel's tail.
+// EPI_CTC_PARTIAL keeps per (row, 32 columns) softmax partials instead of logits (+ ctc_partial_combine_kernel).
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <math.h>
@@ -46,8 +43,7 @@ constexpr int TBM = 128, TBN = 128, TBK = 32;
 constexpr int TILE_BYTES = TBM * TBK * 2;              // 8 KB: one operand tile
 constexpr int STAGE_BYTES = 4 * TILE_BYTES;            // Ah, Al, Wh, Wl
 constexpr int EW = 8;                                  // consumer / epilogue warps (two warpgroups)
-// ring depth: 5 x 32 KB stages; 4 in the LayerNorm-epilogue variant, whose 16 KB of row statistics take the fifth's room
-template <bool LNC> constexpr int kStages = LNC ? 4 : 5;
+constexpr int kStages = 5;                             // ring depth: 5 x 32 KB stages
 constexpr int RES_BYTES = TBM * TBN * 4;               // fp32 result tile, 32 KB per consumer warpgroup
 constexpr int TC_THREADS = 32 * EW + 128;              // + the TMA producer warpgroup
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232; // setmaxnreg: 40 x 128 + 232 x 256 <= 65536
@@ -66,65 +62,14 @@ struct TcParams {
     // conv mode (implicit GEMM over parity planes of the conv-1 activation)
     int conv_T2;       // output rows per utterance (T2max)
     int flags;         // bit 0: stage epilogue stores through shared memory (row-contiguous global writes)
-    // MASR_EPI_RESIDUAL_LN / _LN2 (cluster kernel): LayerNorm(s) of the finished 256-wide row fused behind the residual add
-    const float* ln_g;
-    const float* ln_b;
-    const float* ln_g2;
-    const float* ln_b2;
-    float* y2;         // optional fp32 copy of the last LayerNorm's output (row pitch ldc)
-    float ln_eps;
     // MASR_EPI_CTC_PARTIAL: per (row, 32-column group) softmax partials [group][M] instead of logits
     float* part_m;
     float* part_s;
     int* part_i;
-    const float* ada_s;   // EPI_RESIDUAL_POSTLN: optional per-channel scale / bias applied to the LayerNorm output for the pair
-    const float* ada_b;
-    // LayerNorm prologue (masr_gemm_tc_lnpre_f16x2, K = 256): the A operand is LayerNorm(lnp_x; ln_g, ln_b) — every CTA
-    // normalises the rows of its own tiles into the pair buffer (lnp_h, lnp_l: the A tensor maps point at it) before loading them
-    const float* lnp_x;
-    int64_t lnp_ldx, lnp_ld;
-    __half* lnp_h;
-    __half* lnp_l;
 };
 
-// One LayerNorm row of width 256 by one warp -> the fp16 (h, l) operand pair.  Lane l holds columns (i*32 + l)*4 .. +3, i = 0, 1:
-// the arithmetic, and its order, of layernorm_kernel<256, true> (norm.cu), so the fused path is bit-identical to the separate one.
-__device__ __forceinline__ void ln_row256_split(const float4 (&v)[2], const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                float eps, int lane, __half* __restrict__ yh, __half* __restrict__ yl) {
-    float s = 0.f;
-#pragma unroll
-    for (int i = 0; i < 2; ++i) s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
-    const float mean = warp_sum(s) * (1.0f / 256);
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-        float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, d = v[i].w - mean;
-        q += (a * a + b * b) + (c * c + d * d);
-    }
-    const float rstd = rsqrtf(warp_sum(q) * (1.0f / 256) + eps);
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-        const int c = (i * 32 + lane) * 4;
-        float4 g = ldg_f4(gamma + c), b = ldg_f4(beta + c);
-        float4 o;
-        o.x = (v[i].x - mean) * rstd * g.x + b.x;
-        o.y = (v[i].y - mean) * rstd * g.y + b.y;
-        o.z = (v[i].z - mean) * rstd * g.z + b.z;
-        o.w = (v[i].w - mean) * rstd * g.w + b.w;
-        __half hh[4], ll[4];
-        const float ov[4] = {o.x, o.y, o.z, o.w};
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            hh[j] = __float2half_rn(ov[j]);
-            ll[j] = __float2half_rn((ov[j] - __half2float(hh[j])) * 2048.0f);
-        }
-        *reinterpret_cast<uint2*>(yh + c) = *reinterpret_cast<const uint2*>(hh);
-        *reinterpret_cast<uint2*>(yl + c) = *reinterpret_cast<const uint2*>(ll);
-    }
-}
-
-// internal epilogue codes (continuing include/masr_b200.h's MASR_EPI_*)
-constexpr int EPI_RESIDUAL_LN = 6, EPI_RESIDUAL_LN2 = 7, EPI_CTC_PARTIAL = 8, EPI_RESIDUAL_POSTLN = 9;
+// internal epilogue code (beyond include/masr_b200.h's MASR_EPI_*)
+constexpr int EPI_CTC_PARTIAL = 8;
 
 struct TcMaps {
     CUtensorMap a[8];  // GEMM: a[0]=Ah, a[1]=Al.  CONV: a[2*plane + {0:h,1:l}], plane = (kh&1)*2 + (kw&1)
@@ -281,85 +226,12 @@ __device__ __forceinline__ void emit(const TcParams& p, const EpiCtx& c, const f
     if (p.Ch) emit_pair<W, STG>(c, p.Ch, p.Cl, p.ldc, p.flags, o, n, n_limit);
 }
 
-// ---- LayerNorm fused behind the residual epilogue (cluster of 2 CTAs) --------------------------------------------------------
-// A 256-wide output row is spread over 2 CTAs (the two 128-column tiles of one row block = one cluster) x 4 epilogue warps
-// (32 columns each), one thread per (row, 32 columns).  Row statistics are exchanged through distributed shared memory:
-// every thread stores its partial into BOTH CTAs' `red[buf][src cta][column group][row]`, one lane per warp arrives
-// (release.cluster) on both CTAs' mbarrier, everybody waits on its own (acquire.cluster) and sums the 8 partials in a fixed
-// order — both CTAs obtain bit-identical statistics.  Two-pass (mean, then centred variance) like norm.cu; rounds alternate
-// between two buffers / two barriers, so a fast warp can never overwrite or complete a round that a slow one still reads.
-struct LnCtx {
-    uint32_t red, red_peer;      // shared::cta / shared::cluster byte addresses of red[2][2][4][128] float2
-    uint32_t bar, bar_peer;      // ... of the two mbarriers
-    uint32_t rank, cgrp, row, lane;
-    uint32_t round;
-};
-
-// o = LayerNorm(v) * gamma + beta over the 256-wide row this thread holds 32 columns of (g, b: pointers to those columns).
-// ONE exchange per LayerNorm: every thread sends the mean and the centred sum of squares of its own 32 values (two-pass,
-// in registers); the 8 partials of a row are combined with the pairwise-update formula of Chan et al. (equal counts):
-//   mean = sum(m_i) / 8,   M2 = sum(M2_i) + 32 * sum((m_i - mean)^2),   var = M2 / 256
-// — as stable as the two-pass form of norm.cu.  Must be called BEFORE the thread's global stores of the tile: the
-// release.cluster arrive orders all earlier writes of the thread, and waiting for outstanding global stores there cost
-// several microseconds per exchange in the first version.
-__device__ __forceinline__ void ln_apply(LnCtx& L, const float (&v)[32], float (&o)[32], const float* g, const float* b, float eps) {
-    float s = 0.f;
-#pragma unroll
-    for (int j = 0; j < 32; j += 4) s += (v[j] + v[j + 1]) + (v[j + 2] + v[j + 3]);
-    const float m_loc = s * (1.0f / 32.0f);
-    float q = 0.f;
-#pragma unroll
-    for (int j = 0; j < 32; j += 4) {
-        const float a0 = v[j] - m_loc, a1 = v[j + 1] - m_loc, a2 = v[j + 2] - m_loc, a3 = v[j + 3] - m_loc;
-        q += (a0 * a0 + a1 * a1) + (a2 * a2 + a3 * a3);
-    }
-    const uint32_t buf = L.round & 1;
-    const uint32_t off = ((((buf * 2 + L.rank) * 4 + L.cgrp) * 128) + L.row) * 8;
-    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(L.red + off), "f"(m_loc), "f"(q) : "memory");
-    asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(L.red_peer + off), "f"(m_loc), "f"(q) : "memory");
-    __syncwarp();
-    if (L.lane == 0) {
-        asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(L.bar + buf * 8) : "memory");
-        asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(L.bar_peer + buf * 8) : "memory");
-    }
-    const uint32_t parity = (L.round >> 1) & 1;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred P1;\n\t"
-        "LN_WAIT:\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 P1, [%0], %1;\n\t"
-        "@P1 bra LN_DONE;\n\t"
-        "bra LN_WAIT;\n\t"
-        "LN_DONE:\n\t"
-        "}" ::"r"(L.bar + buf * 8), "r"(parity) : "memory");
-    float pm[8], pq[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k)      // fixed order: both CTAs obtain bit-identical statistics
-        asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(pm[k]), "=f"(pq[k]) : "r"(L.red + (((buf * 8 + k) * 128) + L.row) * 8) : "memory");
-    ++L.round;
-    const float mean = (((pm[0] + pm[1]) + (pm[2] + pm[3])) + ((pm[4] + pm[5]) + (pm[6] + pm[7]))) * 0.125f;
-    float m2 = ((pq[0] + pq[1]) + (pq[2] + pq[3])) + ((pq[4] + pq[5]) + (pq[6] + pq[7]));
-    float dev2 = 0.f;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) { const float dm = pm[k] - mean; dev2 += dm * dm; }
-    m2 = fmaf(32.0f, dev2, m2);
-    const float rstd = rsqrtf(m2 * (1.0f / 256.0f) + eps);
-#pragma unroll
-    for (int j = 0; j < 32; j += 4) {
-        const float4 gg = ldg_f4(g + j), bb = ldg_f4(b + j);          // warp-uniform addresses: one broadcast transaction
-        o[j] = (v[j] - mean) * rstd * gg.x + bb.x;
-        o[j + 1] = (v[j + 1] - mean) * rstd * gg.y + bb.y;
-        o[j + 2] = (v[j + 2] - mean) * rstd * gg.z + bb.z;
-        o[j + 3] = (v[j + 3] - mean) * rstd * gg.w + bb.w;
-    }
-}
-
 // One 32-column slice of a finished output row: bias was already added; apply the epilogue and store.
 // `n` is the global column of v[0] (warp-uniform).
-template <int STG, bool LNC>
-__device__ __forceinline__ void store_chunk(const TcParams& p, const EpiCtx& c, float (&v)[32], int n, LnCtx& L) {
+template <int STG>
+__device__ __forceinline__ void store_chunk(const TcParams& p, const EpiCtx& c, float (&v)[32], int n) {
     constexpr bool BIG = STG >= 4096;
-    if (!LNC && p.epi == EPI_CTC_PARTIAL) {
+    if (p.epi == EPI_CTC_PARTIAL) {
         // CTC head (loss/ctc.py:70 softmax + ctc_greedy_decoder.py:21 argmax): keep only this (row, 32-column group)'s
         // softmax partials — max logit, its first column, sum of exp(x - max) — the [M, V] logits never reach HBM
         if (n + 31 >= p.N) {                                               // ragged last group (warp-uniform): mask once
@@ -401,7 +273,7 @@ __device__ __forceinline__ void store_chunk(const TcParams& p, const EpiCtx& c, 
         emit<16, STG>(p, c, o, n >> 1, p.N >> 1);
         return;
     }
-    switch (LNC ? (int)MASR_EPI_RESIDUAL : p.epi) {
+    switch (p.epi) {
         case MASR_EPI_BIAS_SILU:
             // eight independent SFU chains at a time (a one-register serial chain would outlast the MMA loop)
 #pragma unroll
@@ -457,37 +329,6 @@ __device__ __forceinline__ void store_chunk(const TcParams& p, const EpiCtx& c, 
         }
         default: break;
     }
-    if (LNC) {
-        // v = x + alpha * sublayer(x): the new residual stream.  EPI_RESIDUAL_LN: C <- v, pair <- LN(v) (the next sub-layer's
-        // GEMM operand).  EPI_RESIDUAL_LN2: C <- LN1(v) (norm_final: the block output replaces x), pair <- LN2(LN1(v)).
-        // (all statistics exchanges come before the first global store of the tile, see ln_apply)
-        float o[32];
-        ln_apply(L, v, o, p.ln_g + n, p.ln_b + n, p.ln_eps);
-        if (p.epi == EPI_RESIDUAL_POSTLN) {
-            // post-norm block (Squeezeformer): the stream becomes LN(v); the pair carries the next sub-module's adaptive
-            // scale / bias applied to it (squeezeformer/positionwise.py:57-58), or the LayerNorm output itself
-            emit_f32<32, STG>(c, p.C, p.ldc, p.flags, o, n, p.N);
-            if (p.ada_s) {
-#pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    const float4 as = ldg_f4(p.ada_s + n + j), ab = ldg_f4(p.ada_b + n + j);
-                    o[j] = as.x * o[j] + ab.x; o[j + 1] = as.y * o[j + 1] + ab.y;
-                    o[j + 2] = as.z * o[j + 2] + ab.z; o[j + 3] = as.w * o[j + 3] + ab.w;
-                }
-            }
-            emit_pair<32, STG>(c, p.Ch, p.Cl, p.ldc, p.flags, o, n, p.N);
-        } else if (p.epi == EPI_RESIDUAL_LN2) {
-            ln_apply(L, o, v, p.ln_g2 + n, p.ln_b2 + n, p.ln_eps);
-            emit_f32<32, STG>(c, p.C, p.ldc, p.flags, o, n, p.N);
-            if (p.y2) emit_f32<32, STG>(c, p.y2, p.ldc, p.flags, v, n, p.N);
-            emit_pair<32, STG>(c, p.Ch, p.Cl, p.ldc, p.flags, v, n, p.N);
-        } else {
-            emit_f32<32, STG>(c, p.C, p.ldc, p.flags, v, n, p.N);
-            if (p.y2) emit_f32<32, STG>(c, p.y2, p.ldc, p.flags, o, n, p.N);
-            emit_pair<32, STG>(c, p.Ch, p.Cl, p.ldc, p.flags, o, n, p.N);
-        }
-        return;
-    }
     emit<32, STG>(p, c, v, n, p.N);
 }
 
@@ -497,63 +338,31 @@ __device__ __forceinline__ void store_chunk(const TcParams& p, const EpiCtx& c, 
 // running sum.  The correction product is 2^-11 smaller, so its drift is irrelevant and it accumulates over the tile.
 //
 // Persistent: grid = min(#tiles, #SMs); every CTA walks tiles blockIdx.x, +gridDim.x, ...
-// LNC: the LayerNorm-fused variant (N = 256, launched as clusters of 2 CTAs = the two column tiles of a row block).
-constexpr int LN_RED_BYTES = 2 * 2 * 4 * 128 * 8;     // red[buffer][source CTA][column group][row] (mean, M2)
 constexpr int EPI_STG = 4096;                         // a warp's 32 x 32 fp32 block of the result tile, reused as its store staging
 
 // byte offset of (row r, column c) inside a warp's 32 x 32 fp32 block: 16-byte chunks XOR-swizzled by row, so that one
 // thread per row reading its 32 values (and staged_store<8>) is conflict-free
 __device__ __forceinline__ uint32_t res_off(int r, int c) { return (uint32_t)(r * 128 + ((((c >> 2) ^ (r & 7))) << 4) + (c & 3) * 4); }
 
-// PAIR: clusters of 2 CTAs own 256 x 128 tiles — CTA r computes rows [128 r, 128 r + 128) and loads W rows (output
-// columns) [64 r, 64 r + 64) of every K-block by TMA multicast into BOTH CTAs' stage, so each W tile crosses L2 -> SM once
-// per pair.  A stage is refilled only when the consumer warps of both CTAs have released it (empty barrier: 2 x 8
-// arrivals, half of them remote).  Same products in the same order as the single-CTA form: bit-identical outputs.
-template <bool CONV, bool LNC, bool PAIR = false>
+// p is read in place from the parameter space (__grid_constant__): taken by value, ptxas spills the tile counter at 168 registers
+template <bool CONV>
 __global__ void __launch_bounds__(TC_THREADS, 1)
-tc_gemm_kernel(const __grid_constant__ TcMaps maps, TcParams p, int num_tiles, int tiles_n, int tiles_t) {
+tc_gemm_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcParams p, int num_tiles, int tiles_n, int tiles_t) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    constexpr int TSTAGES = kStages<LNC>;
-    uint8_t* res = smem + TSTAGES * STAGE_BYTES;                      // fp32 result tile: [warpgroup][row group][column group] x 4 KB
-    uint8_t* ln_red = res + RES_BYTES;                                // LNC only
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(ln_red + (LNC ? LN_RED_BYTES : 0));
-    uint64_t* empty_bar = full_bar + TSTAGES;
-    uint64_t* ln_bar = empty_bar + TSTAGES;        // [2] (LNC; lnp: [0])
+    uint8_t* res = smem + kStages * STAGE_BYTES;                      // fp32 result tile: [warpgroup][row group][column group] x 4 KB
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(res + RES_BYTES);
+    uint64_t* empty_bar = full_bar + kStages;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nkb = p.K / TBK;
-    static_assert(!(LNC && PAIR), "the LayerNorm-fused kernel pairs CTAs along N, the PAIR kernel along M");
-    uint32_t crank = 0;                                               // PAIR: rank in the cluster
-    if (PAIR) asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(crank));
-    const int tile_first = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-    const int tile_step = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-    // Tile schedule: CTA u of U walks tiles u, u + U, ... — or, with the LayerNorm prologue, the contiguous range
-    // [T u / U, T (u + 1) / U) (column tile fastest), so that it needs the rows of at most two row blocks and can normalise
-    // them itself up front.
-    const bool lnp = !LNC && !CONV && p.lnp_x != nullptr;
-    const int tile_begin = lnp ? (int)((int64_t)num_tiles * tile_first / tile_step) : tile_first;
-    const int tile_end = lnp ? (int)((int64_t)num_tiles * (tile_first + 1) / tile_step) : num_tiles;
-    const int tile_stride = lnp ? 1 : tile_step;
 
     if (warp == EW && lane == 0) {
         tma_prefetch_desc(&maps.a[0]); tma_prefetch_desc(&maps.a[1]); tma_prefetch_desc(&maps.w[0]); tma_prefetch_desc(&maps.w[1]);
-        for (int s = 0; s < TSTAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], PAIR ? 2 * EW : EW); }
-        for (int s = 0; s < 2; ++s) {
-            if (LNC) mbar_init(&ln_bar[s], 2 * EW);                  // one arrival per epilogue warp of both CTAs
-            else if (lnp) mbar_init(&ln_bar[s], EW);                 // [0]: this CTA's rows are normalised
-        }
+        for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], EW); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    // the peer CTA must have initialised its barriers before anybody arrives on them remotely: arrive here, wait (long
-    // since complete) right before the first exchange / after the producer loop
-    if (LNC) asm volatile("barrier.cluster.arrive.release;" ::: "memory");
-    // PAIR: the peer's multicast bytes and releases may only reach barriers that have been initialised
-    if (PAIR) {
-        asm volatile("barrier.cluster.arrive.release;" ::: "memory");
-        asm volatile("barrier.cluster.wait.acquire;" ::: "memory");
-    }
     // programmatic dependent launch: everything above overlapped the producer kernel's tail; no global memory touched yet
     pdl_wait();
     pdl_launch_dependents();
@@ -562,10 +371,8 @@ tc_gemm_kernel(const __grid_constant__ TcMaps maps, TcParams p, int num_tiles, i
         const int nt = tile % tiles_n;
         const int rest = tile / tiles_n;
         n0 = nt * TBN;
-        // PAIR: `tile` numbers 256-row (CONV: 12 time rows) pair tiles, this CTA owns half `crank` of it; a half beyond
-        // M / T2 loads zeros and stores nothing
-        if (CONV) { t0 = ((rest % tiles_t) * (PAIR ? 2 : 1) + (int)crank) * CONV_TR; b = rest / tiles_t; m0 = 0; }
-        else { m0 = (rest * (PAIR ? 2 : 1) + (int)crank) * TBM; t0 = 0; b = 0; }
+        if (CONV) { t0 = (rest % tiles_t) * CONV_TR; b = rest / tiles_t; m0 = 0; }
+        else { m0 = rest * TBM; t0 = 0; b = 0; }
     };
 
     if (warp >= EW) {
@@ -576,13 +383,12 @@ tc_gemm_kernel(const __grid_constant__ TcMaps maps, TcParams p, int num_tiles, i
             constexpr uint32_t tx_bytes = 2 * a_bytes + 2 * TILE_BYTES;
             uint32_t kg = 0;
             const int kb_tap = CONV ? p.N / TBK : 1;   // CONV: K-blocks per tap (K = 9 C, N = C: 8 at C = 256, 16 = two chunks at 512)
-            if (lnp) mbar_wait(&ln_bar[0], 0);      // the consumer warps have written this CTA's A rows (LayerNorm prologue)
-            for (int tile = tile_begin; tile < tile_end; tile += tile_stride) {
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
                 int n0, m0, t0, b;
                 decode(tile, n0, m0, t0, b);
                 for (int kb = 0; kb < nkb; ++kb, ++kg) {
-                    const uint32_t s = kg % TSTAGES;
-                    mbar_wait(&empty_bar[s], ((kg / TSTAGES) & 1) ^ 1);
+                    const uint32_t s = kg % kStages;
+                    mbar_wait(&empty_bar[s], ((kg / kStages) & 1) ^ 1);
                     uint8_t* st = smem + s * STAGE_BYTES;
                     if (p.flags & 32) {      // profiling switch (tools/gemm_bound_probe.py): no loads, the MMAs run on stale tiles
                         mbar_arrive(&full_bar[s]);
@@ -599,19 +405,12 @@ tc_gemm_kernel(const __grid_constant__ TcMaps maps, TcParams p, int num_tiles, i
                         tma_load_2d(&maps.a[0], &full_bar[s], st, kb * TBK, m0);
                         tma_load_2d(&maps.a[1], &full_bar[s], st + TILE_BYTES, kb * TBK, m0);
                     }
-                    if (PAIR) {          // box: 64 rows, this CTA's half of the W tile, to both CTAs
-                        const uint32_t half = crank * (TILE_BYTES / 2);
-                        tma_load_2d_mc(&maps.w[0], &full_bar[s], st + 2 * TILE_BYTES + half, kb * TBK, n0 + (int)crank * (TBN / 2), 3);
-                        tma_load_2d_mc(&maps.w[1], &full_bar[s], st + 3 * TILE_BYTES + half, kb * TBK, n0 + (int)crank * (TBN / 2), 3);
-                    } else {
-                        tma_load_2d(&maps.w[0], &full_bar[s], st + 2 * TILE_BYTES, kb * TBK, n0);
-                        tma_load_2d(&maps.w[1], &full_bar[s], st + 3 * TILE_BYTES, kb * TBK, n0);
-                    }
+                    tma_load_2d(&maps.w[0], &full_bar[s], st + 2 * TILE_BYTES, kb * TBK, n0);
+                    tma_load_2d(&maps.w[1], &full_bar[s], st + 3 * TILE_BYTES, kb * TBK, n0);
                 }
             }
         }
         __syncwarp();
-        if (LNC) asm volatile("barrier.cluster.wait.acquire;" ::: "memory");
     } else {
         // ---- 2 consumer warpgroups: wg owns tile rows [64 wg, +64) x all 128 columns ----
         setmaxnreg_inc<CONSUMER_REGS>();
@@ -620,16 +419,6 @@ tc_gemm_kernel(const __grid_constant__ TcMaps maps, TcParams p, int num_tiles, i
         const int nchunks = (nkb + CHUNK_KB - 1) / CHUNK_KB;
         EpiCtx ctx;
         ctx.lane = lane;
-        LnCtx lnx;
-        if (LNC) {
-            uint32_t rank;
-            asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
-            lnx.rank = rank; lnx.cgrp = (uint32_t)wi; lnx.lane = (uint32_t)lane; lnx.round = 0;
-            lnx.red = smem_u32(ln_red); lnx.bar = smem_u32(ln_bar);
-            asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(lnx.red_peer) : "r"(lnx.red), "r"(rank ^ 1u));
-            asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(lnx.bar_peer) : "r"(lnx.bar), "r"(rank ^ 1u));
-            asm volatile("barrier.cluster.wait.acquire;" ::: "memory");
-        }
         // row mapping: the warp's 32 tile rows (group q) are 32 consecutive output rows in both modes
         auto map_rows = [&](int m0, int t0, int b, int q) {
             if (CONV) {
@@ -642,58 +431,15 @@ tc_gemm_kernel(const __grid_constant__ TcMaps maps, TcParams p, int num_tiles, i
                 ctx.nvalid = max(0, min(32, p.M - (m0 + q * 32)));
             }
         };
-        if (lnp) {
-            // LayerNorm prologue: the 8 consumer warps normalise this CTA's 128 rows of every row block its tile range touches
-            // (16 rows per warp and block, 4 rows in flight) into the pair buffer the A loads read.  A block shared with the
-            // neighbouring CTA's range is written twice with identical values.
-            if (tile_begin < tile_end) {
-                const int b0 = tile_begin / tiles_n, b1 = (tile_end - 1) / tiles_n;
-                for (int blk = b0; blk <= b1; ++blk) {
-                    const int mrow0 = (blk * (PAIR ? 2 : 1) + (int)crank) * TBM + warp * (TBM / EW);
-#pragma unroll
-                    for (int r4 = 0; r4 < TBM / EW; r4 += 4) {
-                        float4 xv[4][2];
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            const int row = mrow0 + r4 + k;
-                            if (row < p.M) {
-                                const float* xr = p.lnp_x + (int64_t)row * p.lnp_ldx;
-                                xv[k][0] = ldg_f4(xr + lane * 4);
-                                xv[k][1] = ldg_f4(xr + (32 + lane) * 4);
-                            }
-                        }
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            const int row = mrow0 + r4 + k;
-                            if (row < p.M)                          // warp-uniform
-                                ln_row256_split(xv[k], p.ln_g, p.ln_b, p.ln_eps, lane, p.lnp_h + (int64_t)row * p.lnp_ld,
-                                                p.lnp_l + (int64_t)row * p.lnp_ld);
-                        }
-                    }
-                }
-            }
-            // generic-proxy global writes -> ordered before the TMA loads (async proxy) the producer issues after the barrier
-            __threadfence();
-            asm volatile("fence.proxy.async.global;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&ln_bar[0]);
-        }
         const uint32_t wg_bar = 1 + wg;              // named barrier of the warpgroup (0 is __syncthreads)
-        // this warp's MMAs on stage s have retired: lane 0 arrives (and, PAIR, on the peer's barrier: it multicasts into this
-        // stage too), as predicated instructions rather than a branch.
+        // this warp's MMAs on stage s have retired: lane 0 arrives, as a predicated instruction rather than a branch
         const uint32_t is_lane0 = lane == 0;
         auto release = [&](uint32_t s) {
             asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}"
                          ::"r"(smem_u32(&empty_bar[s])), "r"(is_lane0) : "memory");
-            if (PAIR) {
-                uint32_t a;
-                asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(a) : "r"(smem_u32(&empty_bar[s])), "r"(crank ^ 1u));
-                asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %1, 0;\n\t@p mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];\n\t}"
-                             ::"r"(a), "r"(is_lane0) : "memory");
-            }
         };
         uint32_t kg = 0;
-        for (int tile = tile_begin; tile < tile_end; tile += tile_stride) {
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             int n0, m0, t0, b;
             decode(tile, n0, m0, t0, b);
             const int nw = n0 + wi * 32;                               // first column of this warp's epilogue blocks
@@ -709,16 +455,16 @@ tc_gemm_kernel(const __grid_constant__ TcMaps maps, TcParams p, int num_tiles, i
             asm volatile("bar.sync %0, 128;" ::"r"(wg_bar) : "memory");   // every warp is done with the previous tile's blocks
             if (p.flags & 64) {      // profiling switch: loads only, no MMAs
                 for (int kb = 0; kb < nkb; ++kb, ++kg) {
-                    const uint32_t s = kg % TSTAGES;
-                    mbar_wait(&full_bar[s], (kg / TSTAGES) & 1);
+                    const uint32_t s = kg % kStages;
+                    mbar_wait(&full_bar[s], (kg / kStages) & 1);
                     release(s);
                 }
             } else for (int c = 0; c < nchunks; ++c) {
                 const int kb_end = min(nkb, (c + 1) * CHUNK_KB);
                 int pend = -1;                                         // stage whose MMAs are still in flight
                 for (int kb = c * CHUNK_KB; kb < kb_end; ++kb, ++kg) {
-                    const uint32_t s = kg % TSTAGES;
-                    mbar_wait(&full_bar[s], (kg / TSTAGES) & 1);
+                    const uint32_t s = kg % kStages;
+                    mbar_wait(&full_bar[s], (kg / kStages) & 1);
                     const uint32_t sa = smem_u32(smem + s * STAGE_BYTES);
                     const uint32_t sa_m = sa + wg * (TILE_BYTES / 2), sw = sa + 2 * TILE_BYTES;
                     const uint64_t dAh = gmma_desc_sw64(sa_m), dAl = gmma_desc_sw64(sa_m + TILE_BYTES);
@@ -778,13 +524,11 @@ tc_gemm_kernel(const __grid_constant__ TcMaps maps, TcParams p, int num_tiles, i
                     asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(x0), "f"(x1) : "memory");
                 }
             asm volatile("bar.sync %0, 128;" ::"r"(wg_bar) : "memory");
-            // epilogue: pass h covers the 32-row group q = 2 wg + h; warp wi takes its block of column group wi.  All four
-            // column groups of a row are in the same pass (the LayerNorm epilogue exchanges row statistics among them).
+            // epilogue: pass h covers the 32-row group q = 2 wg + h; warp wi takes its block of column group wi
             for (int h = 0; h < 2; ++h) {
                 const int q = 2 * wg + h;
                 map_rows(m0, t0, b, q);
                 ctx.sb = smem_u32(wg_res) + (h * 4 + wi) * EPI_STG;
-                if (LNC) lnx.row = (uint32_t)(q * 32 + lane);
                 if (nw >= p.N) continue;                               // warp-uniform
                 float v[32];
 #pragma unroll
@@ -804,22 +548,16 @@ tc_gemm_kernel(const __grid_constant__ TcMaps maps, TcParams p, int num_tiles, i
                     for (int j = 0; j < 32; ++j)
                         if (nw + j < p.N) v[j] += __ldg(p.bias + nw + j);
                 }
-                store_chunk<EPI_STG, LNC>(p, ctx, v, nw, lnx);
+                store_chunk<EPI_STG>(p, ctx, v, nw);
             }
         }
     }
     __syncthreads();
-    if (LNC || PAIR) {      // neither CTA may exit while its peer can still write into its shared memory / arrive on its barriers
-        asm volatile("barrier.cluster.arrive.release;" ::: "memory");
-        asm volatile("barrier.cluster.wait.acquire;" ::: "memory");
-    }
 }
 
-// shared memory: ring + result tile (+ LayerNorm statistics) + 1024 B for the 1024-byte alignment the 128-byte
-// swizzle needs + 256 B of mbarriers
-constexpr size_t kTcSmem = kStages<false> * STAGE_BYTES + RES_BYTES + 1024 + 256;
-constexpr size_t kTcSmemLn = kStages<true> * STAGE_BYTES + RES_BYTES + LN_RED_BYTES + 1024 + 256;
-static_assert(kTcSmem <= 232448 && kTcSmemLn <= 232448, "tc_gemm shared memory exceeds the 227 KB per-CTA limit of sm_90");
+// shared memory: ring + result tile + 1024 B for the 1024-byte alignment the 128-byte swizzle needs + 256 B of mbarriers
+constexpr size_t kTcSmem = kStages * STAGE_BYTES + RES_BYTES + 1024 + 256;
+static_assert(kTcSmem <= 232448, "tc_gemm shared memory exceeds the 227 KB per-CTA limit of sm_90");
 
 // ---- fp32 -> (h,l) split, elementwise (weights at load time; activations produced by SIMT kernels) ----
 __global__ void __launch_bounds__(256) split_f16_kernel(const float* __restrict__ x, __half* __restrict__ h,
@@ -878,14 +616,14 @@ __global__ void __launch_bounds__(128) ctc_partial_combine_kernel(const float* _
 }
 
 // ---- host: tensor maps ----------------------------------------------------------------------------
-// [rows, K] fp16 row-major (ld elements), box = 32 (K) x box_rows (128),
+// [rows, K] fp16 row-major (ld elements), box = 32 (K) x 128,
 // 64-byte swizzle, zero OOB fill
-static int make_map_2d(CUtensorMap* map, const void* ptr, int64_t rows, int64_t K, int64_t ld, int box_rows = TBM) {
+static int make_map_2d(CUtensorMap* map, const void* ptr, int64_t rows, int64_t K, int64_t ld) {
     EncodeTiledFn fn = get_encode_fn();
     if (!fn) { set_last_error("cuTensorMapEncodeTiled entry point unavailable"); return MASR_ERR_INTERNAL; }
     cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
     cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-    cuuint32_t box[2] = {(cuuint32_t)TBK, (cuuint32_t)box_rows};
+    cuuint32_t box[2] = {(cuuint32_t)TBK, (cuuint32_t)TBM};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
@@ -938,52 +676,21 @@ static int ensure_tc_attrs() {
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) dev = 0;
     if (!g_tc_attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(tc_gemm_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gemm_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gemm_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmemLn);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gemm_kernel<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gemm_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem);
+        cudaError_t e = cudaFuncSetAttribute(tc_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmem);
         if (e != cudaSuccess) { set_last_error("tc_gemm smem attr: %s", cudaGetErrorString(e)); return (int)e; }
         g_tc_attr_set[dev] = true;
     }
     return MASR_OK;
 }
 
-// PAIR kernels (clusters of 2 CTAs along M, W multicast) with MASR_TC_PAIR=1, wherever there is more than one row block;
-// read per call, the A/B tools flip it inside one process.  Off by default: H100 (400 W), headline step 10.95 ms paired vs
-// 8.25 ms single-CTA.
-static bool pair_enabled(bool several_row_blocks) {
-    const char* e = getenv("MASR_TC_PAIR");
-    return several_row_blocks && e != nullptr && atoi(e) != 0;
-}
-
 // Persistent launch over `tiles_m` row blocks (CONV: time-row tiles per utterance, `batch` utterances) x `tiles_n` column
-// tiles: min(#tiles, #SMs) CTAs, or with `pair` min(#pair tiles, #SMs / 2) clusters of 2 CTAs.  The W tensor maps must
-// have 64-row boxes for the pair form.
+// tiles: min(#tiles, #SMs) CTAs.
 template <bool CONV>
-static void launch_tc(const TcMaps& maps, const TcParams& p, bool pair, int tiles_n, int tiles_m, int batch, cudaStream_t stream) {
-    if (!pair) {
-        const int num_tiles = tiles_n * tiles_m * batch;
-        const int grid = num_tiles < num_sms() ? num_tiles : num_sms();
-        launch_pdl(tc_gemm_kernel<CONV, false>, dim3(grid), dim3(TC_THREADS), kTcSmem, stream, maps, p, num_tiles, tiles_n, tiles_m);
-        return;
-    }
-    const int ptiles_m = (tiles_m + 1) / 2;
-    const int num_ptiles = tiles_n * ptiles_m * batch;
-    const int pairs = num_ptiles < num_sms() / 2 ? num_ptiles : num_sms() / 2;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * pairs);
-    cfg.blockDim = dim3(TC_THREADS);
-    cfg.dynamicSmemBytes = kTcSmem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    cudaLaunchKernelEx(&cfg, tc_gemm_kernel<CONV, false, true>, maps, p, num_ptiles, tiles_n, ptiles_m);
+static void launch_tc(const TcMaps& maps, const TcParams& p, int tiles_n, int tiles_m, int batch, cudaStream_t stream) {
+    const int num_tiles = tiles_n * tiles_m * batch;
+    const int grid = num_tiles < num_sms() ? num_tiles : num_sms();
+    launch_pdl(tc_gemm_kernel<CONV>, dim3(grid), dim3(TC_THREADS), kTcSmem, stream, maps, p, num_tiles, tiles_n, tiles_m);
 }
 
 }  // namespace masr
@@ -1008,13 +715,12 @@ extern "C" int masr_conv2_tc_f16x2(const void* c1h, const void* c1l, const void*
         if ((rc = make_map_plane(&maps.a[2 * pl], (const __half*)c1h + pl * plane_elems, B, TH, C))) return rc;
         if ((rc = make_map_plane(&maps.a[2 * pl + 1], (const __half*)c1l + pl * plane_elems, B, TH, C))) return rc;
     }
-    const bool pair = pair_enabled(T2 > CONV_TR);
-    if ((rc = make_map_2d(&maps.w[0], Wh, C, 9 * C, 9 * C, pair ? TBN / 2 : TBN))) return rc;
-    if ((rc = make_map_2d(&maps.w[1], Wl, C, 9 * C, 9 * C, pair ? TBN / 2 : TBN))) return rc;
+    if ((rc = make_map_2d(&maps.w[0], Wh, C, 9 * C, 9 * C))) return rc;
+    if ((rc = make_map_2d(&maps.w[1], Wl, C, 9 * C, 9 * C))) return rc;
     if ((rc = ensure_tc_attrs())) return rc;
     TcParams p{bias, nullptr, out, (__half*)outh, (__half*)outl, 0, C, B * T2 * CONV_W2, C, 9 * C, MASR_EPI_BIAS_RELU, 1.f, T2, tc_flags()};
     const int tiles_n = (C + TBN - 1) / TBN, tiles_t = (T2 + CONV_TR - 1) / CONV_TR;
-    launch_tc<true>(maps, p, pair, tiles_n, tiles_t, B, (cudaStream_t)stream);
+    launch_tc<true>(maps, p, tiles_n, tiles_t, B, (cudaStream_t)stream);
     return check_launch("tc_gemm_kernel<conv>");
 }
 
@@ -1046,51 +752,13 @@ extern "C" int masr_gemm_tc_f16x2(const void* Ah, const void* Al, int64_t lda, c
     int rc;
     if ((rc = make_map_2d(&maps.a[0], Ah, M, K, lda))) return rc;
     if ((rc = make_map_2d(&maps.a[1], Al, M, K, lda))) return rc;
-    const bool pair = pair_enabled(M > TBM);
-    if ((rc = make_map_2d(&maps.w[0], Wh, N, K, K, pair ? TBN / 2 : TBN))) return rc;
-    if ((rc = make_map_2d(&maps.w[1], Wl, N, K, K, pair ? TBN / 2 : TBN))) return rc;
+    if ((rc = make_map_2d(&maps.w[0], Wh, N, K, K))) return rc;
+    if ((rc = make_map_2d(&maps.w[1], Wl, N, K, K))) return rc;
     if ((rc = ensure_tc_attrs())) return rc;
     TcParams p{bias, residual, C, (__half*)Ch, (__half*)Cl, ldr, ldc, M, N, K, epilogue, alpha, 0, tc_flags()};
     const int tiles_n = (N + TBN - 1) / TBN, tiles_m = (M + TBM - 1) / TBM;
-    launch_tc<false>(maps, p, pair, tiles_n, tiles_m, 1, (cudaStream_t)stream);
+    launch_tc<false>(maps, p, tiles_n, tiles_m, 1, (cudaStream_t)stream);
     return check_launch("tc_gemm_kernel");
-}
-
-// LayerNorm + Linear in one launch (K = D = 256): C / (Ch, Cl) = epilogue(LN(x; gamma, beta) . W^T + bias).
-//   encoder.py:122 -> attention.py:72-74 (norm_mha -> q/k/v), :141 -> convolution.py:117 (norm_conv -> pointwise_conv1 + GLU),
-//   :153 / :106 -> positionwise.py:37 (norm_ff / norm_ff_macaron -> w_1 + SiLU)
-// Every CTA (pair) takes a contiguous range of tiles, normalises the <= 2 row blocks that range touches into the operand
-// pair buffer (Ah, Al: [M, 256] fp16, written here, same values as masr_layernorm_split_f16) and then runs the GEMM on it.
-// Replaces masr_layernorm_split_f16 + masr_gemm_tc_f16x2: one launch and its fill / drain less per LayerNorm.
-extern "C" int masr_gemm_tc_lnpre_f16x2(const float* x, int64_t ldx, const float* gamma, const float* beta, float eps, void* Ah,
-                                        void* Al, int64_t lda, const void* Wh, const void* Wl, const float* bias, float* C,
-                                        void* Ch, void* Cl, int64_t ldc, int M, int N, int K, int epilogue, float alpha,
-                                        void* stream) {
-    if (M == 0 || N == 0) return MASR_OK;
-    MASR_REQUIRE(x && gamma && beta && Ah && Al && Wh && Wl, "masr_gemm_tc_lnpre_f16x2: null pointer");
-    MASR_REQUIRE(C || (Ch && Cl), "masr_gemm_tc_lnpre_f16x2: no output");
-    MASR_REQUIRE((Ch == nullptr) == (Cl == nullptr), "masr_gemm_tc_lnpre_f16x2: Ch/Cl must come as a pair");
-    MASR_REQUIRE(K == 256, "masr_gemm_tc_lnpre_f16x2: K=%d unsupported (the LayerNorm width of this build is 256)", K);
-    MASR_REQUIRE(lda % 8 == 0 && ldx % 4 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0,
-                 "masr_gemm_tc_lnpre_f16x2: lda=%lld ldx=%lld alignment", (long long)lda, (long long)ldx);
-    MASR_REQUIRE(epilogue >= MASR_EPI_BIAS && epilogue <= MASR_EPI_BIAS_SCALE, "masr_gemm_tc_lnpre_f16x2: bad epilogue %d", epilogue);
-    MASR_REQUIRE(epilogue != MASR_EPI_BIAS_GLU || N % 32 == 0, "masr_gemm_tc_lnpre_f16x2: GLU epilogue needs N %% 32 == 0");
-    MASR_REQUIRE(ldc % 8 == 0 || (C && !Ch && ldc % 4 == 0), "masr_gemm_tc_lnpre_f16x2: ldc=%lld alignment", (long long)ldc);
-    TcMaps maps;
-    memset(&maps, 0, sizeof(maps));
-    int rc;
-    const int tiles_n = (N + TBN - 1) / TBN, tiles_m = (M + TBM - 1) / TBM;
-    if ((rc = make_map_2d(&maps.a[0], Ah, M, K, lda))) return rc;
-    if ((rc = make_map_2d(&maps.a[1], Al, M, K, lda))) return rc;
-    const bool pair = pair_enabled(M > TBM);
-    if ((rc = make_map_2d(&maps.w[0], Wh, N, K, K, pair ? TBN / 2 : TBN))) return rc;
-    if ((rc = make_map_2d(&maps.w[1], Wl, N, K, K, pair ? TBN / 2 : TBN))) return rc;
-    if ((rc = ensure_tc_attrs())) return rc;
-    TcParams p{bias, nullptr, C, (__half*)Ch, (__half*)Cl, 0, ldc, M, N, K, epilogue, alpha, 0, tc_flags()};
-    p.ln_g = gamma; p.ln_b = beta; p.ln_eps = eps;
-    p.lnp_x = x; p.lnp_ldx = ldx; p.lnp_ld = lda; p.lnp_h = (__half*)Ah; p.lnp_l = (__half*)Al;
-    launch_tc<false>(maps, p, pair, tiles_n, tiles_m, 1, (cudaStream_t)stream);
-    return check_launch("tc_gemm_kernel<ln prologue>");
 }
 
 // ctc_lo Linear + softmax statistics + per-frame argmax (loss/ctc.py:70, ctc_greedy_decoder.py:21-27) without the [M, V]
@@ -1110,94 +778,17 @@ extern "C" int masr_ctc_head_argmax_tc_f16x2(const void* Ah, const void* Al, int
     int rc;
     if ((rc = make_map_2d(&maps.a[0], Ah, M, K, lda))) return rc;
     if ((rc = make_map_2d(&maps.a[1], Al, M, K, lda))) return rc;
-    const bool pair = pair_enabled(M > TBM);
-    if ((rc = make_map_2d(&maps.w[0], Wh, V, K, K, pair ? TBN / 2 : TBN))) return rc;
-    if ((rc = make_map_2d(&maps.w[1], Wl, V, K, K, pair ? TBN / 2 : TBN))) return rc;
+    if ((rc = make_map_2d(&maps.w[0], Wh, V, K, K))) return rc;
+    if ((rc = make_map_2d(&maps.w[1], Wl, V, K, K))) return rc;
     if ((rc = ensure_tc_attrs())) return rc;
     TcParams p{bias, nullptr, nullptr, nullptr, nullptr, 0, 0, M, V, K, EPI_CTC_PARTIAL, 1.f, 0, tc_flags()};
     p.part_m = (float*)workspace;
     p.part_s = p.part_m + (int64_t)groups * M;
     p.part_i = (int*)(p.part_s + (int64_t)groups * M);
     const int tiles_n = (V + TBN - 1) / TBN, tiles_m = (M + TBM - 1) / TBM;
-    launch_tc<false>(maps, p, pair, tiles_n, tiles_m, 1, (cudaStream_t)stream);
+    launch_tc<false>(maps, p, tiles_n, tiles_m, 1, (cudaStream_t)stream);
     if ((rc = check_launch("tc_gemm_kernel<ctc>"))) return rc;
     launch_pdl(ctc_partial_combine_kernel, dim3((M + 31) / 32), dim3(128), 0, (cudaStream_t)stream, (const float*)p.part_m,
                (const float*)p.part_s, (const int*)p.part_i, M, groups, ids, maxp);
     return check_launch("ctc_partial_combine_kernel");
-}
-
-// Sub-layer output projection (N = 256) + residual add + the LayerNorm(s) that follow it, in one kernel:
-//   x_new = residual + alpha * (A.W^T + bias)
-//   gamma2 == NULL:  X <- x_new,  (Yh, Yl) <- LN(x_new; gamma1, beta1)            encoder.py:117->122, 131->141, 145->153
-//   gamma2 != NULL:  X <- LN(x_new; gamma1, beta1),  (Yh, Yl) <- LN(X; gamma2, beta2)   encoder.py:155->161->(next block) 106 / 342
-//   Y2 (optional): fp32 copy of what the pair holds.
-// Launched as clusters of 2 CTAs (the two 128-column tiles of a row block); row statistics cross the pair through
-// distributed shared memory.  Replaces masr_gemm_tc_f16x2(MASR_EPI_RESIDUAL) + masr_layernorm[2]_split_f16.
-static int launch_residual_ln(const void* Ah, const void* Al, int64_t lda, const void* Wh, const void* Wl, const float* bias,
-                              const float* residual, int64_t ldr, float alpha, float* X, const float* gamma1, const float* beta1,
-                              const float* gamma2, const float* beta2, float* Y2, void* Yh, void* Yl, int64_t ldx, int M, int N,
-                              int K, float eps, int epi_override, const float* ada_s, const float* ada_b, void* stream);
-
-extern "C" int masr_gemm_tc_residual_ln_f16x2(const void* Ah, const void* Al, int64_t lda, const void* Wh, const void* Wl,
-                                              const float* bias, const float* residual, int64_t ldr, float alpha, float* X,
-                                              const float* gamma1, const float* beta1, const float* gamma2, const float* beta2,
-                                              float* Y2, void* Yh, void* Yl, int64_t ldx, int M, int N, int K, float eps,
-                                              void* stream) {
-    return launch_residual_ln(Ah, Al, lda, Wh, Wl, bias, residual, ldr, alpha, X, gamma1, beta1, gamma2, beta2, Y2, Yh, Yl, ldx, M, N,
-                              K, eps, 0, nullptr, nullptr, stream);
-}
-
-// Post-norm form (Squeezeformer blocks, squeezeformer/encoder.py:412-463): X <- LN(residual + alpha * (A.W^T + bias); gamma, beta)
-// becomes the stream, (Yh, Yl) <- ada_scale * X + ada_bias (the next sub-module's adaptive scale; NULL: the pair of X itself).
-// Same kernel and restrictions as masr_gemm_tc_residual_ln_f16x2; replaces masr_gemm_tc_f16x2(RESIDUAL) + masr_layernorm_ada_split_f16.
-extern "C" int masr_gemm_tc_residual_postln_f16x2(const void* Ah, const void* Al, int64_t lda, const void* Wh, const void* Wl,
-                                                  const float* bias, const float* residual, int64_t ldr, float alpha, float* X,
-                                                  const float* gamma, const float* beta, const float* ada_scale,
-                                                  const float* ada_bias, void* Yh, void* Yl, int64_t ldx, int M, int N, int K,
-                                                  float eps, void* stream) {
-    MASR_REQUIRE((ada_scale == nullptr) == (ada_bias == nullptr), "masr_gemm_tc_residual_postln_f16x2: ada_scale/ada_bias must come as a pair");
-    return launch_residual_ln(Ah, Al, lda, Wh, Wl, bias, residual, ldr, alpha, X, gamma, beta, nullptr, nullptr, nullptr, Yh, Yl, ldx, M,
-                              N, K, eps, EPI_RESIDUAL_POSTLN, ada_scale, ada_bias, stream);
-}
-
-static int launch_residual_ln(const void* Ah, const void* Al, int64_t lda, const void* Wh, const void* Wl, const float* bias,
-                              const float* residual, int64_t ldr, float alpha, float* X, const float* gamma1, const float* beta1,
-                              const float* gamma2, const float* beta2, float* Y2, void* Yh, void* Yl, int64_t ldx, int M, int N,
-                              int K, float eps, int epi_override, const float* ada_s, const float* ada_b, void* stream) {
-    if (M == 0) return MASR_OK;
-    MASR_REQUIRE(Ah && Al && Wh && Wl && residual && X && gamma1 && beta1 && Yh && Yl, "masr_gemm_tc_residual_ln_f16x2: null pointer");
-    MASR_REQUIRE((gamma2 == nullptr) == (beta2 == nullptr), "masr_gemm_tc_residual_ln_f16x2: gamma2/beta2 must come as a pair");
-    MASR_REQUIRE(N == 2 * TBN, "masr_gemm_tc_residual_ln_f16x2: N=%d unsupported (this build: %d)", N, 2 * TBN);
-    MASR_REQUIRE(K > 0 && K % TBK == 0 && lda % 8 == 0 && ldx % 8 == 0 && ldr % 4 == 0, "masr_gemm_tc_residual_ln_f16x2: K=%d lda=%lld ldx=%lld ldr=%lld",
-                 K, (long long)lda, (long long)ldx, (long long)ldr);
-    TcMaps maps;
-    memset(&maps, 0, sizeof(maps));
-    int rc;
-    if ((rc = make_map_2d(&maps.a[0], Ah, M, K, lda))) return rc;
-    if ((rc = make_map_2d(&maps.a[1], Al, M, K, lda))) return rc;
-    if ((rc = make_map_2d(&maps.w[0], Wh, N, K, K))) return rc;
-    if ((rc = make_map_2d(&maps.w[1], Wl, N, K, K))) return rc;
-    if ((rc = ensure_tc_attrs())) return rc;
-    TcParams p{bias, residual, X, (__half*)Yh, (__half*)Yl, ldr, ldx, M, N, K,
-               epi_override ? epi_override : (gamma2 ? EPI_RESIDUAL_LN2 : EPI_RESIDUAL_LN), alpha, 0, tc_flags() & ~2};
-    p.ln_g = gamma1; p.ln_b = beta1; p.ln_g2 = gamma2; p.ln_b2 = beta2; p.y2 = Y2; p.ln_eps = eps;
-    p.ada_s = ada_s; p.ada_b = ada_b;
-    const int tiles_m = (M + TBM - 1) / TBM;
-    const int num_tiles = 2 * tiles_m;
-    const int sms = num_sms() & ~1;
-    const int grid = num_tiles < sms ? num_tiles : sms;             // even: a cluster = the two column tiles of one row block
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(TC_THREADS);
-    cfg.dynamicSmemBytes = kTcSmemLn;
-    cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    cudaLaunchKernelEx(&cfg, tc_gemm_kernel<false, true>, maps, p, num_tiles, 2, 1);
-    return check_launch("tc_gemm_kernel<ln>");
 }

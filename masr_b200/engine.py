@@ -71,17 +71,11 @@ class ConformerEngine:
         if gemm not in ("tc", "simt"):
             raise ValueError("gemm must be 'tc' or 'simt'")
         self.gemm_path = gemm
-        # fused epilogues of the tensor-core path.  CTC head (softmax partials + argmax in the GEMM epilogue, no [M,V] logits):
-        # on (MASR_FUSE_CTC=0 for A/B runs).  LayerNorm behind the residual projections (cluster of 2 CTAs + DSMEM): with one
-        # tile per CTA the longer epilogue is fully exposed instead of overlapping the next tile's mainloop; off unless
-        # MASR_FUSE_LN=1 (not measured faster on the H100).
+        # fused CTC head of the tensor-core path (softmax partials + argmax in the GEMM epilogue, no [M,V] logits):
+        # on (MASR_FUSE_CTC=0 for A/B runs)
         self.fuse_ctc = os.environ.get("MASR_FUSE_CTC", "1") != "0"
         # attention of utterances up to 256 frames on wgmma (csrc/attention_tc5.cu); MASR_ATTN=mma keeps the mma.sync kernel
         self.attn_tc5 = os.environ.get("MASR_ATTN", "tc5") != "mma"
-        self.fuse = os.environ.get("MASR_FUSE_LN", "0") == "1"
-        # LayerNorm as a PROLOGUE of the GEMM that consumes it (masr_gemm_tc_lnpre_f16x2: norm_mha -> qkv, norm_conv -> pw1,
-        # norm_ff -> w_1): 37 launches fewer per step, results bit-identical.  MASR_FUSE_LNPRE=0/1.
-        self.lnpre = os.environ.get("MASR_FUSE_LNPRE", "0") == "1"
         self.use_graphs = bool(use_graphs)     # replay the batched device step as one CUDA graph per (B, Fmax) shape
         self._graphs = {}
         if not torch.cuda.is_available():
@@ -171,26 +165,9 @@ class ConformerEngine:
         self._k(tag, "masr_gemm_tc_f16x2", _p(A[0]), _p(A[1]), lda, _p(W[0]), _p(W[1]), _p(bias), _p(residual), ldr,
                 _p(C), None if Cp is None else _p(Cp[0]), None if Cp is None else _p(Cp[1]), ldc, M, N, K, epi, alpha)
 
-    def _tc_ln(self, A, lda, W, bias, M, K, alpha, x, ln1, yp, ln2=None, y2=None, tag="gemm"):
-        """x <- x + alpha * (A.W^T + bias) followed by the LayerNorm(s) of the next consumer, one kernel
-        (masr_gemm_tc_residual_ln_f16x2): ln2 is None -> x keeps the sum and yp <- LN1(x); else x <- LN1(sum), yp <- LN2(x)."""
-        d = self.d
-        self._k(tag, "masr_gemm_tc_residual_ln_f16x2", _p(A[0]), _p(A[1]), lda, _p(W[0]), _p(W[1]), _p(bias), _p(x), d, alpha,
-                _p(x), _p(ln1[0]), _p(ln1[1]), None if ln2 is None else _p(ln2[0]), None if ln2 is None else _p(ln2[1]),
-                _p(y2), _p(yp[0]), _p(yp[1]), d, M, d, K, 1e-5)
-
-    def _tc_postln(self, A, lda, W, bias, M, K, x, ln, ada, yp, alpha=1.0, tag="gemm"):
-        """Post-norm blocks (Squeezeformer): x <- LN(x + alpha * (A.W^T + bias)); yp <- ada_scale * x + ada_bias (or pair(x)),
-        one kernel (masr_gemm_tc_residual_postln_f16x2)."""
-        d = self.d
-        self._k(tag, "masr_gemm_tc_residual_postln_f16x2", _p(A[0]), _p(A[1]), lda, _p(W[0]), _p(W[1]), _p(bias), _p(x), d, alpha,
-                _p(x), _p(ln[0]), _p(ln[1]), None if ada is None else _p(ada[0]), None if ada is None else _p(ada[1]),
-                _p(yp[0]), _p(yp[1]), d, M, d, K, 1e-5)
-
     def _ffn_fused(self) -> bool:
-        """The Conformer FFN modules run as one masr_ffn_tc_f16x2 launch each (shape permitting) unless MASR_FUSE_LN=1,
-        whose w_2 launch carries the following LayerNorm(s) instead."""
-        return self.gemm_path == "tc" and not self.fuse and self.d == 256 and self.w.ffn % 256 == 0
+        """The Conformer FFN modules run as one masr_ffn_tc_f16x2 launch each (shape permitting)."""
+        return self.gemm_path == "tc" and self.d == 256 and self.w.ffn % 256 == 0
 
     def _ffn_tc(self, A, W1, b1, W2, b2, M, x, alpha=0.5):
         """x <- x + alpha * (SiLU(A.W1^T + b1) . W2^T + b2) in one launch (masr_ffn_tc_f16x2), A the LayerNorm-ed pair; the
@@ -251,18 +228,6 @@ class ConformerEngine:
             best = min(best, e0.elapsed_time(e1))
         self.launches, self.prof = n0, prof
         return best / (2 * reps)           # fused: reps launches, each counted as a w_1 + w_2 pair
-
-    def _ln_tc(self, x, gb, yp, W, bias, M, N, epi=EPI_BIAS, C=None, Cp=None, ldc=0, tag="gemm"):
-        """C / Cp = epi(LN(x; gb) . W^T + bias) with yp as the operand pair: one launch (masr_gemm_tc_lnpre_f16x2: every CTA
-        normalises the rows of its own tiles first) when `self.lnpre`, else LayerNorm launch + GEMM launch.  Same results."""
-        d = self.d
-        if self.lnpre and d == 256:
-            self._k(tag, "masr_gemm_tc_lnpre_f16x2", _p(x), d, _p(gb[0]), _p(gb[1]), 1e-5, _p(yp[0]), _p(yp[1]), d, _p(W[0]),
-                    _p(W[1]), _p(bias), _p(C), None if Cp is None else _p(Cp[0]), None if Cp is None else _p(Cp[1]), ldc, M, N, d,
-                    epi, 1.0)
-            return
-        self._ln_split(x, gb, yp, M)
-        self._tc(yp, d, W, bias, M, N, d, epi, C=C, Cp=Cp, ldc=ldc, tag=tag)
 
     def _ln_split(self, x, gb, yp, M):
         """yp <- pair(LN(x; gb)).  d = 256: one launch.  d = 512: masr_layernorm_split_f16 has no 512-wide form, so the row goes
@@ -562,59 +527,35 @@ class ConformerEngine:
         lpad = (w.kernel - 1) if self.causal else (w.kernel - 1) // 2
         nl = len(w.layers)
         for i, L in enumerate(w.layers):
-            fuse = self.fuse and d == 256
+            if i == 0:                                # later blocks: t0p is written by the previous block's norm_final (below)
+                self._ln_split(x, L.ln_ffm, t0p, M)
             if ffn_fused:
-                if i == 0:                            # later blocks: t0p is written by the previous block's norm_final (below)
-                    self._ln_split(x, L.ln_ffm, t0p, M)
                 self._ffn_tc(t0p, tw[i, "ffm1"], L.ffm[1], tw[i, "ffm2"], L.ffm[3], M, x)
-            elif i == 0:                              # later blocks: fused with the previous block's norm_final (below)
-                self._ln_tc(x, L.ln_ffm, t0p, tw[i, "ffm1"], L.ffm[1], M, w.ffn, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn, tag="ffn_w1")
             else:
                 self._tc(t0p, d, tw[i, "ffm1"], L.ffm[1], M, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn, tag="ffn_w1")
-            # every sub-layer's output projection adds into the residual stream AND writes the next sub-layer's LayerNorm-ed
-            # operand pair in its epilogue (masr_gemm_tc_residual_ln_f16x2); MASR_FUSE=0: separate LayerNorm launches
-            if fuse:
-                self._tc_ln(hidp, w.ffn, tw[i, "ffm2"], L.ffm[3], M, w.ffn, 0.5, x, L.ln_mha, t0p, tag="ffn_w2")
-            elif not ffn_fused:
                 self._tc(hidp, w.ffn, tw[i, "ffm2"], L.ffm[3], M, d, w.ffn, EPI_RESIDUAL, 0.5, x, d, C=x, ldc=d, tag="ffn_w2")
-            if fuse:
-                self._tc(t0p, d, tw[i, "qkv"], L.bqkv, M, 3 * d, d, C=qkv, Cp=ws["qkvp"], ldc=3 * d, tag="qkv_proj")
-            else:
-                self._ln_tc(x, L.ln_mha, t0p, tw[i, "qkv"], L.bqkv, M, 3 * d, C=qkv, Cp=ws["qkvp"], ldc=3 * d, tag="qkv_proj")
+            self._ln_split(x, L.ln_mha, t0p, M)
+            self._tc(t0p, d, tw[i, "qkv"], L.bqkv, M, 3 * d, d, C=qkv, Cp=ws["qkvp"], ldc=3 * d, tag="qkv_proj")
             self._attention_tc(L, qkv, ws["qkvp"], t1p, T, tlens, B)
-            if fuse:
-                self._tc_ln(t1p, d, tw[i, "wo"], L.bo, M, d, 1.0, x, L.ln_conv, t0p, tag="out_proj")
-            else:
-                self._tc(t1p, d, tw[i, "wo"], L.bo, M, d, d, EPI_RESIDUAL, 1.0, x, d, C=x, ldc=d, tag="out_proj")
-            if fuse:
-                self._tc(t0p, d, tw[i, "pw1"], L.pw1_b, M, 2 * d, d, EPI_BIAS_GLU, C=g, ldc=d, tag="pw1_glu")
-            else:
-                self._ln_tc(x, L.ln_conv, t0p, tw[i, "pw1"], L.pw1_b, M, 2 * d, EPI_BIAS_GLU, C=g, ldc=d, tag="pw1_glu")
+            self._tc(t1p, d, tw[i, "wo"], L.bo, M, d, d, EPI_RESIDUAL, 1.0, x, d, C=x, ldc=d, tag="out_proj")
+            self._ln_split(x, L.ln_conv, t0p, M)
+            self._tc(t0p, d, tw[i, "pw1"], L.pw1_b, M, 2 * d, d, EPI_BIAS_GLU, C=g, ldc=d, tag="pw1_glu")
             self._k("dwconv_ln_silu", "masr_dwconv_ln_silu_f32", _p(g), d, T, _p(L.dw), _p(L.dw_b), _p(L.cn[0]),
                     _p(L.cn[1]), _p(L.glu_pad) if self.causal else None, None, _p(t1p[0]), _p(t1p[1]), d, T, _p(tlens), B,
                     d, w.kernel, lpad, T, 1e-5)
-            if fuse:
-                self._tc_ln(t1p, d, tw[i, "pw2"], L.pw2_b, M, d, 1.0, x, L.ln_ff, t0p, tag="pw2")
-            else:
-                self._tc(t1p, d, tw[i, "pw2"], L.pw2_b, M, d, d, EPI_RESIDUAL, 1.0, x, d, C=x, ldc=d, tag="pw2")
-            if fuse:
-                self._tc(t0p, d, tw[i, "ff1"], L.ff[1], M, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn, tag="ffn_w1")
-            elif ffn_fused:
-                self._ln_split(x, L.ln_ff, t0p, M)
+            self._tc(t1p, d, tw[i, "pw2"], L.pw2_b, M, d, d, EPI_RESIDUAL, 1.0, x, d, C=x, ldc=d, tag="pw2")
+            self._ln_split(x, L.ln_ff, t0p, M)
+            if ffn_fused:
                 self._ffn_tc(t0p, tw[i, "ff1"], L.ff[1], tw[i, "ff2"], L.ff[3], M, x)
             else:
-                self._ln_tc(x, L.ln_ff, t0p, tw[i, "ff1"], L.ff[1], M, w.ffn, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn, tag="ffn_w1")
+                self._tc(t0p, d, tw[i, "ff1"], L.ff[1], M, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn, tag="ffn_w1")
+                self._tc(hidp, w.ffn, tw[i, "ff2"], L.ff[3], M, d, w.ffn, EPI_RESIDUAL, 0.5, x, d, C=x, ldc=d, tag="ffn_w2")
             # x = norm_final(x + 0.5 ffn), then in the same pass the next consumer's LayerNorm: the next block's
             # norm_ff_macaron (pair only) or, after the last block, after_norm (fp32 encoder output + the CTC head's pair)
             nxt = w.layers[i + 1].ln_ffm if i + 1 < nl else w.after_norm
             y2 = None if i + 1 < nl else ws["t0"]
-            if fuse:
-                self._tc_ln(hidp, w.ffn, tw[i, "ff2"], L.ff[3], M, w.ffn, 0.5, x, L.ln_final, t0p, ln2=nxt, y2=y2, tag="ffn_w2")
-            else:
-                if not ffn_fused:
-                    self._tc(hidp, w.ffn, tw[i, "ff2"], L.ff[3], M, d, w.ffn, EPI_RESIDUAL, 0.5, x, d, C=x, ldc=d, tag="ffn_w2")
-                self._k("layernorm", "masr_layernorm2_split_f16", _p(x), d, _p(L.ln_final[0]), _p(L.ln_final[1]), _p(x), _p(nxt[0]),
-                        _p(nxt[1]), _p(y2), _p(t0p[0]), _p(t0p[1]), d, M, d, 1e-5)
+            self._k("layernorm", "masr_layernorm2_split_f16", _p(x), d, _p(L.ln_final[0]), _p(L.ln_final[1]), _p(x), _p(nxt[0]),
+                    _p(nxt[1]), _p(y2), _p(t0p[0]), _p(t0p[1]), d, M, d, 1e-5)
         return ws["t0"][:M], tl, T, ws
 
     # ---- CTC head ----------------------------------------------------------------------------

@@ -55,11 +55,6 @@ class _PoolBase:
         self.feats_in = torch.zeros(n_slots, CHUNK_FRAMES, 80, device=dev, dtype=torch.float32)
         self.lens_host = [0] * n_slots
         self.use_graph = bool(use_graph) and eng.use_graphs
-        # LayerNorm folded into the preceding residual projection (cluster kernel, 4 launches per block fewer): at M = 1024 the
-        # cluster launch + DSMEM exchange replace only a short LayerNorm launch.  Off unless MASR_POOL_FUSE_LN=1 (tests cover
-        # both; not measured faster on the H100).
-        import os
-        self.fuse_ln = os.environ.get("MASR_POOL_FUSE_LN", "0") == "1" and eng.d == 256
         self.beam = None              # PoolBeam: the prefix beam search runs after every step (captured with it)
         self._graph = None
         self._graph_launches = 0
@@ -217,16 +212,11 @@ class ConformerStreamPool(_PoolBase):
                None, _p(b["c2p"][0]), _p(b["c2p"][1]), S, F1, C, d)
         eng._tc(b["c2p"], eng.f2 * d, tw["embed"], w.embed_b, M, d, eng.f2 * d, EPI_BIAS_SCALE, float(d) ** 0.5, C=x, ldc=d)
         LC = self.lorder + C
-        fz, nl = self.fuse_ln, len(w.layers)
         for i, L in enumerate(w.layers):
-            if not fz or i == 0:
-                eng._ln_split(x, L.ln_ffm, t0p, M)
+            eng._ln_split(x, L.ln_ffm, t0p, M)
             eng._tc(t0p, d, tw[i, "ffm1"], L.ffm[1], M, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn)
-            if fz:
-                eng._tc_ln(hidp, w.ffn, tw[i, "ffm2"], L.ffm[3], M, w.ffn, 0.5, x, L.ln_mha, t0p)
-            else:
-                eng._tc(hidp, w.ffn, tw[i, "ffm2"], L.ffm[3], M, d, w.ffn, EPI_RESIDUAL, 0.5, x, d, C=x, ldc=d)
-                eng._ln_split(x, L.ln_mha, t0p, M)
+            eng._tc(hidp, w.ffn, tw[i, "ffm2"], L.ffm[3], M, d, w.ffn, EPI_RESIDUAL, 0.5, x, d, C=x, ldc=d)
+            eng._ln_split(x, L.ln_mha, t0p, M)
             eng._tc(t0p, d, tw[i, "qkv"], L.bqkv, M, 3 * d, d, C=qkv, Cp=qkvp, ldc=3 * d)
             kvh, kvl = self.kv[i]
             self._append_pair(qkvp, 3 * d, d, 2 * d, (kvh, kvl), cap, self.BASE, self.QLEN, C)      # new K|V rows -> caches
@@ -235,11 +225,8 @@ class ConformerStreamPool(_PoolBase):
                    kvl.data_ptr() + 2 * d, 2 * d, cap, _p(ph), _p(pl), d, _p(L.pos_u), _p(L.pos_v), None, _p(t1p[0]), _p(t1p[1]), d, C,
                    qlen, klen, S, eng.h, eng.dk, C)
             # conv module over [cache ++ chunk] per slot (convolution.py:101-109): t0 <- norm_conv(x + out_proj(att))
-            if fz:
-                eng._tc_ln(t1p, d, tw[i, "wo"], L.bo, M, d, 1.0, x, L.ln_conv, t0p, y2=t0)
-            else:
-                eng._tc(t1p, d, tw[i, "wo"], L.bo, M, d, d, EPI_RESIDUAL, 1.0, x, d, C=x, ldc=d)
-                eng._ln(x, L.ln_conv, t0, M)
+            eng._tc(t1p, d, tw[i, "wo"], L.bo, M, d, d, EPI_RESIDUAL, 1.0, x, d, C=x, ldc=d)
+            eng._ln(x, L.ln_conv, t0, M)
             xc = self.xcat[i]                                   # [S, 14+16, d]
             xc[:, self.lorder:].copy_(t0.view(S, C, d))
             eng._k("affine_split", "masr_affine_split_f16", _p(xc), None, None, _p(xcp[0]), _p(xcp[1]), S * LC, d)
@@ -248,20 +235,12 @@ class ConformerStreamPool(_PoolBase):
                    _p(t1p[0]), _p(t1p[1]), d, C, _p(b["clen"]), S, d, w.kernel, 0, C, 1e-5)
             # new left context = the last `lorder` VALID rows: rows [n, n+lorder) of [cache ++ chunk], n = valid chunk rows
             self._shift(xc, None, LC, self.lorder, d * 4, self.QLEN)
-            if fz:
-                eng._tc_ln(t1p, d, tw[i, "pw2"], L.pw2_b, M, d, 1.0, x, L.ln_ff, t0p)
-            else:
-                eng._tc(t1p, d, tw[i, "pw2"], L.pw2_b, M, d, d, EPI_RESIDUAL, 1.0, x, d, C=x, ldc=d)
-                eng._ln_split(x, L.ln_ff, t0p, M)
+            eng._tc(t1p, d, tw[i, "pw2"], L.pw2_b, M, d, d, EPI_RESIDUAL, 1.0, x, d, C=x, ldc=d)
+            eng._ln_split(x, L.ln_ff, t0p, M)
             eng._tc(t0p, d, tw[i, "ff1"], L.ff[1], M, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn)
-            if fz:      # x <- norm_final(x + 0.5 ffn), t0p <- the next block's norm_ff_macaron (or after_norm) of it
-                eng._tc_ln(hidp, w.ffn, tw[i, "ff2"], L.ff[3], M, w.ffn, 0.5, x, L.ln_final, t0p,
-                           ln2=w.layers[i + 1].ln_ffm if i + 1 < nl else w.after_norm)
-            else:
-                eng._tc(hidp, w.ffn, tw[i, "ff2"], L.ff[3], M, d, w.ffn, EPI_RESIDUAL, 0.5, x, d, C=x, ldc=d)
-                eng._ln(x, L.ln_final, x, M)
-        if not fz:
-            eng._ln_split(x, w.after_norm, t0p, M)
+            eng._tc(hidp, w.ffn, tw[i, "ff2"], L.ff[3], M, d, w.ffn, EPI_RESIDUAL, 0.5, x, d, C=x, ldc=d)
+            eng._ln(x, L.ln_final, x, M)
+        eng._ln_split(x, w.after_norm, t0p, M)
         eng._tc(t0p, d, tw["ctc"], w.ctc_b, M, eng.V, d, C=b["logits"], ldc=eng.Vpad)
         eng._k("ctc_argmax", "masr_ctc_frame_argmax_f32", _p(b["logits"]), eng.Vpad, M, eng.V, _p(b["ids"]), _p(b["maxp"]), _p(self.probs), eng.V)
 
@@ -366,17 +345,11 @@ class SqueezeformerStreamPool(_PoolBase):
             eng._k("attention", "masr_relpos_attention_tc", _p(qkv), 3 * d, Ci, kvh.data_ptr(), kvl.data_ptr(), kvh.data_ptr() + 2 * d,
                    kvl.data_ptr() + 2 * d, 2 * d, cap, _p(ph), _p(pl), d, _p(L.pos_u), _p(L.pos_v), None, _p(t1p[0]), _p(t1p[1]), d, Ci,
                    self._m(rq), self._m(rk), S, eng.h, eng.dk, Ci)
-            if self.fuse_ln:
-                eng._tc_postln(t1p, d, tw[i, "wo"], L.bo, Mi, d, x, L.ln1, L.ffn1_ada, t0p)
-            else:
-                eng._tc(t1p, d, tw[i, "wo"], L.bo, Mi, d, d, EPI_RESIDUAL, 1.0, x, d, C=y, ldc=d)
-                eng._ln_ada(y, L.ln1, x, L.ffn1_ada, t0p, Mi)
+            eng._tc(t1p, d, tw[i, "wo"], L.bo, Mi, d, d, EPI_RESIDUAL, 1.0, x, d, C=y, ldc=d)
+            eng._ln_ada(y, L.ln1, x, L.ffn1_ada, t0p, Mi)
             eng._tc(t0p, d, tw[i, "f1a"], L.ffn1[1], Mi, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn)
-            if self.fuse_ln:
-                eng._tc_postln(hidp, w.ffn, tw[i, "f1b"], L.ffn1[3], Mi, w.ffn, x, L.ln2, L.conv_ada, t0p)
-            else:
-                eng._tc(hidp, w.ffn, tw[i, "f1b"], L.ffn1[3], Mi, d, w.ffn, EPI_RESIDUAL, 1.0, x, d, C=y, ldc=d)
-                eng._ln_ada(y, L.ln2, x, L.conv_ada, t0p, Mi)
+            eng._tc(hidp, w.ffn, tw[i, "f1b"], L.ffn1[3], Mi, d, w.ffn, EPI_RESIDUAL, 1.0, x, d, C=y, ldc=d)
+            eng._ln_ada(y, L.ln2, x, L.conv_ada, t0p, Mi)
             # conv module over [cache ++ chunk] per slot
             xh, xl = self.xcat[i]
             xh[:, self.lorder:].copy_(t0p[0][:Mi].view(S, Ci, d))
@@ -386,18 +359,12 @@ class SqueezeformerStreamPool(_PoolBase):
                    None, _p(t1p[0]), _p(t1p[1]), d, Ci, _p(clen), S, d, L.kernel, 0, Ci)
             # new left context = the last `lorder` VALID rows: rows [n, n + lorder) of [cache ++ chunk], n = valid chunk rows
             self._shift(xh, xl, LCi, self.lorder, d * 2, rq)
-            if self.fuse_ln:
-                eng._tc_postln(t1p, d, tw[i, "pw2"], L.pw2_b, Mi, d, x, L.ln3, L.ffn2_ada, t0p)
-            else:
-                eng._tc(t1p, d, tw[i, "pw2"], L.pw2_b, Mi, d, d, EPI_RESIDUAL, 1.0, x, d, C=y, ldc=d)
-                eng._ln_ada(y, L.ln3, x, L.ffn2_ada, t0p, Mi)
+            eng._tc(t1p, d, tw[i, "pw2"], L.pw2_b, Mi, d, d, EPI_RESIDUAL, 1.0, x, d, C=y, ldc=d)
+            eng._ln_ada(y, L.ln3, x, L.ffn2_ada, t0p, Mi)
             eng._tc(t0p, d, tw[i, "f2a"], L.ffn2[1], Mi, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn)
             nxt = w.layers[i + 1].att_ada if (i + 1 < nl and i + 1 not in (eng.REDUCE, eng.RECOVER)) else None
-            if self.fuse_ln:                            # (last block: pair(x) feeds the CTC head)
-                eng._tc_postln(hidp, w.ffn, tw[i, "f2b"], L.ffn2[3], Mi, w.ffn, x, L.ln4, nxt, t0p)
-            else:
-                eng._tc(hidp, w.ffn, tw[i, "f2b"], L.ffn2[3], Mi, d, w.ffn, EPI_RESIDUAL, 1.0, x, d, C=y, ldc=d)
-                eng._ln_ada(y, L.ln4, x, nxt, t0p, Mi)
+            eng._tc(hidp, w.ffn, tw[i, "f2b"], L.ffn2[3], Mi, d, w.ffn, EPI_RESIDUAL, 1.0, x, d, C=y, ldc=d)
+            eng._ln_ada(y, L.ln4, x, nxt, t0p, Mi)           # (last block: pair(x) feeds the CTC head)
         eng._tc(t0p, d, tw["ctc"], w.ctc_b, M, eng.V, d, C=b["logits"], ldc=eng.Vpad)
         eng._k("ctc_argmax", "masr_ctc_frame_argmax_f32", _p(b["logits"]), eng.Vpad, M, eng.V, _p(b["ids"]), _p(b["maxp"]), _p(self.probs), eng.V)
 

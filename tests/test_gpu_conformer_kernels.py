@@ -2,7 +2,7 @@
 float64 CPU references:
 
   relpos attention     masr/model_utils/conformer/attention.py:107-118,230-251  (_f32, the mma.sync _tc, the wgmma _tc5)
-  tensor-core GEMMs    torch.nn.functional.linear + every epilogue, LayerNorm prologue, residual + LayerNorm(s) epilogues
+  tensor-core GEMMs    torch.nn.functional.linear + every epilogue
   CTC head             loss/ctc.py:70 softmax + ctc_greedy_decoder.py:21 first argmax, without the [M, V] logits
   conv subsampling     subsampling.py:81-84 (conv1 into parity planes, conv2 as an implicit GEMM)
 
@@ -282,140 +282,6 @@ def test_tc_gemm_epilogues_float64(rt, M, N, K):
         assert torch.equal(Rd.cpu(), R)
     report(f"tc_gemm M={M} N={N} K={K}", **{f"epi{k}": v for k, v in res.items()})
     assert max(res.values()) < GEMM_RATIO_TOL, res
-
-
-def _ln64(x, ga, be):
-    return F.layer_norm(x.double(), (x.shape[1],), ga.double(), be.double(), 1e-5)
-
-
-@pytest.mark.parametrize("M,N", [(1, 264), (65, 120), (129, 768), (7937, 264)])
-def test_tc_gemm_lnpre_float64(rt, M, N):
-    """masr_gemm_tc_lnpre_f16x2 (LayerNorm prologue + GEMM), epilogues BIAS .. BIAS_SCALE (GLU where N % 32 == 0), against
-    float64 LN + linear.  The [M, 256] scratch pair it leaves behind holds LN(x); its rows past M and columns past 256 (row
-    pitch 264), and everything of C / Ch / Cl outside [M, N], stay NaN; x rows past M hold garbage.
-    Observed max error (H100): LN pair 1.0e-6, outputs 3.5e-6; tolerance 4e-6 / 1.2e-5."""
-    K, ldx, lda = 256, 264, 264
-    g = torch.Generator().manual_seed(M + N)
-    x = garbage((M + 3, ldx), M)
-    x[:M, :K] = torch.randn(M, K, generator=g) * 3 + 0.5
-    ga, be = 1 + 0.1 * torch.randn(K, generator=g), 0.1 * torch.randn(K, generator=g)
-    ln = _ln64(x[:M, :K], ga, be)
-    xd, gd, bed = x.to(rt.dev), ga.to(rt.dev), be.to(rt.dev)
-    errs = {}
-    for epi in (0, 1, 2, 3, 4):
-        if epi == 3 and N % 32:
-            continue
-        No = N // 2 if epi == 3 else N
-        W = torch.randn(N, K, generator=g) / math.sqrt(K)
-        b = torch.randn(N, generator=g)
-        Wh, Wl = split(rt, W.to(rt.dev))
-        bd = b.to(rt.dev)
-        ldc = rup(No, 8) + 8
-        Ah, Al = nan((M + 3, lda), rt.dev, torch.float16), nan((M + 3, lda), rt.dev, torch.float16)
-        C = nan((M + 3, ldc), rt.dev)
-        Ch, Cl = nan((M + 3, ldc), rt.dev, torch.float16), nan((M + 3, ldc), rt.dev, torch.float16)
-        rt.call("masr_gemm_tc_lnpre_f16x2", P(xd), ldx, P(gd), P(bed), 1e-5, P(Ah), P(Al), lda, P(Wh), P(Wl), P(bd), P(C), P(Ch), P(Cl),
-                ldc, M, N, K, epi, 0.5, rt.st())
-        torch.cuda.synchronize()
-        y = ln @ W.double().t() + b.double()
-        ref = {0: y, 1: F.silu(y), 2: F.relu(y), 3: y[:, 0::2] * torch.sigmoid(y[:, 1::2]), 4: 0.5 * y}[epi]
-        C, Ch, Cl = C.cpu(), Ch.cpu(), Cl.cpu()
-        errs[f"epi{epi}"] = err(C[:M, :No], ref)
-        errs["ln"] = err(pair_value(Ah[:M, :K], Al[:M, :K]), ln)
-        assert_pair_reconstructs(Ch[:M, :No], Cl[:M, :No], C[:M, :No])
-        mask = outside(C.shape, M, No)
-        assert all_nan(C, mask) and all_nan(Ch, mask) and all_nan(Cl, mask), f"epilogue {epi} wrote outside [M, N]"
-        amask = outside(Ah.shape, M, K)
-        assert all_nan(Ah, amask) and all_nan(Al, amask), "scratch pair written outside [M, 256]"
-    report(f"tc_gemm_lnpre M={M} N={N}", **errs)
-    assert errs.pop("ln") < 4e-6
-    assert max(errs.values()) < 1.2e-5
-
-
-@pytest.mark.parametrize("M,K,ln2,y2,alias", [(1, 320, False, False, False), (77, 256, True, False, False),
-                                              (129, 2304, True, True, False), (300, 256, False, True, True),
-                                              (7937, 256, False, False, True), (7937, 256, True, False, False)])
-def test_tc_gemm_residual_ln_float64(rt, M, K, ln2, y2, alias):
-    """masr_gemm_tc_residual_ln_f16x2 against float64: Y2 = NULL (the engine's usual call) with and without gamma2; the
-    residual either aliased to X or in its own buffer with ldr = 260 != ldx = 264 (then left untouched); ragged M.  X, Y2,
-    Yh, Yl keep their rows past M and columns past 256 (NaN, or X's own garbage when it is the residual).
-    Observed max error (H100): 2.0e-6; tolerance 7e-6."""
-    N, ldx, ldr, alpha = 256, 264, 260, 0.5
-    g = torch.Generator().manual_seed(M + K + 2 * ln2 + y2)
-    A = torch.randn(M, K, generator=g)
-    W = torch.randn(N, K, generator=g) / math.sqrt(K)
-    b = torch.randn(N, generator=g)
-    g1, b1 = torch.rand(N, generator=g) + 0.5, torch.randn(N, generator=g) * 0.1
-    g2, b2 = torch.rand(N, generator=g) + 0.5, torch.randn(N, generator=g) * 0.1
-    Ah, Al = split(rt, A.to(rt.dev))
-    Wh, Wl = split(rt, W.to(rt.dev))
-    bd, g1d, b1d, g2d, b2d = (t.to(rt.dev) for t in (b, g1, b1, g2, b2))
-    R = garbage((M + 3, ldx if alias else ldr), M)
-    R[:M, :N] = torch.randn(M, N, generator=g) * 3 + 0.5
-    Rd = R.to(rt.dev)
-    X = Rd if alias else nan((M + 3, ldx), rt.dev)
-    Y2 = nan((M + 3, ldx), rt.dev)
-    Yh, Yl = nan((M + 3, ldx), rt.dev, torch.float16), nan((M + 3, ldx), rt.dev, torch.float16)
-    rt.call("masr_gemm_tc_residual_ln_f16x2", P(Ah), P(Al), K, P(Wh), P(Wl), P(bd), P(Rd), ldx if alias else ldr, alpha, P(X),
-            P(g1d), P(b1d), P(g2d) if ln2 else None, P(b2d) if ln2 else None, P(Y2) if y2 else None, P(Yh), P(Yl), ldx, M, N, K,
-            1e-5, rt.st())
-    torch.cuda.synchronize()
-    x_new = R[:M, :N].double() + alpha * (A.double() @ W.double().t() + b.double())
-    l1 = F.layer_norm(x_new, (N,), g1.double(), b1.double(), 1e-5)
-    want_x, want_y = (l1, F.layer_norm(l1, (N,), g2.double(), b2.double(), 1e-5)) if ln2 else (x_new, l1)
-    X, Y2, Yh, Yl = X.cpu(), Y2.cpu(), Yh.cpu(), Yl.cpu()
-    errs = {"x": err(X[:M, :N], want_x), "y": err(pair_value(Yh[:M, :N], Yl[:M, :N]), want_y)}
-    mask = outside(X.shape, M, N)
-    if alias:
-        assert torch.equal(X[mask], R[mask]), "X written outside [M, 256]"
-    else:
-        assert all_nan(X, mask), "X written outside [M, 256]"
-        assert torch.equal(Rd.cpu(), R), "the residual buffer was modified"
-    assert all_nan(Yh, mask) and all_nan(Yl, mask), "pair written outside [M, 256]"
-    if y2:
-        errs["y2"] = err(Y2[:M, :N], want_y)
-        assert_pair_reconstructs(Yh[:M, :N], Yl[:M, :N], Y2[:M, :N])
-        assert all_nan(Y2, mask)
-    else:
-        assert all_nan(Y2), "Y2 = NULL, yet something was written"
-    report(f"residual_ln M={M} K={K} ln2={ln2} y2={y2} alias={alias}", **errs)
-    assert max(errs.values()) < 7e-6
-
-
-@pytest.mark.parametrize("M,K,ada,alias", [(1, 256, True, False), (77, 2304, False, True), (7937, 256, True, False)])
-def test_tc_gemm_residual_postln_float64(rt, M, K, ada, alias):
-    """masr_gemm_tc_residual_postln_f16x2 against float64: X <- LN(residual + A.W^T + b), pair <- ada_scale * X + ada_bias
-    (or X); the same row / column sentinels as the pre-norm form.  Observed max error (H100): 2.1e-6; tolerance 7e-6."""
-    N, ldx, ldr = 256, 264, 260
-    g = torch.Generator().manual_seed(M + K + ada)
-    A = torch.randn(M, K, generator=g)
-    W = torch.randn(N, K, generator=g) / math.sqrt(K)
-    b = torch.randn(N, generator=g)
-    ga, be = torch.rand(N, generator=g) + 0.5, torch.randn(N, generator=g) * 0.1
-    a_s, a_b = torch.rand(N, generator=g) + 0.5, torch.randn(N, generator=g) * 0.2
-    Ah, Al = split(rt, A.to(rt.dev))
-    Wh, Wl = split(rt, W.to(rt.dev))
-    bd, gd, bed, asd, abd = (t.to(rt.dev) for t in (b, ga, be, a_s, a_b))
-    R = garbage((M + 3, ldx if alias else ldr), M + 1)
-    R[:M, :N] = torch.randn(M, N, generator=g) * 2 - 0.3
-    Rd = R.to(rt.dev)
-    X = Rd if alias else nan((M + 3, ldx), rt.dev)
-    Yh, Yl = nan((M + 3, ldx), rt.dev, torch.float16), nan((M + 3, ldx), rt.dev, torch.float16)
-    rt.call("masr_gemm_tc_residual_postln_f16x2", P(Ah), P(Al), K, P(Wh), P(Wl), P(bd), P(Rd), ldx if alias else ldr, 1.0, P(X),
-            P(gd), P(bed), P(asd) if ada else None, P(abd) if ada else None, P(Yh), P(Yl), ldx, M, N, K, 1e-5, rt.st())
-    torch.cuda.synchronize()
-    want_x = F.layer_norm(R[:M, :N].double() + A.double() @ W.double().t() + b.double(), (N,), ga.double(), be.double(), 1e-5)
-    want_y = a_s.double() * want_x + a_b.double() if ada else want_x
-    X, Yh, Yl = X.cpu(), Yh.cpu(), Yl.cpu()
-    errs = {"x": err(X[:M, :N], want_x), "y": err(pair_value(Yh[:M, :N], Yl[:M, :N]), want_y)}
-    mask = outside(X.shape, M, N)
-    if alias:
-        assert torch.equal(X[mask], R[mask]), "X written outside [M, 256]"
-    else:
-        assert all_nan(X, mask) and torch.equal(Rd.cpu(), R)
-    assert all_nan(Yh, mask) and all_nan(Yl, mask), "pair written outside [M, 256]"
-    report(f"residual_postln M={M} K={K} ada={ada} alias={alias}", **errs)
-    assert max(errs.values()) < 7e-6
 
 
 # ---- CTC head ----------------------------------------------------------------------------------------------------------------

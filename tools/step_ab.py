@@ -1,8 +1,10 @@
 """Dev tool: A/B of the headline device step (32 x 10 s, conformer streaming, greedy; inputs resident; one CUDA graph per
 variant) under different kernel-selection environments, INTERLEAVED in one process so that box-to-box and thermal drift
 cancel: every round replays each variant's graph `REPS` times (L2 flushed before every replay, CUDA events), `ROUNDS` rounds.
-Also checks that every variant produces the same token ids.  Variants: name=ENV1:VAL1,ENV2:VAL2 ... on the command line, e.g.
-    python tools/step_ab.py default= pair=MASR_TC_PAIR:1
+Also checks that every variant produces the same token ids.  Variants: name=ENV1:VAL1,ENV2:VAL2 ... on the command line
+(switches the library reads per launch), e.g.
+    python tools/step_ab.py default= unstaged=MASR_TC_FLAGS:0
+Without arguments the default variant alone runs (with AB_LIB: the step time of another build of the library).
 Not a bench value."""
 import json
 import os
@@ -26,7 +28,7 @@ for a in sys.argv[1:]:
     name, _, envs = a.partition("=")
     variants.append((name, dict(kv.split(":") for kv in envs.split(",") if kv)))
 if not variants:
-    variants = [("default", {}), ("pair", {"MASR_TC_PAIR": "1"})]
+    variants = [("default", {})]
 touched = sorted({k for _, e in variants for k in e})
 
 eng = ConformerEngine(synth.conformer_state_dict(0, 4233), streaming=True)
@@ -37,8 +39,6 @@ for name, env in variants:
     for k in touched:
         os.environ.pop(k, None)
     os.environ.update(env)
-    eng.lnpre = os.environ.get("MASR_FUSE_LNPRE", "0") == "1"          # engine-level switches are read at construction: refresh
-    eng.fuse = os.environ.get("MASR_FUSE_LN", "0") == "1"
     eng._graphs.clear()
     st = eng.prepare_resident(waves)
     for _ in range(3):
