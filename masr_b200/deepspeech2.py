@@ -147,19 +147,7 @@ class DeepSpeech2Engine(ConformerEngine):
                 t[l, "wih"] = [self._split(x) for x in ent["wih"]]
         torch.cuda.synchronize(self.device)
 
-    def _workspace(self, B: int, Fmax: int):
-        key = (B, Fmax)
-        ws = self._ws.get(key)
-        if ws is not None:
-            return ws
-        ws = self._alloc_workspace(B, Fmax)
-        if len(self._ws) > 8:
-            self._ws.clear()
-        self._ws[key] = ws
-        return ws
-
     def _alloc_workspace(self, B: int, Fmax: int):
-        """The device buffers of one (B, Fmax) pass, owned by the caller (``_workspace`` caches them per shape)."""
         dev, f32, f16 = self.device, torch.float32, torch.float16
         F1 = (Fmax - 1) // 2
         T = subsampled_len(Fmax)
@@ -258,12 +246,6 @@ class DeepSpeech2Engine(ConformerEngine):
     def _ctc_operand(self, ws):
         return ws["xp"], self.H * self.dirs
 
-    def ctc_logits(self, enc, ws):
-        M = enc.shape[0]
-        D = self.H * self.dirs
-        self._tc(ws["xp"], D, self._tcw["ctc"], self.w.ctc_b, M, self.V, D, C=ws["logits"], ldc=self.Vpad, tag="ctc_head")
-        return ws["logits"]
-
     # ---- streaming ----------------------------------------------------------------------------------
     def new_stream(self, n: int = 1) -> DeepSpeech2Stream:
         """The carried recurrent state of `n` streams (``DeepSpeech2StreamPool`` keeps one for all its slots)."""
@@ -289,11 +271,3 @@ class DeepSpeech2Engine(ConformerEngine):
         logits = self._ctc_argmax(ws, T, probs)
         st.last_logits = logits[:T]                    # (the streaming beam search reads the chunk's logits)
         return ws["ids"][:T], ws["maxp"][:T], probs
-
-    def _ctc_argmax(self, ws, M: int, probs: Optional[torch.Tensor] = None):
-        """CTC head over the M rows of the last LayerNorm output, then per row the argmax id and its probability (and the
-        posteriors into `probs` [M, V] when given) -> the logits [M, Vpad]."""
-        logits = self.ctc_logits(ws["t0"][:M], ws)
-        self._k("ctc_argmax", "masr_ctc_frame_argmax_f32", _p(logits), self.Vpad, M, self.V, _p(ws["ids"]), _p(ws["maxp"]),
-                _p(probs), self.V)
-        return logits

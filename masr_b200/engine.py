@@ -177,6 +177,13 @@ class ConformerEngine:
         self._k("ffn_fused", "masr_ffn_tc_f16x2", _p(A[0]), _p(A[1]), d, _p(W1[0]), _p(W1[1]), _p(b1), _p(W2[0]), _p(W2[1]),
                 _p(b2), _p(x), d, M, d, self.w.ffn, alpha)
 
+    def _ffn_gemms(self, A, W1, b1, W2, b2, M, res, out, alpha, hidp):
+        """out <- res + alpha * (SiLU(A.W1^T + b1) . W2^T + b2) as two launches: w_1 (EPI_BIAS_SILU) into the hidden pair
+        `hidp`, then w_2 (EPI_RESIDUAL)."""
+        d, ffn = self.d, self.w.ffn
+        self._tc(A, d, W1, b1, M, ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=ffn, tag="ffn_w1")
+        self._tc(hidp, ffn, W2, b2, M, d, ffn, EPI_RESIDUAL, alpha, res, d, C=out, ldc=d, tag="ffn_w2")
+
     def _hidp(self, ws):
         """The [M, ffn] hidden pair of the two-launch FFN form, allocated on first use (the fused FFN does not need it)."""
         if "hidp" not in ws:
@@ -191,7 +198,7 @@ class ConformerEngine:
         host/launch latency that event pairs around single eager launches include (bench.py's roofline leg).
         With the fused FFN kernel (``_ffn_fused``) the replay is of that kernel, and the result is HALF a fused launch: one
         fused launch does the work of one w_1 and one w_2 launch, so the FLOPs per "GEMM launch" stay 2 M 256 ffn."""
-        w, d, tw, L = self.w, self.d, self._tcw, self.w.layers[0]
+        tw, L = self._tcw, self.w.layers[0]
         t0p = ws["t0p"]
         xs = torch.zeros_like(ws["x"])                       # scratch residual stream (the replays keep adding into it)
         dev = self.device
@@ -201,10 +208,8 @@ class ConformerEngine:
             for _ in range(reps):
                 if fused:
                     self._ffn_tc(t0p, tw[0, "ffm1"], L.ffm[1], tw[0, "ffm2"], L.ffm[3], M, xs)
-                    continue
-                hidp = self._hidp(ws)
-                self._tc(t0p, d, tw[0, "ffm1"], L.ffm[1], M, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn, tag="ffn_w1")
-                self._tc(hidp, w.ffn, tw[0, "ffm2"], L.ffm[3], M, d, w.ffn, EPI_RESIDUAL, 0.5, xs, d, C=xs, ldc=d, tag="ffn_w2")
+                else:
+                    self._ffn_gemms(t0p, tw[0, "ffm1"], L.ffm[1], tw[0, "ffm2"], L.ffm[3], M, xs, xs, 0.5, self._hidp(ws))
 
         prof, self.prof = self.prof, None
         n0 = self.launches
@@ -240,6 +245,44 @@ class ConformerEngine:
         tmp = self._ln_tmp
         self._ln(x, gb, tmp, M)
         self._k("layernorm", "masr_split_f16", _p(tmp), _p(yp[0]), _p(yp[1]), M * self.d)
+
+    def _embed_epilogue(self):
+        """Epilogue and alpha of the embed GEMM: xscale = sqrt(d) applied to its output (embedding.py)."""
+        return EPI_BIAS_SCALE, float(self.d) ** 0.5
+
+    def _subsample(self, feats, planes, B: int, Fmax: int, T: int, out):
+        """Conv2dSubsampling4 (+ CMVN) and the embed linear on the tensor cores: feats [B, Fmax, 80] -> out fp32 [B*T, d],
+        through the "c1p" / "c2p" pairs of `planes` (``_subsample_planes``)."""
+        w, d, tw = self.w, self.d, self._tcw
+        F1 = (Fmax - 1) // 2
+        c1p, c2p = planes["c1p"], planes["c2p"]
+        self._k("conv1", "masr_conv1_cmvn_relu_planes_f16", _p(feats), _p(w.cmvn_mean), _p(w.cmvn_istd), _p(w.conv1_w),
+                _p(w.conv1_b), _p(c1p[0]), _p(c1p[1]), B, Fmax, w.idim, F1, self.w1_cols, d)
+        self._k("conv2", "masr_conv2_tc_f16x2", _p(c1p[0]), _p(c1p[1]), _p(tw["conv2"][0]), _p(tw["conv2"][1]),
+                _p(w.conv2_b), None, _p(c2p[0]), _p(c2p[1]), B, F1, T, d)
+        epi, alpha = self._embed_epilogue()
+        self._tc(c2p, self.f2 * d, tw["embed"], w.embed_b, B * T, d, self.f2 * d, epi, alpha, C=out, ldc=d, tag="embed_linear")
+
+    def _dw_context(self, L, cached: bool):
+        """(pad_vec, lpad) of a depthwise conv: with a cache the left context is in the input rows; without one, a causal
+        conv pads `kernel - 1` GLU-of-zero rows on the left and a symmetric one `(kernel - 1) // 2` zero rows."""
+        if cached:
+            return None, 0
+        return (_p(L.glu_pad), L.kernel - 1) if self.causal else (None, (L.kernel - 1) // 2)
+
+    def _dwconv(self, L, g, g_rows: int, lens, B: int, out_rows: int, out, out_stride: Optional[int] = None,
+                cached: bool = False, stride: int = 1):
+        """Depthwise conv + LayerNorm + SiLU of the conv module over g [B * g_rows, d] -> `out` (fp32 tensor or fp16 pair),
+        `out_rows` rows per utterance spaced `out_stride` (default `out_rows`) apart; `stride` 2 is the strided form."""
+        d = self.d
+        y, yp = (None, out) if isinstance(out, tuple) else (out, (None, None))
+        pad, lpad = self._dw_context(L, cached)
+        args = (_p(g), d, g_rows, _p(L.dw), _p(L.dw_b), _p(L.cn[0]), _p(L.cn[1]), pad, _p(y), _p(yp[0]), _p(yp[1]), d,
+                out_rows if out_stride is None else out_stride, _p(lens), B, d, L.kernel, lpad)
+        if stride == 1:
+            self._k("dwconv_ln_silu", "masr_dwconv_ln_silu_f32", *args, out_rows, 1e-5)
+        else:
+            self._k("dwconv_ln_silu", "masr_dwconv_ln_silu_strided_f32", *args, stride, out_rows, 1e-5)
 
     # ------------------------------------------------------------------------------------------
     def _stream(self):
@@ -300,18 +343,44 @@ class ConformerEngine:
         ld = self.d if ld is None else ld
         self._k("layernorm", "masr_layernorm_f32", _p(x), ld, _p(gb[0]), _p(gb[1]), _p(y), ld, M, self.d, 1e-5)
 
+    def _half_rate(self, i: int) -> bool:
+        """Block i runs at half the encoder frame rate (and sees pos_emb[:, ::2])."""
+        return False
+
     def _precompute_pos(self):
-        """linear_pos(pe) for every layer: input-independent (attention.py:228), done once on the GPU."""
-        for L in self.w.layers:
-            L.ptab = torch.empty(self.w.max_len, self.d, device=self.device, dtype=torch.float32)
-            self._gemm(self.w.pe, self.d, L.wpos, None, L.ptab, self.d, self.w.max_len, self.d, self.d)
+        """linear_pos(pe) for every layer: input-independent (attention.py:228), done once on the GPU.  A half-rate block's
+        table is linear_pos(pe[::2])."""
+        half = [self._half_rate(i) for i in range(len(self.w.layers))]
+        pe2 = self.w.pe[::2].contiguous() if any(half) else None
+        for L, h in zip(self.w.layers, half):
+            pe = pe2 if h else self.w.pe
+            L.ptab = torch.empty(pe.shape[0], self.d, device=self.device, dtype=torch.float32)
+            self._gemm(pe, self.d, L.wpos, None, L.ptab, self.d, pe.shape[0], self.d, self.d)
         torch.cuda.synchronize(self.device)
 
     def _workspace(self, B: int, Fmax: int) -> Dict[str, torch.Tensor]:
+        """The device buffers of one (B, Fmax) pass, cached per shape."""
         key = (B, Fmax)
         ws = self._ws.get(key)
         if ws is not None:
             return ws
+        ws = self._alloc_workspace(B, Fmax)
+        if len(self._ws) > 8:
+            self._ws.clear()
+        self._ws[key] = ws
+        return ws
+
+    def _subsample_planes(self, B: int, Fmax: int) -> Dict[str, tuple]:
+        """The fp16 pairs of the tensor-core subsampling front-end for B rows of Fmax frames: conv-1 parity planes "c1p"
+        ([4][B][(F1+1)/2][20][d], include/masr_b200.h) and conv-2 output rows "c2p"."""
+        dev, f16, d = self.device, torch.float16, self.d
+        TH = ((Fmax - 1) // 2 + 1) // 2
+        M = max(1, B * subsampled_len(Fmax))
+        return {"c1p": (torch.zeros(4 * B * TH * 20 * d, device=dev, dtype=f16), torch.zeros(4 * B * TH * 20 * d, device=dev, dtype=f16)),
+                "c2p": (torch.empty(M * self.f2, d, device=dev, dtype=f16), torch.empty(M * self.f2, d, device=dev, dtype=f16))}
+
+    def _alloc_workspace(self, B: int, Fmax: int) -> Dict[str, torch.Tensor]:
+        """The device buffers of one (B, Fmax) pass, owned by the caller (``_workspace`` caches them per shape)."""
         dev, f32 = self.device, torch.float32
         F1 = (Fmax - 1) // 2
         T = subsampled_len(Fmax)
@@ -333,17 +402,12 @@ class ConformerEngine:
         self._alloc_out_pack(ws, B, T)
         if self.gemm_path == "tc":
             f16 = torch.float16
-            TH = (F1 + 1) // 2
             Mx = max(1, M)
             del ws["c1"], ws["c2"], ws["hid"]
-            ws["c1p"] = (torch.zeros(4 * B * TH * 20 * d, device=dev, dtype=f16), torch.zeros(4 * B * TH * 20 * d, device=dev, dtype=f16))
-            ws["c2p"] = (torch.empty(Mx * self.f2, d, device=dev, dtype=f16), torch.empty(Mx * self.f2, d, device=dev, dtype=f16))
+            ws.update(self._subsample_planes(B, Fmax))
             ws["t0p"] = (torch.empty(Mx, d, device=dev, dtype=f16), torch.empty(Mx, d, device=dev, dtype=f16))
             ws["t1p"] = (torch.empty(Mx, d, device=dev, dtype=f16), torch.empty(Mx, d, device=dev, dtype=f16))
             ws["qkvp"] = (torch.empty(Mx, 3 * d, device=dev, dtype=f16), torch.empty(Mx, 3 * d, device=dev, dtype=f16))
-        if len(self._ws) > 8:
-            self._ws.clear()
-        self._ws[key] = ws
         return ws
 
     def _alloc_out_pack(self, ws, B: int, T: int):
@@ -471,7 +535,7 @@ class ConformerEngine:
             self.h2d_bytes += 4 * B
         tlens = ws["tlens"]
         if self.gemm_path == "tc":
-            return self._encode_tc(feats, ws, tl, tlens, B, Fmax, F1, T, M)
+            return self._encode_tc(feats, ws, tl, tlens, B, Fmax, T, M)
         # Conv2dSubsampling4 (+ CMVN) -> x * sqrt(d)
         self._k("conv1", "masr_conv1_cmvn_relu_f32", _p(feats), _p(w.cmvn_mean), _p(w.cmvn_istd), _p(w.conv1_w),
                 _p(w.conv1_b), _p(ws["c1"]), B, Fmax, w.idim, F1, self.w1_cols, d)
@@ -480,7 +544,6 @@ class ConformerEngine:
         x, t0, t1, g, hid, qkv = ws["x"], ws["t0"], ws["t1"], ws["g"], ws["hid"], ws["qkv"]
         self._gemm(ws["c2"], self.f2 * d, w.embed_w, w.embed_b, x, d, M, d, self.f2 * d, EPI_BIAS_SCALE, float(d) ** 0.5,
                    tag="embed_linear")
-        lpad = (w.kernel - 1) if self.causal else (w.kernel - 1) // 2
         for L in w.layers:
             # macaron FFN: x += 0.5 * W2 silu(W1 LN(x))
             self._ln(x, L.ln_ffm, t0, M)
@@ -496,9 +559,7 @@ class ConformerEngine:
             # convolution module
             self._ln(x, L.ln_conv, t0, M)
             self._gemm(t0, d, L.pw1, L.pw1_b, g, d, M, 2 * d, d, EPI_BIAS_GLU, tag="pw1_glu")
-            self._k("dwconv_ln_silu", "masr_dwconv_ln_silu_f32", _p(g), d, T, _p(L.dw), _p(L.dw_b), _p(L.cn[0]),
-                    _p(L.cn[1]), _p(L.glu_pad) if self.causal else None, _p(t1), None, None, d, T, _p(tlens), B, d,
-                    w.kernel, lpad, T, 1e-5)
+            self._dwconv(L, g, T, tlens, B, T, t1)
             self._gemm(t1, d, L.pw2, L.pw2_b, x, d, M, d, d, EPI_RESIDUAL, 1.0, x, d, tag="pw2")
             # FFN
             self._ln(x, L.ln_ff, t0, M)
@@ -508,23 +569,17 @@ class ConformerEngine:
         self._ln(x, w.after_norm, t0, M)
         return t0[:M], tl, T, ws
 
-    def _encode_tc(self, feats, ws, tl, tlens, B, Fmax, F1, T, M):
+    def _encode_tc(self, feats, ws, tl, tlens, B, Fmax, T, M):
         """Same layer program as ``encode`` with every dense contraction on wgmma (FP16x2 split): GEMM inputs
         travel as fp16 (h,l) pairs written by the producing kernel's epilogue, the residual stream stays fp32."""
         w, d, tw = self.w, self.d, self._tcw
         x, g, qkv = ws["x"], ws["g"], ws["qkv"]
-        t0p, t1p, c1p, c2p = ws["t0p"], ws["t1p"], ws["c1p"], ws["c2p"]
+        t0p, t1p = ws["t0p"], ws["t1p"]
         self._ln_tmp = ws["t1"]                       # fp32 scratch of _ln_split at d = 512 (not otherwise used on this path)
         # the FFN modules: one fused launch each (masr_ffn_tc_f16x2), or w_1 + w_2 through the hidden pair
         ffn_fused = self._ffn_fused()
         hidp = None if ffn_fused else self._hidp(ws)
-        self._k("conv1", "masr_conv1_cmvn_relu_planes_f16", _p(feats), _p(w.cmvn_mean), _p(w.cmvn_istd), _p(w.conv1_w),
-                _p(w.conv1_b), _p(c1p[0]), _p(c1p[1]), B, Fmax, w.idim, F1, self.w1_cols, d)
-        self._k("conv2", "masr_conv2_tc_f16x2", _p(c1p[0]), _p(c1p[1]), _p(tw["conv2"][0]), _p(tw["conv2"][1]),
-                _p(w.conv2_b), None, _p(c2p[0]), _p(c2p[1]), B, F1, T, d)
-        self._tc(c2p, self.f2 * d, tw["embed"], w.embed_b, M, d, self.f2 * d, EPI_BIAS_SCALE, float(d) ** 0.5, C=x, ldc=d,
-                 tag="embed_linear")
-        lpad = (w.kernel - 1) if self.causal else (w.kernel - 1) // 2
+        self._subsample(feats, ws, B, Fmax, T, x)
         nl = len(w.layers)
         for i, L in enumerate(w.layers):
             if i == 0:                                # later blocks: t0p is written by the previous block's norm_final (below)
@@ -532,24 +587,20 @@ class ConformerEngine:
             if ffn_fused:
                 self._ffn_tc(t0p, tw[i, "ffm1"], L.ffm[1], tw[i, "ffm2"], L.ffm[3], M, x)
             else:
-                self._tc(t0p, d, tw[i, "ffm1"], L.ffm[1], M, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn, tag="ffn_w1")
-                self._tc(hidp, w.ffn, tw[i, "ffm2"], L.ffm[3], M, d, w.ffn, EPI_RESIDUAL, 0.5, x, d, C=x, ldc=d, tag="ffn_w2")
+                self._ffn_gemms(t0p, tw[i, "ffm1"], L.ffm[1], tw[i, "ffm2"], L.ffm[3], M, x, x, 0.5, hidp)
             self._ln_split(x, L.ln_mha, t0p, M)
             self._tc(t0p, d, tw[i, "qkv"], L.bqkv, M, 3 * d, d, C=qkv, Cp=ws["qkvp"], ldc=3 * d, tag="qkv_proj")
             self._attention_tc(L, qkv, ws["qkvp"], t1p, T, tlens, B)
             self._tc(t1p, d, tw[i, "wo"], L.bo, M, d, d, EPI_RESIDUAL, 1.0, x, d, C=x, ldc=d, tag="out_proj")
             self._ln_split(x, L.ln_conv, t0p, M)
             self._tc(t0p, d, tw[i, "pw1"], L.pw1_b, M, 2 * d, d, EPI_BIAS_GLU, C=g, ldc=d, tag="pw1_glu")
-            self._k("dwconv_ln_silu", "masr_dwconv_ln_silu_f32", _p(g), d, T, _p(L.dw), _p(L.dw_b), _p(L.cn[0]),
-                    _p(L.cn[1]), _p(L.glu_pad) if self.causal else None, None, _p(t1p[0]), _p(t1p[1]), d, T, _p(tlens), B,
-                    d, w.kernel, lpad, T, 1e-5)
+            self._dwconv(L, g, T, tlens, B, T, t1p)
             self._tc(t1p, d, tw[i, "pw2"], L.pw2_b, M, d, d, EPI_RESIDUAL, 1.0, x, d, C=x, ldc=d, tag="pw2")
             self._ln_split(x, L.ln_ff, t0p, M)
             if ffn_fused:
                 self._ffn_tc(t0p, tw[i, "ff1"], L.ff[1], tw[i, "ff2"], L.ff[3], M, x)
             else:
-                self._tc(t0p, d, tw[i, "ff1"], L.ff[1], M, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn, tag="ffn_w1")
-                self._tc(hidp, w.ffn, tw[i, "ff2"], L.ff[3], M, d, w.ffn, EPI_RESIDUAL, 0.5, x, d, C=x, ldc=d, tag="ffn_w2")
+                self._ffn_gemms(t0p, tw[i, "ff1"], L.ff[1], tw[i, "ff2"], L.ff[3], M, x, x, 0.5, hidp)
             # x = norm_final(x + 0.5 ffn), then in the same pass the next consumer's LayerNorm: the next block's
             # norm_ff_macaron (pair only) or, after the last block, after_norm (fp32 encoder output + the CTC head's pair)
             nxt = w.layers[i + 1].ln_ffm if i + 1 < nl else w.after_norm
@@ -563,14 +614,23 @@ class ConformerEngine:
         """The fp16 (h,l) pair of the encoder output the CTC head multiplies, and its width."""
         return ws["t0p"], self.d
 
-    def ctc_logits(self, enc: torch.Tensor, ws) -> torch.Tensor:
-        M = enc.shape[0]
+    def ctc_logits(self, ws, M: int) -> torch.Tensor:
+        """CTC head over the first M encoder output rows -> ws["logits"] [M, Vpad].  Tensor-core path: from the pair
+        ``_ctc_operand(ws)``; simt path: from the fp32 encoder output ws["t0"]."""
         if self.gemm_path == "tc":
-            self._tc(ws["t0p"], self.d, self._tcw["ctc"], self.w.ctc_b, M, self.V, self.d, C=ws["logits"], ldc=self.Vpad,
-                     tag="ctc_head")
+            Ap, K = self._ctc_operand(ws)
+            self._tc(Ap, K, self._tcw["ctc"], self.w.ctc_b, M, self.V, K, C=ws["logits"], ldc=self.Vpad, tag="ctc_head")
         else:
-            self._gemm(enc, self.d, self.w.ctc_w, self.w.ctc_b, ws["logits"], self.Vpad, M, self.V, self.d, tag="ctc_head")
+            self._gemm(ws["t0"], self.d, self.w.ctc_w, self.w.ctc_b, ws["logits"], self.Vpad, M, self.V, self.d, tag="ctc_head")
         return ws["logits"]
+
+    def _ctc_argmax(self, ws, M: int, probs: Optional[torch.Tensor] = None):
+        """CTC head over M rows, then per row the argmax id and its probability into ws["ids"] / ws["maxp"] (and the
+        posteriors into `probs` [M, V] when given) -> the logits [M, Vpad]."""
+        logits = self.ctc_logits(ws, M)
+        self._k("ctc_argmax", "masr_ctc_frame_argmax_f32", _p(logits), self.Vpad, M, self.V, _p(ws["ids"]), _p(ws["maxp"]),
+                _p(probs), self.V)
+        return logits
 
     def ctc_greedy(self, enc: torch.Tensor, out_lens: Sequence[int], T: int, ws, want_probs: bool = False):
         """-> device tensors (tokens [B,T], ntok, psum, pcount, ids [B*T], probs or None)."""
@@ -587,10 +647,8 @@ class ConformerEngine:
                     _p(self._tcw["ctc"][1]), _p(self.w.ctc_b), M, self.V, K, _p(ws["ctc_part"]), ws["ctc_part"].numel(),
                     _p(ws["ids"]), _p(ws["maxp"]), n=2)
         else:
-            logits = self.ctc_logits(enc, ws)
             probs = torch.empty(M, self.V, device=self.device, dtype=torch.float32) if want_probs else None
-            self._k("ctc_argmax", "masr_ctc_frame_argmax_f32", _p(logits), self.Vpad, M, self.V, _p(ws["ids"]),
-                    _p(ws["maxp"]), _p(probs), self.V)
+            self._ctc_argmax(ws, M, probs)
         self._k("ctc_collapse", "masr_ctc_greedy_collapse", _p(ws["ids"]), _p(ws["maxp"]), T, _p(ws["tlens"]), B, 0,
                 _p(ws["tokens"]), ws["tokens"].shape[1], _p(ws["ntok"]), _p(ws["psum"]), _p(ws["pcount"]))
         return probs
@@ -606,7 +664,7 @@ class ConformerEngine:
         in ws["beam_score"], and ln p_blank per row in ws["blank_lp"]).  Parity unpinned (DESIGN.md)."""
         B, Tb = len(out_lens), max(1, T)
         settings = (beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta)
-        logits = self.ctc_logits(enc, ws)
+        logits = self.ctc_logits(ws, enc.shape[0])
         if "beam" not in ws or not ws["beam"].fits(B, Tb, *settings):
             ws.pop("beam", None)                      # (the old buffers go back to the allocator before the new ones are taken)
             ws["beam"] = BeamSearch(self.device, ONE_SHOT, B, B * Tb, Tb, *settings)
@@ -691,7 +749,7 @@ class ConformerEngine:
                     slot["h_sc"][:B].zero_()
                     slot["done"].record(main)
                 else:
-                    bs.topk(self, self.ctc_logits(enc, ws), self.Vpad, B * T)
+                    bs.topk(self, self.ctc_logits(ws, enc.shape[0]), self.Vpad, B * T)
                     slot["tlens"][:B].copy_(ws["tlens"][:B])
                     slot["ready"].record(main)
                     side.wait_event(slot["ready"])
@@ -1048,7 +1106,7 @@ class ConformerEngine:
         model.py:169-190): feats_chunk [n<=67, 80] raw log-mel on device -> per-frame (ids, max-prob)
         device tensors of length c = ((n-1)//2-1)//2 (+ posteriors [c,V] if asked).  Updates the
         stream's attention / convolution caches and ``offset`` like inference_predictor.py:84-93."""
-        w, d, s = self.w, self.d, self._stream()
+        w, d = self.w, self.d
         n = int(feats_chunk.shape[0])
         c = subsampled_len(n)
         if c == 0:
@@ -1063,11 +1121,10 @@ class ConformerEngine:
             raise AssertionError("offset: {} + x.shape[1]: {} is larger than the max_len: {}".format(st.offset, c, w.max_len))
         st.reserve(key_size)
         ws = st.ws
-        call("masr_conv1_cmvn_relu_f32", _p(feats_chunk), _p(w.cmvn_mean), _p(w.cmvn_istd), _p(w.conv1_w), _p(w.conv1_b),
-             _p(ws["c1"]), 1, n, w.idim, F1, self.w1_cols, d, s)
-        call("masr_conv2_s2_relu_f32", _p(ws["c1"]), _p(w.conv2_w), _p(w.conv2_b), _p(ws["c2"]), 1, F1, self.w1_cols, c,
-             self.f2, d, s)
-        self.launches += 2
+        self._k("conv1", "masr_conv1_cmvn_relu_f32", _p(feats_chunk), _p(w.cmvn_mean), _p(w.cmvn_istd), _p(w.conv1_w),
+                _p(w.conv1_b), _p(ws["c1"]), 1, n, w.idim, F1, self.w1_cols, d)
+        self._k("conv2", "masr_conv2_s2_relu_f32", _p(ws["c1"]), _p(w.conv2_w), _p(w.conv2_b), _p(ws["c2"]), 1, F1,
+                self.w1_cols, c, self.f2, d)
         x, t0, t1, g, hid, q, xcat = ws["x"], ws["t0"], ws["t1"], ws["g"], ws["hid"], ws["q"], ws["xcat"]
         self._gemm(ws["c2"], self.f2 * d, w.embed_w, w.embed_b, x, d, c, d, self.f2 * d, EPI_BIAS_SCALE, float(d) ** 0.5)
         ws["qlen"].fill_(c)
@@ -1081,23 +1138,19 @@ class ConformerEngine:
             self._ln(x, L.ln_mha, t0, c)
             kv = st.kv[li]                                             # [cap, 2d] rows = key positions
             self._gemm(t0, d, L.wqkv, L.bqkv, q, d, c, d, d)           # q
-            call("masr_gemm_f32", _p(t0), d, L.wqkv.data_ptr() + 4 * d * d, L.bqkv.data_ptr() + 4 * d, None, 0,
-                 kv.data_ptr() + 4 * (st.cache_start + cache_t1) * 2 * d, 2 * d, c, 2 * d, d, EPI_BIAS, 1.0, s)  # k|v appended
+            self._k("gemm", "masr_gemm_f32", _p(t0), d, L.wqkv.data_ptr() + 4 * d * d, L.bqkv.data_ptr() + 4 * d, None, 0,
+                    kv.data_ptr() + 4 * (st.cache_start + cache_t1) * 2 * d, 2 * d, c, 2 * d, d, EPI_BIAS, 1.0)  # k|v appended
             kbase = kv.data_ptr() + 4 * st.cache_start * 2 * d
-            call("masr_relpos_attention_f32", _p(q), d, 0, kbase, kbase + 4 * d, 2 * d, 0,
-                 L.ptab.data_ptr() + 4 * pos_start * d, d, _p(L.pos_u), _p(L.pos_v), _p(t1), None, None, d, 0, _p(ws["qlen"]),
-                 _p(ws["klen"]), 1, self.h, self.dk, c, s)
-            self.launches += 2
+            self._k("attention", "masr_relpos_attention_f32", _p(q), d, 0, kbase, kbase + 4 * d, 2 * d, 0,
+                    L.ptab.data_ptr() + 4 * pos_start * d, d, _p(L.pos_u), _p(L.pos_v), _p(t1), None, None, d, 0,
+                    _p(ws["qlen"]), _p(ws["klen"]), 1, self.h, self.dk, c)
             self._gemm(t1, d, L.wo, L.bo, x, d, c, d, d, EPI_RESIDUAL, 1.0, x, d)
             # conv module over [cache ++ chunk] (convolution.py:101-109); zero cache == the reference's zero pad
             xc = xcat[li]
-            call("masr_layernorm_f32", _p(x), d, _p(L.ln_conv[0]), _p(L.ln_conv[1]), xc.data_ptr() + 4 * lorder * d, d, c,
-                 d, 1e-5, s)
-            self.launches += 1
+            self._k("layernorm", "masr_layernorm_f32", _p(x), d, _p(L.ln_conv[0]), _p(L.ln_conv[1]),
+                    xc.data_ptr() + 4 * lorder * d, d, c, d, 1e-5)
             self._gemm(xc, d, L.pw1, L.pw1_b, g, d, lorder + c, 2 * d, d, EPI_BIAS_GLU)
-            call("masr_dwconv_ln_silu_f32", _p(g), d, 0, _p(L.dw), _p(L.dw_b), _p(L.cn[0]), _p(L.cn[1]), None, _p(t1), None, None, d, 0,
-                 _p(ws["clen"]), 1, d, w.kernel, 0, c, 1e-5, s)
-            self.launches += 1
+            self._dwconv(L, g, 0, ws["clen"], 1, c, t1, out_stride=0, cached=True)
             # new cnn cache = last `lorder` rows of [cache ++ chunk]; overlapping move -> go through a scratch
             ws["ctmp"][:lorder].copy_(xc[c:c + lorder])
             xc[:lorder].copy_(ws["ctmp"][:lorder])
@@ -1109,9 +1162,8 @@ class ConformerEngine:
         self._ln(x, w.after_norm, t0, c)
         self._gemm(t0, d, w.ctc_w, w.ctc_b, ws["logits"], self.Vpad, c, self.V, d)
         probs = torch.empty(c, self.V, device=self.device, dtype=torch.float32) if want_probs else None
-        call("masr_ctc_frame_argmax_f32", _p(ws["logits"]), self.Vpad, c, self.V, _p(ws["ids"]), _p(ws["maxp"]), _p(probs),
-             self.V, s)
-        self.launches += 1
+        self._k("ctc_argmax", "masr_ctc_frame_argmax_f32", _p(ws["logits"]), self.Vpad, c, self.V, _p(ws["ids"]),
+                _p(ws["maxp"]), _p(probs), self.V)
         # cache bookkeeping (encoder.py:397-402, inference_predictor.py:93)
         if required_cache_size < 0:
             keep = key_size
@@ -1245,13 +1297,9 @@ class EfficientConformerEngine(ConformerEngine):
         if gemm != "tc":
             raise ValueError("EfficientConformerEngine implements the tensor-core path only")
         super().__init__(weights_src, streaming, device, max_len, gemm, use_graphs)
-        # blocks after the strided one see pos_emb[:, ::2] (encoder.py:257): their linear_pos table comes from pe[::2]
-        pe2 = self.w.pe[::2].contiguous()
-        for i, L in enumerate(self.w.layers):
-            if i > self.STRIDE_LAYER:
-                L.ptab = torch.empty(pe2.shape[0], self.d, device=self.device, dtype=torch.float32)
-                self._gemm(pe2, self.d, L.wpos, None, L.ptab, self.d, pe2.shape[0], self.d, self.d)
-        torch.cuda.synchronize(self.device)
+
+    def _half_rate(self, i: int) -> bool:
+        return i > self.STRIDE_LAYER           # blocks after the strided one see pos_emb[:, ::2] (encoder.py:257)
 
     def _pack(self, sd, max_len):
         return pack_conformer(sd, self.device, max_len, family="efficient_conformer")
@@ -1271,29 +1319,22 @@ class EfficientConformerEngine(ConformerEngine):
             raise ValueError("create the stream with new_stream(keep_probs=True) to get the chunk posteriors")
         return st.encode_chunk(feats_chunk, required_cache_size)
 
-    def _encode_tc(self, feats, ws, tl, tlens, B, Fmax, F1, T, M):
+    def _encode_tc(self, feats, ws, tl, tlens, B, Fmax, T, M):
         w, d, tw = self.w, self.d, self._tcw
         x, g, qkv = ws["x"], ws["g"], ws["qkv"]
-        t0p, t1p, hidp, c1p, c2p = ws["t0p"], ws["t1p"], self._hidp(ws), ws["c1p"], ws["c2p"]
+        t0p, t1p, hidp = ws["t0p"], ws["t1p"], self._hidp(ws)
         T2 = self.final_len(T)
         if "tlens2" not in ws:
             ws["tlens2"] = torch.zeros(B, device=self.device, dtype=torch.int32)
         tlens2 = ws["tlens2"]
         torch.div(tlens + 1, 2, rounding_mode="floor", out=tlens2)
-        self._k("conv1", "masr_conv1_cmvn_relu_planes_f16", _p(feats), _p(w.cmvn_mean), _p(w.cmvn_istd), _p(w.conv1_w),
-                _p(w.conv1_b), _p(c1p[0]), _p(c1p[1]), B, Fmax, w.idim, F1, self.w1_cols, d)
-        self._k("conv2", "masr_conv2_tc_f16x2", _p(c1p[0]), _p(c1p[1]), _p(tw["conv2"][0]), _p(tw["conv2"][1]),
-                _p(w.conv2_b), None, _p(c2p[0]), _p(c2p[1]), B, F1, T, d)
-        self._tc(c2p, self.f2 * d, tw["embed"], w.embed_b, M, d, self.f2 * d, EPI_BIAS_SCALE, float(d) ** 0.5, C=x, ldc=d,
-                 tag="embed_linear")
+        self._subsample(feats, ws, B, Fmax, T, x)
         qb, kb, vb = qkv.view(-1)[:M * d].view(M, d), qkv.view(-1)[M * d:2 * M * d].view(M, d), qkv.view(-1)[2 * M * d:3 * M * d].view(M, d)
         cur_T, cur_M, cur_lens = T, M, tlens
         for i, L in enumerate(w.layers):
             Mi, Ti = cur_M, cur_T
-            lpad = (L.kernel - 1) if self.causal else (L.kernel - 1) // 2
             self._ln_split(x, L.ln_ffm, t0p, Mi)
-            self._tc(t0p, d, tw[i, "ffm1"], L.ffm[1], Mi, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn, tag="ffn_w1")
-            self._tc(hidp, w.ffn, tw[i, "ffm2"], L.ffm[3], Mi, d, w.ffn, EPI_RESIDUAL, 0.5, x, d, C=x, ldc=d, tag="ffn_w2")
+            self._ffn_gemms(t0p, tw[i, "ffm1"], L.ffm[1], tw[i, "ffm2"], L.ffm[3], Mi, x, x, 0.5, hidp)
             self._ln_split(x, L.ln_mha, t0p, Mi)
             if L.grouped:
                 wh, wl = tw[i, "qkv"]
@@ -1308,23 +1349,18 @@ class EfficientConformerEngine(ConformerEngine):
             self._tc(t1p, d, tw[i, "wo"], L.bo, Mi, d, d, EPI_RESIDUAL, 1.0, x, d, C=x, ldc=d, tag="out_proj")
             self._ln_split(x, L.ln_conv, t0p, Mi)
             self._tc(t0p, d, tw[i, "pw1"], L.pw1_b, Mi, 2 * d, d, EPI_BIAS_GLU, C=g, ldc=d, tag="pw1_glu")
-            pad_vec = _p(L.glu_pad) if self.causal else None
             if i == self.STRIDE_LAYER:
                 M2 = B * T2
-                self._k("dwconv_ln_silu", "masr_dwconv_ln_silu_strided_f32", _p(g), d, Ti, _p(L.dw), _p(L.dw_b), _p(L.cn[0]),
-                        _p(L.cn[1]), pad_vec, None, _p(t1p[0]), _p(t1p[1]), d, T2, _p(cur_lens), B, d, L.kernel, lpad, 2, T2,
-                        1e-5)
+                self._dwconv(L, g, Ti, cur_lens, B, T2, t1p, stride=2)
                 self._k("avgpool", "masr_avgpool2_time_f32", _p(x), Ti, _p(ws["t0"]), T2, _p(cur_lens), B, T2, d)
                 self._tc(t1p, d, tw[i, "pw2"], L.pw2_b, M2, d, d, EPI_RESIDUAL, 1.0, ws["t0"], d, C=x, ldc=d, tag="pw2")
                 cur_T, cur_M, cur_lens = T2, M2, tlens2
                 Mi, Ti = cur_M, cur_T
             else:
-                self._k("dwconv_ln_silu", "masr_dwconv_ln_silu_f32", _p(g), d, Ti, _p(L.dw), _p(L.dw_b), _p(L.cn[0]),
-                        _p(L.cn[1]), pad_vec, None, _p(t1p[0]), _p(t1p[1]), d, Ti, _p(cur_lens), B, d, L.kernel, lpad, Ti, 1e-5)
+                self._dwconv(L, g, Ti, cur_lens, B, Ti, t1p)
                 self._tc(t1p, d, tw[i, "pw2"], L.pw2_b, Mi, d, d, EPI_RESIDUAL, 1.0, x, d, C=x, ldc=d, tag="pw2")
             self._ln_split(x, L.ln_ff, t0p, Mi)
-            self._tc(t0p, d, tw[i, "ff1"], L.ff[1], Mi, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn, tag="ffn_w1")
-            self._tc(hidp, w.ffn, tw[i, "ff2"], L.ff[3], Mi, d, w.ffn, EPI_RESIDUAL, 0.5, x, d, C=x, ldc=d, tag="ffn_w2")
+            self._ffn_gemms(t0p, tw[i, "ff1"], L.ff[1], tw[i, "ff2"], L.ff[3], Mi, x, x, 0.5, hidp)
             self._ln(x, L.ln_final, x, Mi)
         self._ln(x, w.after_norm, ws["t0"], cur_M)
         self._ln_split(x, w.after_norm, t0p, cur_M)

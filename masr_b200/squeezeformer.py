@@ -12,7 +12,7 @@ from typing import Dict, List
 
 import torch
 
-from ._lib import EPI_BIAS, EPI_BIAS_GLU, EPI_BIAS_SILU, EPI_RESIDUAL
+from ._lib import EPI_BIAS, EPI_BIAS_GLU, EPI_RESIDUAL
 from .engine import ConformerEngine, _p, subsampled_len
 from .weights import check_supported, sinusoid_table
 
@@ -159,12 +159,12 @@ class SqueezeformerEngine(ConformerEngine):
         if gemm != "tc":
             raise ValueError("SqueezeformerEngine implements the tensor-core path only")
         super().__init__(weights_src, streaming, device, max_len, gemm, use_graphs)
-        pe2 = self.w.pe[::2].contiguous()         # reduced-rate blocks see pos_emb[:, ::2] (encoder.py:194)
-        for i, L in enumerate(self.w.layers):
-            if self.REDUCE <= i < self.RECOVER:
-                L.ptab = torch.empty(pe2.shape[0], self.d, device=self.device, dtype=torch.float32)
-                self._gemm(pe2, self.d, L.wpos, None, L.ptab, self.d, pe2.shape[0], self.d, self.d)
-        torch.cuda.synchronize(self.device)
+
+    def _half_rate(self, i: int) -> bool:
+        return self.REDUCE <= i < self.RECOVER    # reduced-rate blocks see pos_emb[:, ::2] (encoder.py:194)
+
+    def _embed_epilogue(self):
+        return EPI_BIAS, 1.0                      # pack_squeezeformer folds the sqrt(d) scale into the embed weight
 
     def _pack(self, sd, max_len):
         return pack_squeezeformer(sd, self.device, max_len)
@@ -197,24 +197,27 @@ class SqueezeformerEngine(ConformerEngine):
                 None if ada is None else _p(ada[0]), None if ada is None else _p(ada[1]), _p(yp[0]), _p(yp[1]), self.d, M,
                 self.d, 1e-5)
 
-    def _encode_tc(self, feats, ws, tl, tlens, B, Fmax, F1, T, M):
+    def _dwconv(self, L, g, g_rows: int, lens, B: int, out_rows: int, out, cached: bool = False, stride: int = 1):
+        """The conv module's depthwise conv + BatchNorm (eval) + SiLU (masr_dwconv_bn_silu_f32) -> the fp16 pair `out`."""
+        assert stride == 1, "the Squeezeformer conv module has no strided form"
+        d = self.d
+        pad, lpad = self._dw_context(L, cached)
+        self._k("dwconv_bn_silu", "masr_dwconv_bn_silu_f32", _p(g), d, g_rows, _p(L.dw), _p(L.dw_b), _p(L.bn[0]), _p(L.bn[1]),
+                pad, None, _p(out[0]), _p(out[1]), d, out_rows, _p(lens), B, d, L.kernel, lpad, out_rows)
+
+    def _encode_tc(self, feats, ws, tl, tlens, B, Fmax, T, M):
         w, d, tw = self.w, self.d, self._tcw
         x, g, qkv, y = ws["x"], ws["g"], ws["qkv"], ws["t1"]        # y: pre-LayerNorm sums
-        t0p, t1p, hidp, c1p, c2p = ws["t0p"], ws["t1p"], self._hidp(ws), ws["c1p"], ws["c2p"]
+        t0p, t1p, hidp = ws["t0p"], ws["t1p"], self._hidp(ws)
         T2 = (T + 1) // 2
         if "tlens2" not in ws:
             ws["tlens2"] = torch.zeros(B, device=self.device, dtype=torch.int32)
             ws["saved"] = torch.empty(max(1, M), d, device=self.device, dtype=torch.float32)
         tlens2, saved = ws["tlens2"], ws["saved"]
         torch.div(tlens + 1, 2, rounding_mode="floor", out=tlens2)
-        self._k("conv1", "masr_conv1_cmvn_relu_planes_f16", _p(feats), _p(w.cmvn_mean), _p(w.cmvn_istd), _p(w.conv1_w),
-                _p(w.conv1_b), _p(c1p[0]), _p(c1p[1]), B, Fmax, w.idim, F1, self.w1_cols, d)
-        self._k("conv2", "masr_conv2_tc_f16x2", _p(c1p[0]), _p(c1p[1]), _p(tw["conv2"][0]), _p(tw["conv2"][1]),
-                _p(w.conv2_b), None, _p(c2p[0]), _p(c2p[1]), B, F1, T, d)
-        self._tc(c2p, self.f2 * d, tw["embed"], w.embed_b, M, d, self.f2 * d, EPI_BIAS, C=y, ldc=d, tag="embed_linear")
+        self._subsample(feats, ws, B, Fmax, T, y)
         # preln -> x (fp32 residual stream) + pair(ada_att0(x))
         self._ln_ada(y, w.preln, x, w.layers[0].att_ada, t0p, M)
-        lpad = (w.kernel - 1) if self.causal else (w.kernel - 1) // 2
         cur_T, cur_M, cur_lens = T, M, tlens
         nl = len(w.layers)
         for i, L in enumerate(w.layers):
@@ -243,20 +246,14 @@ class SqueezeformerEngine(ConformerEngine):
             self._attention_tc(L, qkv, ws["qkvp"], t1p, Ti, cur_lens, B)
             self._tc(t1p, d, tw[i, "wo"], L.bo, Mi, d, d, EPI_RESIDUAL, 1.0, x, d, C=y, ldc=d, tag="out_proj")
             self._ln_ada(y, L.ln1, x, L.ffn1_ada, t0p, Mi)
-            # FFN1
-            self._tc(t0p, d, tw[i, "f1a"], L.ffn1[1], Mi, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn, tag="ffn_w1")
-            self._tc(hidp, w.ffn, tw[i, "f1b"], L.ffn1[3], Mi, d, w.ffn, EPI_RESIDUAL, 1.0, x, d, C=y, ldc=d, tag="ffn_w2")
+            self._ffn_gemms(t0p, tw[i, "f1a"], L.ffn1[1], tw[i, "f1b"], L.ffn1[3], Mi, x, y, 1.0, hidp)
             self._ln_ada(y, L.ln2, x, L.conv_ada, t0p, Mi)
             # conv module
             self._tc(t0p, d, tw[i, "pw1"], L.pw1_b, Mi, 2 * d, d, EPI_BIAS_GLU, C=g, ldc=d, tag="pw1_glu")
-            self._k("dwconv_bn_silu", "masr_dwconv_bn_silu_f32", _p(g), d, Ti, _p(L.dw), _p(L.dw_b), _p(L.bn[0]), _p(L.bn[1]),
-                    _p(L.glu_pad) if self.causal else None, None, _p(t1p[0]), _p(t1p[1]), d, Ti, _p(cur_lens), B, d, L.kernel,
-                    lpad, Ti)
+            self._dwconv(L, g, Ti, cur_lens, B, Ti, t1p)
             self._tc(t1p, d, tw[i, "pw2"], L.pw2_b, Mi, d, d, EPI_RESIDUAL, 1.0, x, d, C=y, ldc=d, tag="pw2")
             self._ln_ada(y, L.ln3, x, L.ffn2_ada, t0p, Mi)
-            # FFN2
-            self._tc(t0p, d, tw[i, "f2a"], L.ffn2[1], Mi, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn, tag="ffn_w1")
-            self._tc(hidp, w.ffn, tw[i, "f2b"], L.ffn2[3], Mi, d, w.ffn, EPI_RESIDUAL, 1.0, x, d, C=y, ldc=d, tag="ffn_w2")
+            self._ffn_gemms(t0p, tw[i, "f2a"], L.ffn2[1], tw[i, "f2b"], L.ffn2[3], Mi, x, y, 1.0, hidp)
             nxt = w.layers[i + 1].att_ada if (i + 1 < nl and i + 1 not in (self.REDUCE, self.RECOVER)) else None
             self._ln_ada(y, L.ln4, x, nxt, t0p, Mi)     # last block: pair(x) feeds the CTC head
         ws["tlens"] = cur_lens

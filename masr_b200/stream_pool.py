@@ -19,7 +19,7 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 import torch
 
-from ._lib import EPI_BIAS, EPI_BIAS_GLU, EPI_BIAS_SCALE, EPI_BIAS_SILU, EPI_RESIDUAL
+from ._lib import EPI_BIAS, EPI_BIAS_GLU, EPI_RESIDUAL
 from .audio import pcm_bytes_to_float32, samples_to_float32
 from .beam import POOL, BeamSearch
 from .engine import ConformerEngine, _p, greedy_score, subsampled_len
@@ -139,6 +139,39 @@ class _PoolBase:
     def _shift(self, x0, x1, rows_per_slot, lorder, row_bytes, cnt_row):
         self.eng._k("stream_shift", "masr_stream_shift_cache", _p(x0), _p(x1), rows_per_slot, lorder, row_bytes, self._m(cnt_row), self.S)
 
+    def _rate(self, half: bool):
+        """(chunk rows per slot, cache rows per slot, `meta` rows of the query count, key count and cache fill) of the blocks
+        at the full or at the halved frame rate."""
+        if half:
+            return CHUNK_OUT // 2, self.cap2, self.QLEN2, self.KLEN2, self.BASE2
+        return CHUNK_OUT, self.cap, self.QLEN, self.KLEN, self.BASE
+
+    def _cached_attention(self, i: int, L, rate, out):
+        """Append the chunk's K|V rows (pair b["qkvp"]) to every slot's layer-i cache, then rel-pos attention of the chunk's
+        queries (b["qkv"]) over [cache ++ chunk] -> the fp16 pair `out`."""
+        eng, d, b = self.eng, self.eng.d, self.b
+        Ci, cap, rq, rk, rb = rate
+        kvh, kvl = self.kv[i]
+        self._append_pair(b["qkvp"], 3 * d, d, 2 * d, (kvh, kvl), cap, rb, rq, Ci)
+        ph, pl, _ = eng._ptab_pair(L)
+        eng._k("attention", "masr_relpos_attention_tc", _p(b["qkv"]), 3 * d, Ci, kvh.data_ptr(), kvl.data_ptr(), kvh.data_ptr() + 2 * d,
+               kvl.data_ptr() + 2 * d, 2 * d, cap, _p(ph), _p(pl), d, _p(L.pos_u), _p(L.pos_v), None, _p(out[0]), _p(out[1]), d, Ci,
+               self._m(rq), self._m(rk), self.S, eng.h, eng.dk, Ci)
+
+    def _cached_conv(self, i: int, L, rate, cache, clen, out, A=None, stride: int = 1):
+        """Conv module middle over every slot's [cache ++ chunk] rows `cache` ([S, kernel - 1 + chunk rows, d]: fp32, or an
+        fp16 pair): pw1 + GLU from the pair `A` (default: `cache` itself), the depthwise stage (in_lens `clen`) -> the fp16
+        pair `out`, then each slot's new left context = the last kernel - 1 valid rows."""
+        eng, d = self.eng, self.eng.d
+        Ci, rq = rate[0], rate[2]
+        lorder = L.kernel - 1
+        g = self.b["g"]
+        x0, x1 = cache if isinstance(cache, tuple) else (cache, None)
+        eng._tc(cache if A is None else A, d, eng._tcw[i, "pw1"], L.pw1_b, self.S * (lorder + Ci), 2 * d, d, EPI_BIAS_GLU, C=g,
+                ldc=d, tag="pw1_glu")
+        eng._dwconv(L, g, lorder + Ci, clen, self.S, Ci // stride, out, cached=True, stride=stride)
+        self._shift(x0, x1, lorder + Ci, lorder, d * x0.element_size(), rq)
+
     def step(self, feats: torch.Tensor, nframes: Sequence[int]):
         """feats [S, 67, 80] raw log-mel (device), nframes[s] = valid feature frames of slot s this round (0 = idle).
         -> (ids [S, OUT_ROWS] int32, maxp [S, OUT_ROWS], valid output frames per slot)."""
@@ -169,15 +202,12 @@ class ConformerStreamPool(_PoolBase):
         nl = len(w.layers)
         S, C = n_slots, CHUNK_OUT
         self.lorder = w.kernel - 1
-        F1 = (CHUNK_FRAMES - 1) // 2
-        TH = (F1 + 1) // 2
         M = S * C
         self.kv = [(torch.zeros(S * self.cap, 2 * d, device=dev, dtype=f16), torch.zeros(S * self.cap, 2 * d, device=dev, dtype=f16))
                    for _ in range(nl)]
         self.xcat = torch.zeros(nl, S, self.lorder + C, d, device=dev, dtype=f32)
         self.b = {
-            "c1p": (torch.zeros(4 * S * TH * 20 * d, device=dev, dtype=f16), torch.zeros(4 * S * TH * 20 * d, device=dev, dtype=f16)),
-            "c2p": (torch.empty(M * eng.f2, d, device=dev, dtype=f16), torch.empty(M * eng.f2, d, device=dev, dtype=f16)),
+            **eng._subsample_planes(S, CHUNK_FRAMES),
             "x": torch.empty(M, d, device=dev, dtype=f32), "t0": torch.empty(M, d, device=dev, dtype=f32),
             "t0p": (torch.empty(M, d, device=dev, dtype=f16), torch.empty(M, d, device=dev, dtype=f16)),
             "t1p": (torch.empty(M, d, device=dev, dtype=f16), torch.empty(M, d, device=dev, dtype=f16)),
@@ -198,51 +228,32 @@ class ConformerStreamPool(_PoolBase):
 
     def _body(self):
         """One batched ``forward_chunk`` over all slots (fixed launch sequence; per-slot lengths come from `meta`)."""
-        eng, S, C, cap = self.eng, self.S, CHUNK_OUT, self.cap
+        eng, S, C = self.eng, self.S, CHUNK_OUT
         w, d, tw, b = eng.w, eng.d, eng._tcw, self.b
-        feats = self.feats_in
-        qlen, klen = self._m(self.QLEN), self._m(self.KLEN)
         M = S * C
-        F1 = (CHUNK_FRAMES - 1) // 2
-        x, t0, t0p, t1p, hidp, qkv, qkvp, g, xcp = b["x"], b["t0"], b["t0p"], b["t1p"], b["hidp"], b["qkv"], b["qkvp"], b["g"], b["xcp"]
+        rate = self._rate(False)
+        x, t0, t0p, t1p, hidp, qkv, qkvp, xcp = b["x"], b["t0"], b["t0p"], b["t1p"], b["hidp"], b["qkv"], b["qkvp"], b["xcp"]
         eng._ln_tmp = t0                              # scratch of eng._ln_split at d = 512: t0 is live only from norm_conv to its copy into xcat
-        eng._k("conv1", "masr_conv1_cmvn_relu_planes_f16", _p(feats), _p(w.cmvn_mean), _p(w.cmvn_istd), _p(w.conv1_w), _p(w.conv1_b),
-               _p(b["c1p"][0]), _p(b["c1p"][1]), S, CHUNK_FRAMES, w.idim, F1, eng.w1_cols, d)
-        eng._k("conv2", "masr_conv2_tc_f16x2", _p(b["c1p"][0]), _p(b["c1p"][1]), _p(tw["conv2"][0]), _p(tw["conv2"][1]), _p(w.conv2_b),
-               None, _p(b["c2p"][0]), _p(b["c2p"][1]), S, F1, C, d)
-        eng._tc(b["c2p"], eng.f2 * d, tw["embed"], w.embed_b, M, d, eng.f2 * d, EPI_BIAS_SCALE, float(d) ** 0.5, C=x, ldc=d)
-        LC = self.lorder + C
+        eng._subsample(self.feats_in, b, S, CHUNK_FRAMES, C, x)
         for i, L in enumerate(w.layers):
             eng._ln_split(x, L.ln_ffm, t0p, M)
-            eng._tc(t0p, d, tw[i, "ffm1"], L.ffm[1], M, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn)
-            eng._tc(hidp, w.ffn, tw[i, "ffm2"], L.ffm[3], M, d, w.ffn, EPI_RESIDUAL, 0.5, x, d, C=x, ldc=d)
+            eng._ffn_gemms(t0p, tw[i, "ffm1"], L.ffm[1], tw[i, "ffm2"], L.ffm[3], M, x, x, 0.5, hidp)
             eng._ln_split(x, L.ln_mha, t0p, M)
             eng._tc(t0p, d, tw[i, "qkv"], L.bqkv, M, 3 * d, d, C=qkv, Cp=qkvp, ldc=3 * d)
-            kvh, kvl = self.kv[i]
-            self._append_pair(qkvp, 3 * d, d, 2 * d, (kvh, kvl), cap, self.BASE, self.QLEN, C)      # new K|V rows -> caches
-            ph, pl, _ = eng._ptab_pair(L)
-            eng._k("attention", "masr_relpos_attention_tc", _p(qkv), 3 * d, C, kvh.data_ptr(), kvl.data_ptr(), kvh.data_ptr() + 2 * d,
-                   kvl.data_ptr() + 2 * d, 2 * d, cap, _p(ph), _p(pl), d, _p(L.pos_u), _p(L.pos_v), None, _p(t1p[0]), _p(t1p[1]), d, C,
-                   qlen, klen, S, eng.h, eng.dk, C)
+            self._cached_attention(i, L, rate, t1p)
             # conv module over [cache ++ chunk] per slot (convolution.py:101-109): t0 <- norm_conv(x + out_proj(att))
             eng._tc(t1p, d, tw[i, "wo"], L.bo, M, d, d, EPI_RESIDUAL, 1.0, x, d, C=x, ldc=d)
             eng._ln(x, L.ln_conv, t0, M)
             xc = self.xcat[i]                                   # [S, 14+16, d]
             xc[:, self.lorder:].copy_(t0.view(S, C, d))
-            eng._k("affine_split", "masr_affine_split_f16", _p(xc), None, None, _p(xcp[0]), _p(xcp[1]), S * LC, d)
-            eng._tc(xcp, d, tw[i, "pw1"], L.pw1_b, S * LC, 2 * d, d, EPI_BIAS_GLU, C=g, ldc=d)
-            eng._k("dwconv_ln_silu", "masr_dwconv_ln_silu_f32", _p(g), d, LC, _p(L.dw), _p(L.dw_b), _p(L.cn[0]), _p(L.cn[1]), None, None,
-                   _p(t1p[0]), _p(t1p[1]), d, C, _p(b["clen"]), S, d, w.kernel, 0, C, 1e-5)
-            # new left context = the last `lorder` VALID rows: rows [n, n+lorder) of [cache ++ chunk], n = valid chunk rows
-            self._shift(xc, None, LC, self.lorder, d * 4, self.QLEN)
+            eng._k("affine_split", "masr_affine_split_f16", _p(xc), None, None, _p(xcp[0]), _p(xcp[1]), S * (self.lorder + C), d)
+            self._cached_conv(i, L, rate, xc, b["clen"], t1p, A=xcp)
             eng._tc(t1p, d, tw[i, "pw2"], L.pw2_b, M, d, d, EPI_RESIDUAL, 1.0, x, d, C=x, ldc=d)
             eng._ln_split(x, L.ln_ff, t0p, M)
-            eng._tc(t0p, d, tw[i, "ff1"], L.ff[1], M, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn)
-            eng._tc(hidp, w.ffn, tw[i, "ff2"], L.ff[3], M, d, w.ffn, EPI_RESIDUAL, 0.5, x, d, C=x, ldc=d)
+            eng._ffn_gemms(t0p, tw[i, "ff1"], L.ff[1], tw[i, "ff2"], L.ff[3], M, x, x, 0.5, hidp)
             eng._ln(x, L.ln_final, x, M)
         eng._ln_split(x, w.after_norm, t0p, M)
-        eng._tc(t0p, d, tw["ctc"], w.ctc_b, M, eng.V, d, C=b["logits"], ldc=eng.Vpad)
-        eng._k("ctc_argmax", "masr_ctc_frame_argmax_f32", _p(b["logits"]), eng.Vpad, M, eng.V, _p(b["ids"]), _p(b["maxp"]), _p(self.probs), eng.V)
+        eng._ctc_argmax(b, M, self.probs)
 
 
 class SqueezeformerStreamPool(_PoolBase):
@@ -269,8 +280,6 @@ class SqueezeformerStreamPool(_PoolBase):
         S, C = n_slots, CHUNK_OUT
         C2 = C // 2
         self.lorder = w.kernel - 1
-        F1 = (CHUNK_FRAMES - 1) // 2
-        TH = (F1 + 1) // 2
         M = S * C
         LC = self.lorder + C
         self.reduced = [eng.REDUCE <= i < eng.RECOVER for i in range(nl)]
@@ -280,8 +289,7 @@ class SqueezeformerStreamPool(_PoolBase):
         self.xcat = [(torch.zeros(S, self.lorder + (C2 if r else C), d, device=dev, dtype=f16),
                       torch.zeros(S, self.lorder + (C2 if r else C), d, device=dev, dtype=f16)) for r in self.reduced]
         self.b = {
-            "c1p": (torch.zeros(4 * S * TH * 20 * d, device=dev, dtype=f16), torch.zeros(4 * S * TH * 20 * d, device=dev, dtype=f16)),
-            "c2p": (torch.empty(M * eng.f2, d, device=dev, dtype=f16), torch.empty(M * eng.f2, d, device=dev, dtype=f16)),
+            **eng._subsample_planes(S, CHUNK_FRAMES),
             "x": torch.zeros(M, d, device=dev, dtype=f32), "y": torch.zeros(M, d, device=dev, dtype=f32),
             "saved": torch.zeros(M, d, device=dev, dtype=f32),
             "t0p": (torch.zeros(M, d, device=dev, dtype=f16), torch.zeros(M, d, device=dev, dtype=f16)),
@@ -307,21 +315,14 @@ class SqueezeformerStreamPool(_PoolBase):
         eng, S, C = self.eng, self.S, CHUNK_OUT
         C2 = C // 2
         w, d, tw, b = eng.w, eng.d, eng._tcw, self.b
-        feats = self.feats_in
         M, M2 = S * C, S * C2
-        F1 = (CHUNK_FRAMES - 1) // 2
-        x, y, saved, t0p, t1p, hidp, qkv, qkvp, g = (b["x"], b["y"], b["saved"], b["t0p"], b["t1p"], b["hidp"], b["qkv"],
-                                                      b["qkvp"], b["g"])
-        eng._k("conv1", "masr_conv1_cmvn_relu_planes_f16", _p(feats), _p(w.cmvn_mean), _p(w.cmvn_istd), _p(w.conv1_w), _p(w.conv1_b),
-               _p(b["c1p"][0]), _p(b["c1p"][1]), S, CHUNK_FRAMES, w.idim, F1, eng.w1_cols, d)
-        eng._k("conv2", "masr_conv2_tc_f16x2", _p(b["c1p"][0]), _p(b["c1p"][1]), _p(tw["conv2"][0]), _p(tw["conv2"][1]), _p(w.conv2_b),
-               None, _p(b["c2p"][0]), _p(b["c2p"][1]), S, F1, C, d)
-        eng._tc(b["c2p"], eng.f2 * d, tw["embed"], w.embed_b, M, d, eng.f2 * d, EPI_BIAS, C=y, ldc=d)
+        x, y, saved, t0p, t1p, hidp, qkv, qkvp = b["x"], b["y"], b["saved"], b["t0p"], b["t1p"], b["hidp"], b["qkv"], b["qkvp"]
+        eng._subsample(self.feats_in, b, S, CHUNK_FRAMES, C, y)
         eng._ln_ada(y, w.preln, x, w.layers[0].att_ada, t0p, M)
         nl = len(w.layers)
-        full = (M, C, self.QLEN, self.KLEN, self.BASE, b["clen"], self.cap)
-        half = (M2, C2, self.QLEN2, self.KLEN2, self.BASE2, b["clen2"], self.cap2)
-        Mi, Ci, rq, rk, rb, clen, cap = full
+        full = (M, b["clen"], self._rate(False))
+        half = (M2, b["clen2"], self._rate(True))
+        Mi, clen, rate = full
         for i, L in enumerate(w.layers):
             if i == eng.REDUCE:
                 saved.copy_(x)
@@ -329,44 +330,32 @@ class SqueezeformerStreamPool(_PoolBase):
                        C2, self._m(self.QLEN), S, C2, int(w.tr_dw.shape[1]), 0, d)
                 eng._tc(t1p, d, tw["tr_pw"], w.tr_pw_b, M2, d, d, EPI_BIAS, C=x, ldc=d)
                 eng._k("affine_split", "masr_affine_split_f16", _p(x), _p(L.att_ada[0]), _p(L.att_ada[1]), _p(t0p[0]), _p(t0p[1]), M2, d)
-                Mi, Ci, rq, rk, rb, clen, cap = half
+                Mi, clen, rate = half
             if i == eng.RECOVER:
                 eng._k("affine_split", "masr_affine_split_f16", _p(x), None, None, _p(t1p[0]), _p(t1p[1]), M2, d)
                 eng._tc(t1p, d, tw["rec"], w.rec_b, M2, d, d, EPI_BIAS, C=y, ldc=d)
                 eng._k("upsample_add", "masr_upsample2_add_f32", _p(saved), _p(y), _p(x), C, C2, S, C, d)
-                Mi, Ci, rq, rk, rb, clen, cap = full
+                Mi, clen, rate = full
                 eng._k("affine_split", "masr_affine_split_f16", _p(x), _p(L.att_ada[0]), _p(L.att_ada[1]), _p(t0p[0]), _p(t0p[1]), Mi, d)
-            LCi = self.lorder + Ci
+            Ci = rate[0]
             # MHA over [cache ++ chunk] keys
             eng._tc(t0p, d, tw[i, "qkv"], L.bqkv, Mi, 3 * d, d, C=qkv, Cp=qkvp, ldc=3 * d)
-            kvh, kvl = self.kv[i]
-            self._append_pair(qkvp, 3 * d, d, 2 * d, (kvh, kvl), cap, rb, rq, Ci)
-            ph, pl, _ = eng._ptab_pair(L)
-            eng._k("attention", "masr_relpos_attention_tc", _p(qkv), 3 * d, Ci, kvh.data_ptr(), kvl.data_ptr(), kvh.data_ptr() + 2 * d,
-                   kvl.data_ptr() + 2 * d, 2 * d, cap, _p(ph), _p(pl), d, _p(L.pos_u), _p(L.pos_v), None, _p(t1p[0]), _p(t1p[1]), d, Ci,
-                   self._m(rq), self._m(rk), S, eng.h, eng.dk, Ci)
+            self._cached_attention(i, L, rate, t1p)
             eng._tc(t1p, d, tw[i, "wo"], L.bo, Mi, d, d, EPI_RESIDUAL, 1.0, x, d, C=y, ldc=d)
             eng._ln_ada(y, L.ln1, x, L.ffn1_ada, t0p, Mi)
-            eng._tc(t0p, d, tw[i, "f1a"], L.ffn1[1], Mi, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn)
-            eng._tc(hidp, w.ffn, tw[i, "f1b"], L.ffn1[3], Mi, d, w.ffn, EPI_RESIDUAL, 1.0, x, d, C=y, ldc=d)
+            eng._ffn_gemms(t0p, tw[i, "f1a"], L.ffn1[1], tw[i, "f1b"], L.ffn1[3], Mi, x, y, 1.0, hidp)
             eng._ln_ada(y, L.ln2, x, L.conv_ada, t0p, Mi)
             # conv module over [cache ++ chunk] per slot
             xh, xl = self.xcat[i]
             xh[:, self.lorder:].copy_(t0p[0][:Mi].view(S, Ci, d))
             xl[:, self.lorder:].copy_(t0p[1][:Mi].view(S, Ci, d))
-            eng._tc((xh, xl), d, tw[i, "pw1"], L.pw1_b, S * LCi, 2 * d, d, EPI_BIAS_GLU, C=g, ldc=d)
-            eng._k("dwconv_bn_silu", "masr_dwconv_bn_silu_f32", _p(g), d, LCi, _p(L.dw), _p(L.dw_b), _p(L.bn[0]), _p(L.bn[1]), None,
-                   None, _p(t1p[0]), _p(t1p[1]), d, Ci, _p(clen), S, d, L.kernel, 0, Ci)
-            # new left context = the last `lorder` VALID rows: rows [n, n + lorder) of [cache ++ chunk], n = valid chunk rows
-            self._shift(xh, xl, LCi, self.lorder, d * 2, rq)
+            self._cached_conv(i, L, rate, (xh, xl), clen, t1p)
             eng._tc(t1p, d, tw[i, "pw2"], L.pw2_b, Mi, d, d, EPI_RESIDUAL, 1.0, x, d, C=y, ldc=d)
             eng._ln_ada(y, L.ln3, x, L.ffn2_ada, t0p, Mi)
-            eng._tc(t0p, d, tw[i, "f2a"], L.ffn2[1], Mi, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn)
             nxt = w.layers[i + 1].att_ada if (i + 1 < nl and i + 1 not in (eng.REDUCE, eng.RECOVER)) else None
-            eng._tc(hidp, w.ffn, tw[i, "f2b"], L.ffn2[3], Mi, d, w.ffn, EPI_RESIDUAL, 1.0, x, d, C=y, ldc=d)
+            eng._ffn_gemms(t0p, tw[i, "f2a"], L.ffn2[1], tw[i, "f2b"], L.ffn2[3], Mi, x, y, 1.0, hidp)
             eng._ln_ada(y, L.ln4, x, nxt, t0p, Mi)           # (last block: pair(x) feeds the CTC head)
-        eng._tc(t0p, d, tw["ctc"], w.ctc_b, M, eng.V, d, C=b["logits"], ldc=eng.Vpad)
-        eng._k("ctc_argmax", "masr_ctc_frame_argmax_f32", _p(b["logits"]), eng.Vpad, M, eng.V, _p(b["ids"]), _p(b["maxp"]), _p(self.probs), eng.V)
+        eng._ctc_argmax(b, M, self.probs)
 
 
 class EfficientConformerStreamPool(_PoolBase):
@@ -394,8 +383,6 @@ class EfficientConformerStreamPool(_PoolBase):
         S, C = n_slots, CHUNK_OUT
         C2 = C // 2
         self.SL = eng.STRIDE_LAYER
-        F1 = (CHUNK_FRAMES - 1) // 2
-        TH = (F1 + 1) // 2
         M = S * C
         self.kv32 = {i: torch.zeros(S * self.cap, 2 * d, device=dev, dtype=f32) for i, L in enumerate(w.layers) if L.grouped}
         self.kv = {i: (torch.zeros(S * (self.cap if i <= self.SL else self.cap2), 2 * d, device=dev, dtype=f16),
@@ -406,8 +393,7 @@ class EfficientConformerStreamPool(_PoolBase):
                      for i, L in enumerate(w.layers)]
         LCmax = max(x[0].shape[1] for x in self.xcat)
         self.b = {
-            "c1p": (torch.zeros(4 * S * TH * 20 * d, device=dev, dtype=f16), torch.zeros(4 * S * TH * 20 * d, device=dev, dtype=f16)),
-            "c2p": (torch.empty(M * eng.f2, d, device=dev, dtype=f16), torch.empty(M * eng.f2, d, device=dev, dtype=f16)),
+            **eng._subsample_planes(S, CHUNK_FRAMES),
             "x": torch.zeros(M, d, device=dev, dtype=f32), "t0": torch.zeros(M, d, device=dev, dtype=f32),
             "t0p": (torch.zeros(M, d, device=dev, dtype=f16), torch.zeros(M, d, device=dev, dtype=f16)),
             "t1p": (torch.zeros(M, d, device=dev, dtype=f16), torch.zeros(M, d, device=dev, dtype=f16)),
@@ -431,26 +417,18 @@ class EfficientConformerStreamPool(_PoolBase):
         eng, S, C = self.eng, self.S, CHUNK_OUT
         C2 = C // 2
         w, d, tw, b = eng.w, eng.d, eng._tcw, self.b
-        feats = self.feats_in
         M, M2 = S * C, S * C2
-        F1 = (CHUNK_FRAMES - 1) // 2
-        x, t0, t0p, t1p, hidp, qkv, qkvp, g, qb, kvn = (b["x"], b["t0"], b["t0p"], b["t1p"], b["hidp"], b["qkv"], b["qkvp"],
-                                                         b["g"], b["qb"], b["kvn"])
-        eng._k("conv1", "masr_conv1_cmvn_relu_planes_f16", _p(feats), _p(w.cmvn_mean), _p(w.cmvn_istd), _p(w.conv1_w), _p(w.conv1_b),
-               _p(b["c1p"][0]), _p(b["c1p"][1]), S, CHUNK_FRAMES, w.idim, F1, eng.w1_cols, d)
-        eng._k("conv2", "masr_conv2_tc_f16x2", _p(b["c1p"][0]), _p(b["c1p"][1]), _p(tw["conv2"][0]), _p(tw["conv2"][1]), _p(w.conv2_b),
-               None, _p(b["c2p"][0]), _p(b["c2p"][1]), S, F1, C, d)
-        eng._tc(b["c2p"], eng.f2 * d, tw["embed"], w.embed_b, M, d, eng.f2 * d, EPI_BIAS_SCALE, float(d) ** 0.5, C=x, ldc=d)
+        x, t0, t0p, t1p, hidp, qkv, qkvp, qb, kvn = (b["x"], b["t0"], b["t0p"], b["t1p"], b["hidp"], b["qkv"], b["qkvp"], b["qb"],
+                                                      b["kvn"])
+        eng._subsample(self.feats_in, b, S, CHUNK_FRAMES, C, x)
         for i, L in enumerate(w.layers):
             half = i > self.SL
-            Mi, Ci = (M2, C2) if half else (M, C)
-            rq, rk, rb = (self.QLEN2, self.KLEN2, self.BASE2) if half else (self.QLEN, self.KLEN, self.BASE)
-            cap = self.cap2 if half else self.cap
+            rate = self._rate(half)
+            Ci, cap, rq, rk, rb = rate
+            Mi = S * Ci
             lorder = L.kernel - 1
-            LCi = lorder + Ci
             eng._ln_split(x, L.ln_ffm, t0p, Mi)
-            eng._tc(t0p, d, tw[i, "ffm1"], L.ffm[1], Mi, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn)
-            eng._tc(hidp, w.ffn, tw[i, "ffm2"], L.ffm[3], Mi, d, w.ffn, EPI_RESIDUAL, 0.5, x, d, C=x, ldc=d)
+            eng._ffn_gemms(t0p, tw[i, "ffm1"], L.ffm[1], tw[i, "ffm2"], L.ffm[3], Mi, x, x, 0.5, hidp)
             eng._ln_split(x, L.ln_mha, t0p, Mi)
             if L.grouped:
                 wh, wl = tw[i, "qkv"]
@@ -463,38 +441,26 @@ class EfficientConformerStreamPool(_PoolBase):
                        eng.GROUP, Ci)
             else:
                 eng._tc(t0p, d, tw[i, "qkv"], L.bqkv, Mi, 3 * d, d, C=qkv, Cp=qkvp, ldc=3 * d)
-                kvh, kvl = self.kv[i]
-                self._append_pair(qkvp, 3 * d, d, 2 * d, (kvh, kvl), cap, rb, rq, Ci)
-                ph, pl, _ = eng._ptab_pair(L)
-                eng._k("attention", "masr_relpos_attention_tc", _p(qkv), 3 * d, Ci, kvh.data_ptr(), kvl.data_ptr(), kvh.data_ptr() + 2 * d,
-                       kvl.data_ptr() + 2 * d, 2 * d, cap, _p(ph), _p(pl), d, _p(L.pos_u), _p(L.pos_v), None, _p(t1p[0]), _p(t1p[1]), d, Ci,
-                       self._m(rq), self._m(rk), S, eng.h, eng.dk, Ci)
+                self._cached_attention(i, L, rate, t1p)
             eng._tc(t1p, d, tw[i, "wo"], L.bo, Mi, d, d, EPI_RESIDUAL, 1.0, x, d, C=x, ldc=d)
             # conv module over [cache ++ chunk] per slot (convolution.py:93-111)
             eng._ln_split(x, L.ln_conv, t0p, Mi)
             xh, xl = self.xcat[i]
             xh[:, lorder:].copy_(t0p[0][:Mi].view(S, Ci, d))
             xl[:, lorder:].copy_(t0p[1][:Mi].view(S, Ci, d))
-            eng._tc((xh, xl), d, tw[i, "pw1"], L.pw1_b, S * LCi, 2 * d, d, EPI_BIAS_GLU, C=g, ldc=d)
             if i == self.SL:
-                eng._k("dwconv_ln_silu", "masr_dwconv_ln_silu_strided_f32", _p(g), d, LCi, _p(L.dw), _p(L.dw_b), _p(L.cn[0]), _p(L.cn[1]),
-                       None, None, _p(t1p[0]), _p(t1p[1]), d, C2, _p(b["clen"]), S, d, L.kernel, 0, 2, C2, 1e-5)
+                self._cached_conv(i, L, rate, (xh, xl), b["clen"], t1p, stride=2)
                 eng._k("avgpool", "masr_avgpool2_time_f32", _p(x), C, _p(t0), C2, self._m(self.QLEN), S, C2, d)
                 Mo, res = M2, t0
             else:
-                eng._k("dwconv_ln_silu", "masr_dwconv_ln_silu_f32", _p(g), d, LCi, _p(L.dw), _p(L.dw_b), _p(L.cn[0]), _p(L.cn[1]), None,
-                       None, _p(t1p[0]), _p(t1p[1]), d, Ci, _p(b["clen"]), S, d, L.kernel, 0, Ci, 1e-5)
+                self._cached_conv(i, L, rate, (xh, xl), b["clen"], t1p)
                 Mo, res = Mi, x
-            # new left context = the last `lorder` VALID rows of [cache ++ chunk]
-            self._shift(xh, xl, LCi, lorder, d * 2, rq)
             eng._tc(t1p, d, tw[i, "pw2"], L.pw2_b, Mo, d, d, EPI_RESIDUAL, 1.0, res, d, C=x, ldc=d)
             eng._ln_split(x, L.ln_ff, t0p, Mo)
-            eng._tc(t0p, d, tw[i, "ff1"], L.ff[1], Mo, w.ffn, d, EPI_BIAS_SILU, Cp=hidp, ldc=w.ffn)
-            eng._tc(hidp, w.ffn, tw[i, "ff2"], L.ff[3], Mo, d, w.ffn, EPI_RESIDUAL, 0.5, x, d, C=x, ldc=d)
+            eng._ffn_gemms(t0p, tw[i, "ff1"], L.ff[1], tw[i, "ff2"], L.ff[3], Mo, x, x, 0.5, hidp)
             eng._ln(x, L.ln_final, x, Mo)
         eng._ln_split(x, w.after_norm, t0p, M2)
-        eng._tc(t0p, d, tw["ctc"], w.ctc_b, M2, eng.V, d, C=b["logits"], ldc=eng.Vpad)
-        eng._k("ctc_argmax", "masr_ctc_frame_argmax_f32", _p(b["logits"]), eng.Vpad, M2, eng.V, _p(b["ids"]), _p(b["maxp"]), _p(self.probs), eng.V)
+        eng._ctc_argmax(b, M2, self.probs)
 
 
 class DeepSpeech2StreamPool(_PoolBase):
