@@ -104,12 +104,14 @@ int masr_conv1_cmvn_relu_f32(const float* feats, const float* mean, const float*
 
 /* Conv2d(C,C,3,2) + ReLU (subsampling.py:83-84) as an implicit GEMM over the channels-last conv-1
  * activation.  w2p [C, 3, 3, C] = reference weight [co,ci,kh,kw] permuted to [co,kh,kw,ci].
- * out [B, T2max, W2, C] (== the [B*T2max, W2*C] input of the `out` linear, subsampling.py:110). */
+ * out [B, T2max, W2, C] (== the [B*T2max, W2*C] input of the `out` linear, subsampling.py:110).
+ * C % 16 == 0; c1, w2p and out 16-byte aligned (128-bit loads and stores). */
 int masr_conv2_s2_relu_f32(const float* c1, const float* w2p, const float* b2, float* out, int B, int F1max,
                            int W1, int T2max, int W2, int C, void* stream);
 
 /* torch.nn.functional.linear / Conv1d(k=1) with a fused epilogue: C[M,N] = epi(A[M,K] . W[N,K]^T).
- * K % 16 == 0, lda % 4 == 0.  For MASR_EPI_BIAS_GLU the weight/bias rows are interleaved
+ * K % 16 == 0, lda % 4 == 0; A, W and C 16-byte aligned (C is written with 128-bit stores when ldc % 4 == 0);
+ * bias may be NULL (no bias).  For MASR_EPI_BIAS_GLU the weight/bias rows are interleaved
  * (row 2j = value j, row 2j+1 = gate j) and C has N/2 columns. */
 int masr_gemm_f32(const float* A, int64_t lda, const float* W, const float* bias, const float* residual,
                   int64_t ldr, float* C, int64_t ldc, int M, int N, int K, int epilogue, float alpha,

@@ -239,6 +239,7 @@ extern "C" int masr_gemm_f32(const float* A, int64_t lda, const float* W, const 
     MASR_REQUIRE(lda % 4 == 0, "masr_gemm_f32: lda=%lld must be a multiple of 4 (128-bit loads)", (long long)lda);
     MASR_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(W) & 15) == 0,
                  "masr_gemm_f32: A and W must be 16-byte aligned");
+    MASR_REQUIRE((reinterpret_cast<uintptr_t>(C) & 15) == 0, "masr_gemm_f32: C must be 16-byte aligned");   // float4 stores
     MASR_REQUIRE(epilogue >= MASR_EPI_BIAS && epilogue <= MASR_EPI_RESIDUAL, "masr_gemm_f32: bad epilogue %d", epilogue);
     MASR_REQUIRE(epilogue != MASR_EPI_RESIDUAL || residual, "masr_gemm_f32: residual epilogue needs a residual");
     MASR_REQUIRE(epilogue != MASR_EPI_BIAS_GLU || N % 4 == 0, "masr_gemm_f32: GLU epilogue needs N %% 4 == 0");
@@ -256,6 +257,9 @@ extern "C" int masr_conv2_s2_relu_f32(const float* c1, const float* w2p, const f
     if (B == 0 || T2max == 0) return MASR_OK;
     MASR_REQUIRE(c1 && w2p && out, "masr_conv2_s2_relu_f32: null pointer");
     MASR_REQUIRE(C % 16 == 0, "masr_conv2_s2_relu_f32: C=%d must be a multiple of 16", C);
+    MASR_REQUIRE((reinterpret_cast<uintptr_t>(c1) & 15) == 0 && (reinterpret_cast<uintptr_t>(w2p) & 15) == 0,
+                 "masr_conv2_s2_relu_f32: c1 and w2p must be 16-byte aligned");
+    MASR_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0, "masr_conv2_s2_relu_f32: out must be 16-byte aligned");
     MASR_REQUIRE(2 * (T2max - 1) + 2 < F1max && 2 * (W2 - 1) + 2 < W1, "masr_conv2_s2_relu_f32: window exceeds input");
     GemmParams p{};
     p.A = c1; p.W = w2p; p.bias = b2; p.C = out;

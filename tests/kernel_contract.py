@@ -71,6 +71,19 @@ def err(out, ref):
     return (out - ref.double()).abs().max().item() if out.numel() else 0.0
 
 
+def gemm_scale(A, W, y):
+    """Per-element float32 error scale of y = A.W^T (+ bias): u * (sqrt(K) * ||a_i o w_j||_2 + |y|), u = 2^-24."""
+    K = A.shape[1]
+    return 2.0 ** -24 * (math.sqrt(K) * torch.sqrt((A.double() ** 2) @ (W.double() ** 2).t()) + y.abs())
+
+
+def ratio(out, ref, scale):
+    """max |out - ref| / scale over the valid block; the kernel output must be finite."""
+    out = out.detach().double().cpu()
+    assert torch.isfinite(out).all(), "non-finite kernel output in a valid row"
+    return ((out - ref) / scale).abs().max().item() if out.numel() else 0.0
+
+
 def report(name, **errs):
     print(f"[max error] {name}: " + ", ".join(f"{k}={v:.3g}" for k, v in errs.items()))
 

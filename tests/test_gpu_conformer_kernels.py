@@ -17,7 +17,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from kernel_contract import P, assert_pair_reconstructs, err, garbage, nan, pair_value, relpos_reference, report, runtime
+from kernel_contract import (P, assert_pair_reconstructs, err, garbage, gemm_scale, nan, pair_value, ratio, relpos_reference,
+                             report, runtime)
 
 pytestmark = pytest.mark.gpu
 
@@ -196,19 +197,6 @@ def test_relpos_attention_tc5_uses_at_most_256_keys(rt):
 
 
 # ---- tensor-core GEMM family -----------------------------------------------------------------------------------------------
-
-def gemm_scale(A, W, y):
-    """Per-element float32 error scale of y = A.W^T (+ bias): u * (sqrt(K) * ||a_i o w_j||_2 + |y|)."""
-    K = A.shape[1]
-    return U32 * (math.sqrt(K) * torch.sqrt((A.double() ** 2) @ (W.double() ** 2).t()) + y.abs())
-
-
-def ratio(out, ref, scale):
-    """max |out - ref| / scale over the valid block; the kernel output must be finite."""
-    out = out.detach().double().cpu()
-    assert torch.isfinite(out).all(), "non-finite kernel output in a valid row"
-    return ((out - ref) / scale).abs().max().item()
-
 
 def rup(n, m):
     return (n + m - 1) // m * m
