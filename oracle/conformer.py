@@ -178,7 +178,7 @@ def get_encoder_out_chunk(sd, cfg, feats_chunk: torch.Tensor, st: ChunkState, re
     chunk = x.shape[1]
     cache_t1 = 0 if st.att_cache is None else st.att_cache.shape[2]
     key_size = cache_t1 + chunk
-    pe = sinusoid_table(cfg)
+    pe = sinusoid_table(cfg).to(x.dtype)           # (float32 table; the input's dtype so a float64 run stays float64)
     pos_emb = pe[None, st.offset - cache_t1: st.offset - cache_t1 + key_size]
     if required_cache_size < 0:
         start = 0

@@ -175,7 +175,7 @@ def get_encoder_out_chunk(sd, cfg: EfficientConfig, feats_chunk: torch.Tensor, s
     chunk = x.shape[1]
     cache_t1 = 0 if st.att_cache is None else st.att_cache.shape[2]
     key_size = cache_t1 + chunk
-    pos_emb = oc.sinusoid_table(cfg)[None, offset - cache_t1: offset - cache_t1 + key_size]
+    pos_emb = oc.sinusoid_table(cfg).to(x.dtype)[None, offset - cache_t1: offset - cache_t1 + key_size]
     if required_cache_size < 0:
         start = 0
     elif required_cache_size == 0:

@@ -188,7 +188,7 @@ def get_encoder_out_chunk(sd, cfg: SqueezeformerConfig, feats_chunk: torch.Tenso
     chunk = x.shape[1]
     cache_t1 = 0 if st.att_cache is None else st.att_cache.shape[2]
     key_size = cache_t1 + chunk
-    pe = oc.sinusoid_table(oc.ConformerConfig(d_model=cfg.d_model, max_len=cfg.max_len))
+    pe = oc.sinusoid_table(oc.ConformerConfig(d_model=cfg.d_model, max_len=cfg.max_len)).to(x.dtype)
     pos_emb = pe[None, st.offset - cache_t1: st.offset - cache_t1 + key_size]
     if required_cache_size < 0:
         start = 0
