@@ -6,8 +6,9 @@ unpinned: ``pip install paddlespeech_ctcdecoders -U``, docs/beam_search.md:5) pl
 time (:19-25).  Neither the library, its source nor the LM exist in /root/reference or in this image, and no reference
 test pins its results, so this restatement follows the algorithm's *public definition* (DeepSpeech2-style prefix beam
 search, SURVEY.md Appendix D) with the parameters MASR passes (beam_size=300, cutoff_prob=0.99, cutoff_top_n=40,
-blank_id=0, configs/conformer.yml:74-88) and scorer=None.  It is validated only against itself: beam=1 on one-hot
-posteriors == greedy, score monotonicity, and exact agreement with the CUDA implementation.
+blank_id=0, configs/conformer.yml:74-88) and scorer=None.  It is validated against itself (beam=1 on one-hot posteriors ==
+greedy, score monotonicity, exact agreement with the CUDA implementation) and against a float64 CTC forward: where no live
+prefix is pruned, every beam entry's score equals the forward of its prefix to 2.0e-7 (tests/test_gpu_beam_contract.py).
 
 Definition used (log domain, natural log):
   per frame  : candidates = the tokens, sorted by probability (descending, ties by lower id), of the shortest prefix of
@@ -36,7 +37,8 @@ NEG_INF = -float("inf")
 # log(exp(a) + exp(b)) with the SAME rounding at every step.  libm's / CUDA's expf, log1pf differ in the last bit, so the
 # function is defined here operation by operation (one correctly rounded float32 +, -, *, / or round-to-nearest-even per
 # line; no fused multiply-add) and csrc/beam.cu evaluates exactly this sequence with __fmul_rn / __fadd_rn / __fdiv_rn.
-# Accuracy: a few ulp — irrelevant for the search; determinism is the point.
+# Accuracy against float64 (tests/test_gpu_beam_contract.py): exp32_det 4 ulp and log1p32_det 3.2 ulp relative, logaddexp32
+# 1 ulp of 1 + |result| — irrelevant for the search; determinism is the point.
 _F = np.float32
 _LOG2E, _LN2_HI, _LN2_LO = _F(1.4426950408889634), _F(0.693145751953125), _F(1.42860682030941723212e-6)
 _EXP_C = [_F(1.0 / 720.0), _F(1.0 / 120.0), _F(1.0 / 24.0), _F(1.0 / 6.0), _F(0.5), _F(1.0), _F(1.0)]
