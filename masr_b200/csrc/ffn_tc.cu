@@ -32,6 +32,12 @@
 //   kernel (C7514 / C7518) when MMAs are in flight across the chunk loop's back-edge.
 //   The second H buffer costs the ring its fourth stage, too few to hide HBM latency when the weights are cold, so each CTA
 //   first prefetches its share of the weights into L2 (cp.async.bulk.prefetch).
+//   Clusters of 2 CTAs: cluster c owns row blocks 2 c + rank, then steps by 2 x clusters (both CTAs run the same number of
+//   row blocks; one past the last row block of an odd count, a CTA runs the schedule on the last block's rows and stores
+//   nothing).  Every CTA loads its own X K-blocks; each W1 / W2 K-block is loaded once per cluster, each CTA issuing half of
+//   its rows with a TMA multicast into the same stage of both CTAs, so the weights cross L2 once per two row blocks.  A
+//   stage is refilled only when the consumers of both CTAs have released it: every consumer warp arrives on the empty
+//   barrier of both CTAs (16 arrivals).  The K-block order does not depend on data, so both CTAs walk the same sequence.
 //   Shared memory: ring 3 x 32 KB | H 2 x 32 KB | running sum 64 x 256 fp32 = 64 KB | mbarriers  (= 224 KB + alignment)
 //   Registers per consumer thread: 32 + 32 (phase A) + 64 + 64 (phase B) accumulators.
 #include <cuda.h>
@@ -54,6 +60,7 @@ constexpr int F_STAGE_BYTES = 32768;           // phase A: Xh, Xl (4 KB each) + 
 constexpr int F_H_BYTES = FM * FHC * 2 * 2;    // one H buffer, a hidden chunk as (h, l): [K-block][h / l] 64 x 32 tiles of 4 KB
 constexpr int F_SUM_BYTES = FM * FD * 4;       // running fp32 sum of the finished 256-chunks (each thread: its own elements)
 constexpr int F_THREADS = 384;
+constexpr int F_CLUSTER = 2;                   // CTAs per cluster, sharing each weight K-block
 constexpr int F_PRODUCER_REGS = 40, F_CONSUMER_REGS = 232;
 constexpr uint32_t F_TX_A = 2 * FM * FBK * 2 + 2 * FHC * FBK * 2;   // 24 KB
 constexpr uint32_t F_TX_B = 2 * FD * FBK * 2;                       // 32 KB
@@ -63,8 +70,8 @@ static_assert(F_PRODUCER_REGS * 128 + F_CONSUMER_REGS * 256 <= 65536, "register 
 
 struct FfnMaps {
     CUtensorMap xh, xl;       // [M, 256], box 32 x 64
-    CUtensorMap w1h, w1l;     // [F, 256], box 32 x 128
-    CUtensorMap w2h, w2l;     // [256, F], box 32 x 256
+    CUtensorMap w1h, w1l;     // [F, 256], box 32 x 64: half of a W1 K-block, one per CTA of the cluster
+    CUtensorMap w2h, w2l;     // [256, F], box 32 x 128: half of a W2 K-block
 };
 
 struct FfnParams {
@@ -115,12 +122,16 @@ __global__ void __launch_bounds__(F_THREADS, 1) ffn_tc_kernel(const __grid_const
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nrb = (p.M + FM - 1) / FM;
     const int nch = p.F / FHC;                 // hidden chunks per row block (even: F % 256 == 0)
-    // chunk g % nch of row block blockIdx.x + (g / nch) gridDim.x
+    // 1-D grid of (F_CLUSTER, 1, 1) clusters: the CTA's rank in its cluster is blockIdx.x % F_CLUSTER.  Row block
+    // pair * F_CLUSTER + rank for pair = cluster, cluster + clusters, ...: the same trip count in both CTAs.
+    const uint32_t rank = blockIdx.x % F_CLUSTER;
+    const int cluster = blockIdx.x / F_CLUSTER, clusters = gridDim.x / F_CLUSTER;
+    const int npairs = (nrb + F_CLUSTER - 1) / F_CLUSTER;
 
     if (warp == 8 && lane == 0) {
         tma_prefetch_desc(&maps.xh); tma_prefetch_desc(&maps.xl); tma_prefetch_desc(&maps.w1h);
         tma_prefetch_desc(&maps.w1l); tma_prefetch_desc(&maps.w2h); tma_prefetch_desc(&maps.w2l);
-        for (int s = 0; s < F_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
+        for (int s = 0; s < F_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8 * F_CLUSTER); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         // Every CTA reads all of the weights, chunk by chunk, and they come cold from HBM in a model step.  Each CTA
         // prefetches its 1 / gridDim share of them into L2 at once (no kernel writes them, so before griddepcontrol.wait),
@@ -133,7 +144,7 @@ __global__ void __launch_bounds__(F_THREADS, 1) ffn_tc_kernel(const __grid_const
                 asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;"
                              ::"l"(static_cast<const uint8_t*>(p.w[t]) + off), "r"(min(share, wbytes - off)) : "memory");
     }
-    __syncthreads();
+    cluster_sync();                            // both CTAs' barriers are initialised before either multicasts into the other
     pdl_wait();
     pdl_launch_dependents();
 
@@ -150,8 +161,10 @@ __global__ void __launch_bounds__(F_THREADS, 1) ffn_tc_kernel(const __grid_const
                 ++kg;
                 return s;
             };
-            auto load_a = [&](int m0, int j) {          // A(j): X rows m0.., W1 rows 128 j ..
-                const int n0 = j * FHC;
+            constexpr uint16_t both = (1u << F_CLUSTER) - 1;
+            // A(j): X rows m0.. (this CTA), W1 rows 128 j + 64 rank .. (both CTAs; the peer issues the other 64)
+            auto load_a = [&](int m0, int j) {
+                const int n0 = j * FHC + (FHC / F_CLUSTER) * rank;
 #pragma unroll 1
                 for (int kb = 0; kb < FD / FBK; ++kb) {
                     const uint32_t s = acquire(F_TX_A);
@@ -159,21 +172,24 @@ __global__ void __launch_bounds__(F_THREADS, 1) ffn_tc_kernel(const __grid_const
                     uint8_t* st = smem + s * F_STAGE_BYTES;
                     tma_load_2d(&maps.xh, &full_bar[s], st, kb * FBK, m0);
                     tma_load_2d(&maps.xl, &full_bar[s], st + 4096, kb * FBK, m0);
-                    tma_load_2d(&maps.w1h, &full_bar[s], st + 8192, kb * FBK, n0);
-                    tma_load_2d(&maps.w1l, &full_bar[s], st + 16384, kb * FBK, n0);
+                    tma_load_2d_multicast(&maps.w1h, &full_bar[s], st + 8192 + 4096 * rank, kb * FBK, n0, both);
+                    tma_load_2d_multicast(&maps.w1l, &full_bar[s], st + 16384 + 4096 * rank, kb * FBK, n0, both);
                 }
             };
-            for (int rb = blockIdx.x; rb < nrb; rb += gridDim.x) {
-                load_a(rb * FM, 0);
+            for (int pair = cluster; pair < npairs; pair += clusters) {
+                // a CTA past the last row block loads the last one's rows again, and its consumers store nothing
+                const int m0 = min(pair * F_CLUSTER + (int)rank, nrb - 1) * FM;
+                load_a(m0, 0);
                 for (int j = 0; j < nch; ++j) {
-                    if (j + 1 < nch) load_a(rb * FM, j + 1);
+                    if (j + 1 < nch) load_a(m0, j + 1);
 #pragma unroll 1
-                    for (int kb = 0; kb < FHC / FBK; ++kb) {    // B(j): W2 [256 rows, hidden 128 j + 32 kb ..]
+                    for (int kb = 0; kb < FHC / FBK; ++kb) {    // B(j): W2 [rows 128 rank.., hidden 128 j + 32 kb ..]
                         const uint32_t s = acquire(F_TX_B);
                         if (no_loads) continue;
                         uint8_t* st = smem + s * F_STAGE_BYTES;
-                        tma_load_2d(&maps.w2h, &full_bar[s], st, j * FHC + kb * FBK, 0);
-                        tma_load_2d(&maps.w2l, &full_bar[s], st + F_STAGE_BYTES / 2, j * FHC + kb * FBK, 0);
+                        const int k0 = j * FHC + kb * FBK, r0 = (FD / F_CLUSTER) * rank;
+                        tma_load_2d_multicast(&maps.w2h, &full_bar[s], st + 8192 * rank, k0, r0, both);
+                        tma_load_2d_multicast(&maps.w2l, &full_bar[s], st + F_STAGE_BYTES / 2 + 8192 * rank, k0, r0, both);
                     }
                 }
             }
@@ -187,9 +203,11 @@ __global__ void __launch_bounds__(F_THREADS, 1) ffn_tc_kernel(const __grid_const
         const uint32_t h_base = smem_u32(hbuf);
         const uint32_t sum_base = smem_u32(sum) + wg * (F_SUM_BYTES / 2) + tid * 8;
         const uint32_t is_lane0 = lane == 0;
+        // the stage is free for the producers of both CTAs, whose multicasts write it in both
+        const uint32_t empty0 = cluster_map(smem_u32(empty_bar), 0), empty1 = cluster_map(smem_u32(empty_bar), 1);
         auto release = [&](uint32_t s) {
-            asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}"
-                         ::"r"(smem_u32(&empty_bar[s])), "r"(is_lane0) : "memory");
+            mbar_arrive_cluster(empty0 + 8 * s, is_lane0);
+            mbar_arrive_cluster(empty1 + 8 * s, is_lane0);
         };
         float acc1[32], cor1[32], acc2[64], cor2[64];
         uint32_t kg = 0;
@@ -337,7 +355,8 @@ __global__ void __launch_bounds__(F_THREADS, 1) ffn_tc_kernel(const __grid_const
         };
 
 #pragma unroll 1
-        for (int rb = blockIdx.x; rb < nrb; rb += gridDim.x) {
+        for (int pair = cluster; pair < npairs; pair += clusters) {
+            const int rb = pair * F_CLUSTER + (int)rank;             // rb == nrb: no rows, write_out stores nothing
             // prologue: A(0), its epilogue into H[0], A(1) (nch >= 2).  The previous row block's last chunks have drained,
             // and the barrier below is passed by both warpgroups before either writes H[1] again.
             phase_a(0, FD / FBK);
@@ -377,7 +396,7 @@ __global__ void __launch_bounds__(F_THREADS, 1) ffn_tc_kernel(const __grid_const
             }
         }
     }
-    __syncthreads();
+    cluster_sync();                            // the peer's consumers may still arrive on this CTA's empty barriers
 }
 
 // [rows, K] fp16 row-major (ld elements), box = 32 (K) x box_rows, 64-byte swizzle, zero OOB fill
@@ -396,6 +415,7 @@ int ffn_map(CUtensorMap* map, const void* ptr, int64_t rows, int64_t K, int64_t 
 }
 
 bool g_ffn_attr_set[64] = {false};
+int g_ffn_clusters[64][2] = {};                // clusters resident at once, per device, for ffn_tc_kernel<false / true>
 
 }  // namespace
 
@@ -422,10 +442,10 @@ extern "C" int masr_ffn_tc_f16x2(const void* Ah, const void* Al, int64_t lda, co
     int rc;
     if ((rc = ffn_map(&maps.xh, Ah, M, D, lda, FM))) return rc;
     if ((rc = ffn_map(&maps.xl, Al, M, D, lda, FM))) return rc;
-    if ((rc = ffn_map(&maps.w1h, W1h, F, D, D, FHC))) return rc;
-    if ((rc = ffn_map(&maps.w1l, W1l, F, D, D, FHC))) return rc;
-    if ((rc = ffn_map(&maps.w2h, W2h, D, F, F, FD))) return rc;
-    if ((rc = ffn_map(&maps.w2l, W2l, D, F, F, FD))) return rc;
+    if ((rc = ffn_map(&maps.w1h, W1h, F, D, D, FHC / F_CLUSTER))) return rc;
+    if ((rc = ffn_map(&maps.w1l, W1l, F, D, D, FHC / F_CLUSTER))) return rc;
+    if ((rc = ffn_map(&maps.w2h, W2h, D, F, F, FD / F_CLUSTER))) return rc;
+    if ((rc = ffn_map(&maps.w2l, W2l, D, F, F, FD / F_CLUSTER))) return rc;
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) dev = 0;
@@ -437,13 +457,37 @@ extern "C" int masr_ffn_tc_f16x2(const void* Ah, const void* Al, int64_t lda, co
         }
         g_ffn_attr_set[dev] = true;
     }
-    int sms = 0;
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
-    const int nrb = (M + FM - 1) / FM;
     const char* env = getenv("MASR_FFN_FLAGS");   // profiling switches only (FFN_NO_*); unset or 0 in normal use
     const int flags = env ? atoi(env) : 0;
+    const int kind = flags ? 1 : 0;
+    cudaLaunchConfig_t cfg = {};
+    cfg.blockDim = dim3(F_THREADS);
+    cfg.dynamicSmemBytes = kFfnSmem;
+    cudaLaunchAttribute attr[2];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = F_CLUSTER;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[1].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    if (!g_ffn_clusters[dev][kind]) {
+        // one CTA per SM, and a GPC with an odd number of SMs leaves one of them out of every pairing: ask the driver
+        cfg.gridDim = dim3(F_CLUSTER);
+        int n = 0;
+        const cudaError_t e = cudaOccupancyMaxActiveClusters(&n, kernels[kind], &cfg);
+        if (e != cudaSuccess || n <= 0) {
+            set_last_error("ffn_tc: no cluster of %d CTAs fits (%s)", F_CLUSTER, cudaGetErrorString(e));
+            return e != cudaSuccess ? (int)e : MASR_ERR_INTERNAL;
+        }
+        g_ffn_clusters[dev][kind] = n;
+    }
+    const int npairs = ((M + FM - 1) / FM + F_CLUSTER - 1) / F_CLUSTER;
     FfnParams p{{W1h, W1l, W2h, W2l}, b1, b2, x, ldx, M, F, alpha, flags};
-    const dim3 grid(nrb < sms ? nrb : sms);
-    launch_pdl(kernels[flags ? 1 : 0], grid, dim3(F_THREADS), kFfnSmem, (cudaStream_t)stream, maps, p);
+    cfg.gridDim = dim3(F_CLUSTER * (npairs < g_ffn_clusters[dev][kind] ? npairs : g_ffn_clusters[dev][kind]));
+    cfg.stream = (cudaStream_t)stream;
+    cfg.numAttrs = pdl_enabled() ? 2 : 1;
+    cudaLaunchKernelEx(&cfg, kernels[kind], maps, p);
     return check_launch("ffn_tc_kernel");
 }

@@ -36,6 +36,25 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* ba
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
+// The same box into smem_dst of every CTA of the cluster in cta_mask; each destination CTA's mbarrier at bar's offset
+// receives the box's bytes
+__device__ __forceinline__ void tma_load_2d_multicast(const CUtensorMap* map, uint64_t* bar, void* smem_dst, int c0, int c1,
+                                                      uint16_t cta_mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+        " [%0], [%1, {%3, %4}], [%2], %5;"
+        ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask) : "memory");
+}
+// shared::cluster address of the variable at shared::cta address a in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t cluster_map(uint32_t a, uint32_t rank) {
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(a), "r"(rank));
+    return r;
+}
+// every thread of every CTA of the cluster: prior memory accesses (mbarrier inits included) visible cluster-wide
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
@@ -126,6 +145,14 @@ __device__ __forceinline__ void split_f16x2(float x0, float x1, __half2& h, __ha
 
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+// arrive on the mbarrier at shared::cluster address a (cluster_map), in this CTA or another of the cluster, if pred != 0;
+// predicated rather than branched so that a warp stays converged around its wgmmas.  Default (CTA-scope) release: the
+// arrive only has to follow reads that wgmma.wait_group has already completed, and a cluster-scope release compiles to
+// MEMBAR.ALL.GPU before every arrive.
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t a, uint32_t pred) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cluster.b64 _, [%0];\n\t}"
+                 ::"r"(a), "r"(pred) : "memory");
 }
 
 // explicit shared-space accesses: through a generic pointer these compile to generic LD.E/ST.E, whose

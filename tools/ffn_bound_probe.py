@@ -2,7 +2,8 @@
 the profiling switches of MASR_FFN_FLAGS — 1: no TMA loads (the MMAs run on stale stages), 2: no MMAs, 4: no hidden
 epilogue (no bias / SiLU / split / store of H) — and their combinations.  Outputs are garbage under the switches; only the
 timings mean something.  20 launches in a CUDA graph, best of 5 replays.  Prints us per launch, the bytes each launch
-streams from L2 (X, W1 and W2 pairs once per hidden chunk of every row block, from the shapes) and the implied rate.
+streams from L2 (X pairs once per hidden chunk of every row block, W1 and W2 pairs once per hidden chunk of every 2-CTA
+cluster's row-block pair, which the TMA multicast delivers to both CTAs; from the shapes) and the implied rate.
 AB_LIB=path loads another build of the library; PROBE_WSETS=20 gives every launch its own weights, cold in HBM."""
 import json
 import os
@@ -74,7 +75,8 @@ def run(s):
 
 
 nrb, nch = (M + FM - 1) // FM, F // FHC
-l2_bytes = nrb * nch * (FM * D + FHC * D + D * FHC) * 4          # h and l halves of X, W1 and W2 K-blocks per chunk
+npairs = (nrb + 1) // 2
+l2_bytes = nch * (nrb * FM * D + npairs * (FHC * D + D * FHC)) * 4   # h and l halves of X, W1 and W2 K-blocks per chunk
 mma_flop = 3 * 2 * M * 2 * D * F
 row = {"lib": os.environ.get("AB_LIB", "in-tree"), "gpu": torch.cuda.get_device_name(), "M": M, "F": F, "weight_sets": WSETS,
        "l2_bytes_per_launch": l2_bytes}
