@@ -514,6 +514,21 @@ int masr_ctc_prefix_beam_wordlm_pool(const int* cand_id, const float* cand_logp,
                                      int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int* fresh, int* out_tok,
                                      int64_t tok_stride, int* out_n, float* out_score, float* out_approx, void* stream);
 
+/* The silero VAD network (16 kHz branch of silero_vad.onnx, weights packed by masr_b200/silero.py) over one recording
+ * of n_samples 16 kHz samples in windows of `window` samples (512, 1024 or 1536; the last window zero-padded),
+ * T = window / 512 recurrent steps per window, N = ceil(n_samples / window) windows.
+ * masr_silero_vad_layout: floats[0..3] = float32 counts of the STFT basis, the packed encoder and recurrence buffers,
+ * and the gate-input row (256) per step.
+ * masr_silero_vad_encode_f32: every window in parallel, reflect pad -> STFT -> magnitude / log -> adaptive
+ * normalisation -> first_layer -> encoder -> gates_x[N*T][256] = W_ih1 x + (Wb1 + Rb1) (gate rows i, f, g, o).
+ * masr_silero_vad_recur_f32: one CTA runs both LSTM layers (state zero at the start) over all N*T steps, then the
+ * decoder: logits[N*T] (workspace), probs[N] = mean over each window's steps of sigmoid(logit). */
+int masr_silero_vad_layout(int64_t* floats);
+int masr_silero_vad_encode_f32(const float* audio, int64_t n_samples, int window, const float* basis, const float* enc,
+                               float* gates_x, void* stream);
+int masr_silero_vad_recur_f32(const float* gates_x, int64_t n_windows, int window, const float* rec, float* logits,
+                              float* probs, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -247,15 +247,15 @@ class MASRPredictor:
 
     def init_vad(self, vad_predictor=None, vad_model_path=None):
         """predict.py:139-142.  ``vad_predictor``: any object with the reference's ``get_speech_timestamps(samples,
-        sampling_rate)``; else the silero ONNX model at ``vad_model_path`` through onnxruntime (masr_b200.vad.SileroVAD)."""
+        sampling_rate)``; else the silero ONNX model at ``vad_model_path``, run on the GPU (masr_b200.vad.GpuSileroVAD)."""
         if vad_predictor is not None:
             self.vad_predictor = vad_predictor
         elif getattr(self, "vad_predictor", None) is None:
             if vad_model_path is None:
                 raise Exception("masr_b200: predict_long needs a VAD: pass vad_predictor=... (an object with "
-                                "get_speech_timestamps) or vad_model_path=<silero_vad.onnx> (needs onnxruntime)")
-            from .vad import SileroVAD
-            self.vad_predictor = SileroVAD(vad_model_path)
+                                "get_speech_timestamps) or vad_model_path=<silero_vad.onnx>")
+            from .vad import GpuSileroVAD
+            self.vad_predictor = GpuSileroVAD(vad_model_path, device=self.predictor.device)
 
     def predict_long(self, audio_data, use_pun=False, is_itn=False, sample_rate=16000, vad_predictor=None, vad_model_path=None):
         """Long-form recognition (predict.py:195-234): VAD segments -> recognise -> join with '，' and average the scores.

@@ -1,17 +1,20 @@
 """Long-form recognition support (SURVEY.md §8 f4): the segmentation half of ``MASRPredictor.predict_long``.
 
 The reference runs the silero VAD network (an ONNX model shipped next to masr/infer_utils/vad_predictor.py, evaluated with
-onnxruntime on the CPU, 512-sample windows) and turns its per-window speech probabilities into speech segments with a
-hysteresis state machine (vad_predictor.py:106-175).  The network is a third-party model and stays what it is in the
-reference — an ONNX session on the host (``SileroVAD``, needs ``onnxruntime`` and the model file; neither is part of this
-image).  The state machine is restated here (``speech_timestamps_from_probs``) and pinned to the reference's own
-implementation by tests/golden/vad_timestamps_golden.json; any object with the reference's
-``get_speech_timestamps(samples, sampling_rate)`` method can be plugged into ``MASRPredictor.predict_long``.
-The recognition half is where the GPU path changes the picture: all segments of a recording go through ONE batched pass
-(``predict_batch``) instead of the reference's one-``predict``-per-segment loop (predict.py:216-224).
+onnxruntime on the CPU, one 512-sample window per session call) and turns its per-window speech probabilities into
+speech segments with a hysteresis state machine (vad_predictor.py:106-175).  Here the network runs on the GPU
+(``GpuSileroVAD``): the model file is read and packed by ``masr_b200.silero``, one launch encodes every window of the
+recording in parallel and one persistent single-CTA launch runs the LSTM across all windows (csrc/vad.cu).
+``SileroVAD`` keeps the reference's onnxruntime form for hosts that have it.  The state machine is restated here
+(``speech_timestamps_from_probs``) and pinned to the reference's own implementation by
+tests/golden/vad_timestamps_golden.json; any object with the reference's ``get_speech_timestamps(samples,
+sampling_rate)`` method can be plugged into ``MASRPredictor.predict_long``.
+The recognition half then sends all segments of a recording through ONE batched pass (``predict_batch``) instead of the
+reference's one-``predict``-per-segment loop (predict.py:216-224).
 """
 from __future__ import annotations
 
+import ctypes as C
 from typing import Dict, List, Sequence
 
 import numpy as np
@@ -118,3 +121,71 @@ class SileroVAD(ProbabilityVAD):
                                               "sr": np.array(sr, dtype=np.int64)})
             out.append(float(np.asarray(o).item()))
         return out
+
+
+class GpuSileroVAD(ProbabilityVAD):
+    """The reference's VADPredictor with the silero network on the GPU (csrc/vad.cu): the model file's 16 kHz branch is
+    checked and packed once (``masr_b200.silero``), then each recording costs two launches, the window-parallel encoder
+    and the single-CTA recurrence, whatever its length.  ``window_size_samples`` is 512, 1024 or 1536."""
+
+    def __init__(self, path: str, device="cuda", **kw):
+        import torch
+        from . import _lib, silero
+        super().__init__(self._probs, **kw)
+        W = self.kw["window_size_samples"]
+        if W not in (512, 1024, 1536):
+            raise ValueError(f"window_size_samples = {W}: the 16 kHz silero network takes 512, 1024 or 1536")
+        if not torch.cuda.is_available():
+            raise _lib.MasrB200Error("GpuSileroVAD needs a CUDA device (there is no CPU fallback)")
+        packed = silero.load_silero_16k(path)
+        sizes = (C.c_int64 * 4)()
+        _lib.call("masr_silero_vad_layout", sizes)
+        want = {"basis": sizes[0], "enc": sizes[1], "rec": sizes[2]}
+        for k, n in want.items():
+            if packed[k].size != n:
+                raise _lib.MasrB200Error(f"packed silero buffer {k} has {packed[k].size} floats, the kernels read {n}")
+        self.gate_width = int(sizes[3])
+        self.device = torch.device(device)
+        self.weights = {k: torch.from_numpy(v).to(self.device) for k, v in packed.items()}
+
+    def _stream(self):
+        import torch
+        return torch.cuda.current_stream(self.device).cuda_stream
+
+    def encode(self, samples):
+        """Layer-1 LSTM gate inputs ``W_ih1 x + b1`` [N * T, 256] (rows i, f, g, o) of 16 kHz ``samples`` (a float32
+        array or CUDA tensor)."""
+        import torch
+        from . import _lib
+        x = torch.as_tensor(samples, dtype=torch.float32).to(self.device).contiguous()
+        W = self.kw["window_size_samples"]
+        n_windows = (x.numel() + W - 1) // W
+        gx = torch.empty(n_windows * (W // 512), self.gate_width, dtype=torch.float32, device=self.device)
+        _lib.call("masr_silero_vad_encode_f32", x.data_ptr(), x.numel(), W, self.weights["basis"].data_ptr(),
+                  self.weights["enc"].data_ptr(), gx.data_ptr(), self._stream())
+        return gx
+
+    def recur(self, gx):
+        """Per-window speech probabilities [N] from the gate inputs of ``encode`` (CUDA tensor)."""
+        import torch
+        from . import _lib
+        W = self.kw["window_size_samples"]
+        T = W // 512
+        gx = gx.contiguous()
+        n_windows = gx.shape[0] // T
+        logits = torch.empty(gx.shape[0], dtype=torch.float32, device=self.device)
+        probs = torch.empty(n_windows, dtype=torch.float32, device=self.device)
+        _lib.call("masr_silero_vad_recur_f32", gx.data_ptr(), n_windows, W, self.weights["rec"].data_ptr(),
+                  logits.data_ptr(), probs.data_ptr(), self._stream())
+        return probs
+
+    def _probs(self, audio: np.ndarray, sr: int):
+        if sr != 16000 and sr % 16000 == 0:
+            audio, sr = audio[::sr // 16000], 16000
+        if sr == 8000:
+            raise ValueError("GpuSileroVAD runs the silero network's 16 kHz branch only; resample 8 kHz audio to 16 kHz")
+        if sr != 16000:
+            raise ValueError("Supported sampling rates: [8000, 16000] (or multiply of 16000)")
+        if len(audio) == 0:
+            return []
+        return self.recur(self.encode(np.ascontiguousarray(audio, np.float32))).cpu().numpy().tolist()
