@@ -158,11 +158,12 @@ int masr_conv2_tc_f16x2(const void* c1h, const void* c1l, const void* Wh, const 
 /* fp32 -> fp16 (h, l) pair, elementwise over n contiguous values. */
 int masr_split_f16(const float* x, void* h, void* l, int64_t n, void* stream);
 
-/* torch.nn.LayerNorm(D, eps) over the last dimension (encoder.py:64-72; convolution.py:66). */
+/* torch.nn.LayerNorm(D, eps) over the last dimension (encoder.py:64-72; convolution.py:66).  D = 256, 512, 1024, 2048 or 4096
+ * (4096: the bidirectional DeepSpeech2 at rnn_size 2048, deepspeech2/encoder.py:34). */
 int masr_layernorm_f32(const float* x, int64_t ldx, const float* gamma, const float* beta, float* y, int64_t ldy,
                        int M, int D, float eps, void* stream);
 
-/* LayerNorm writing the fp16 (h, l) operand pair of masr_gemm_tc_f16x2 instead of fp32.  D = 256, 1024 or 2048 (a 512-wide
+/* LayerNorm writing the fp16 (h, l) operand pair of masr_gemm_tc_f16x2 instead of fp32.  D = 256, 1024, 2048 or 4096 (a 512-wide
  * row goes through masr_layernorm_f32 + masr_split_f16, which write the same pair). */
 int masr_layernorm_split_f16(const float* x, int64_t ldx, const float* gamma, const float* beta, void* yh, void* yl,
                              int64_t ldy, int M, int D, float eps, void* stream);
@@ -301,6 +302,26 @@ int masr_gru_step_f32(const float* gates_x, int64_t ldg, int64_t bstride, const 
 int masr_gru_seq_f32(const float* gates_x, int64_t ldg, int64_t bstride, const float* Whh, const float* h0_T, float* hN_T,
                      const float* bhn, float* out, void* outh, void* outl, int64_t ld_out, int col_off, const int* lens, int B,
                      int H, int T, int reverse, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* The persistent recurrences of masr_lstm_seq_f32 / masr_gru_seq_f32 at H = 2048 (encoder_conf.rnn_size: 2048, the large-
+ * data size of configs/deepspeech2.yml; encoder.py:36-45, gru.py:6-22), on the tensor cores: W_hh . h_{t-1} by mma.sync
+ * m16n8k16 in the FP16x2 split of masr_gemm_tc_f16x2 (fp32 accumulators), the cell in fp32.  One CTA per 16 hidden units
+ * (H / 16 = 128 CTAs, all co-resident, a grid barrier per step); part of each CTA's weight slice stays in shared memory, the
+ * rest is streamed from L2 on every step.  Same arguments and semantics as the fp32 forms (ragged lengths, both directions,
+ * h0_T == hN_T allowed, c_state in place, fp32 and/or pair output at col_off) except:
+ *   Whh_packed: W_hh [G*H, H] packed once by masr_rnn_tc_pack_f16x2 (G = 4 for the LSTM, 3 for the GRU; G*H*H*4 bytes);
+ *   workspace:  masr_rnn_seq_tc_workspace_bytes(B, H).
+ * H = 2048 only.  Fails with MASR_ERR_INVALID_ARGUMENT, launching nothing, when the grid cannot be resident at once. */
+int masr_rnn_seq_tc_workspace_bytes(int B, int H, int64_t* bytes);
+int masr_rnn_tc_pack_f16x2(const float* Whh, void* packed, int G, int H, void* stream);
+int masr_lstm_seq_tc_f16x2(const float* gates_x, int64_t ldg, int64_t bstride, const void* Whh_packed, const float* h0_T,
+                           float* hN_T, float* c_state, float* out, void* outh, void* outl, int64_t ld_out, int col_off,
+                           const int* lens, int B, int H, int T, int reverse, void* workspace, int64_t workspace_bytes,
+                           void* stream);
+int masr_gru_seq_tc_f16x2(const float* gates_x, int64_t ldg, int64_t bstride, const void* Whh_packed, const float* h0_T,
+                          float* hN_T, const float* bhn, float* out, void* outh, void* outl, int64_t ld_out, int col_off,
+                          const int* lens, int B, int H, int T, int reverse, void* workspace, int64_t workspace_bytes,
+                          void* stream);
 
 /* ---- batched chunk (streaming) state ------------------------------------------------------------ */
 

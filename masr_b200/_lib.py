@@ -88,6 +88,10 @@ SIGNATURES = {
     "masr_lstm_seq_f32": [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _vp, _i, _i, _i, _i, _vp, _i64, _vp],
     "masr_gru_step_f32": [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _vp, _i, _i, _i, _i, _vp],
     "masr_gru_seq_f32": [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _vp, _i, _i, _i, _i, _vp, _i64, _vp],
+    "masr_rnn_seq_tc_workspace_bytes": [_i, _i, C.POINTER(_i64)],
+    "masr_rnn_tc_pack_f16x2": [_vp, _vp, _i, _i, _vp],
+    "masr_lstm_seq_tc_f16x2": [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _vp, _i, _i, _i, _i, _vp, _i64, _vp],
+    "masr_gru_seq_tc_f16x2": [_vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _vp, _i, _i, _i, _i, _vp, _i64, _vp],
     "masr_stream_append_rows": [_vp, _vp, _i64, _i64, _i, _vp, _vp, _i64, _i64, _vp, _vp, _i, _i, _vp],
     "masr_stream_shift_cache": [_vp, _vp, _i64, _i, _i, _vp, _i, _vp],
     "masr_ctc_frame_argmax_f32": [_vp, _i64, _i, _i, _vp, _vp, _vp, _i64, _vp],

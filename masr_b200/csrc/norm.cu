@@ -172,8 +172,9 @@ extern "C" int masr_layernorm_f32(const float* x, int64_t ldx, const float* gamm
         case 512: launch_pdl(layernorm_kernel<512, false>, grid, dim3(256), 0, st, x, ldx, gamma, beta, y, nullptr, nullptr, ldy, M, eps, (const float*)nullptr, (const float*)nullptr); break;
         case 1024: launch_pdl(layernorm_kernel<1024, false>, grid, dim3(256), 0, st, x, ldx, gamma, beta, y, nullptr, nullptr, ldy, M, eps, (const float*)nullptr, (const float*)nullptr); break;
         case 2048: launch_pdl(layernorm_kernel<2048, false>, grid, dim3(256), 0, st, x, ldx, gamma, beta, y, nullptr, nullptr, ldy, M, eps, (const float*)nullptr, (const float*)nullptr); break;
+        case 4096: launch_pdl(layernorm_kernel<4096, false>, grid, dim3(256), 0, st, x, ldx, gamma, beta, y, nullptr, nullptr, ldy, M, eps, (const float*)nullptr, (const float*)nullptr); break;
         default:
-            set_last_error("masr_layernorm_f32: unsupported width D=%d (256/512/1024/2048)", D);
+            set_last_error("masr_layernorm_f32: unsupported width D=%d (256/512/1024/2048/4096)", D);
             return MASR_ERR_INVALID_ARGUMENT;
     }
     return check_launch("layernorm_kernel");
@@ -191,8 +192,9 @@ extern "C" int masr_layernorm_split_f16(const float* x, int64_t ldx, const float
         case 256: launch_pdl(layernorm_kernel<256, true>, grid, dim3(256), 0, st, x, ldx, gamma, beta, nullptr, (__half*)yh, (__half*)yl, ldy, M, eps, (const float*)nullptr, (const float*)nullptr); break;
         case 1024: launch_pdl(layernorm_kernel<1024, true>, grid, dim3(256), 0, st, x, ldx, gamma, beta, nullptr, (__half*)yh, (__half*)yl, ldy, M, eps, (const float*)nullptr, (const float*)nullptr); break;
         case 2048: launch_pdl(layernorm_kernel<2048, true>, grid, dim3(256), 0, st, x, ldx, gamma, beta, nullptr, (__half*)yh, (__half*)yl, ldy, M, eps, (const float*)nullptr, (const float*)nullptr); break;
+        case 4096: launch_pdl(layernorm_kernel<4096, true>, grid, dim3(256), 0, st, x, ldx, gamma, beta, nullptr, (__half*)yh, (__half*)yl, ldy, M, eps, (const float*)nullptr, (const float*)nullptr); break;
         default:
-            set_last_error("masr_layernorm_split_f16: unsupported width D=%d (256/1024/2048)", D);
+            set_last_error("masr_layernorm_split_f16: unsupported width D=%d (256/1024/2048/4096)", D);
             return MASR_ERR_INVALID_ARGUMENT;
     }
     return check_launch("layernorm_kernel<split>");

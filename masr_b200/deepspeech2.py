@@ -1,9 +1,10 @@
 """DeepSpeech2 engine (configs/deepspeech2.yml; masr/model_utils/deepspeech2/{conv,encoder,model}.py):
-CMVN -> Conv2d(1,32,3,2)+ReLU -> Conv2d(32,32,3,2)+ReLU -> 5 x [LSTM(1024) or GRU(1024) (use_gru), uni (streaming) / bi ->
-LayerNorm] -> CTC.
+CMVN -> Conv2d(1,32,3,2)+ReLU -> Conv2d(32,32,3,2)+ReLU -> 5 x [LSTM(H) or GRU(H) (use_gru), uni (streaming) / bi ->
+LayerNorm] -> CTC, H = encoder_conf.rnn_size (1024; 2048 for large data).
 
-Input projections and the CTC head are tensor-core GEMMs (FP16x2 split); the first projection (K = 608) and the
-recurrence run on the fp32 FMA pipe, one persistent launch per layer and direction (or one launch per time step).
+Input projections and the CTC head are tensor-core GEMMs (FP16x2 split); the first projection (K = 608) runs on the fp32
+FMA pipe.  The recurrence is one persistent launch per layer and direction: on the fp32 FMA pipe up to H = 1024, on the
+tensor cores (FP16x2 split) at H = 2048; with MASR_LSTM_PERSISTENT=0, or at other widths, one launch per time step.
 Whole-utterance batches and the chunked streaming path with carried state (inference_predictor.py:66-78: (h, c) for the
 LSTM, h for the GRU) are both implemented.  The cell type comes from the weights, as in the reference."""
 from __future__ import annotations
@@ -18,6 +19,8 @@ import torch
 from . import _lib
 from ._lib import EPI_BIAS, call
 from .engine import ConformerEngine, _p, subsampled_len
+
+TC_HIDDEN = 2048      # the width of the tensor-core persistent recurrence (masr_{lstm,gru}_seq_tc_f16x2)
 
 
 @dataclass
@@ -132,6 +135,30 @@ class DeepSpeech2Engine(ConformerEngine):
         self.G = self.w.gates
         self._seq_fn, self._step_fn = (("masr_gru_seq_f32", "masr_gru_step_f32") if self.w.cell == "gru" else
                                        ("masr_lstm_seq_f32", "masr_lstm_step_f32"))
+        self._seq_tc_fn = f"masr_{self.w.cell}_seq_tc_f16x2"
+        if self.H == TC_HIDDEN:
+            self._pack_rnn_tc()
+
+    @property
+    def rnn_form(self) -> str:
+        """Which recurrence kernel runs: the fp32 persistent one ("seq", W_hh slices resident in shared memory) up to
+        H = 1024, the tensor-core persistent one ("seq_tc", W_hh partly resident, partly streamed from L2 every step) at
+        H = 2048, and one launch per time step ("step") at any other width or with ``persistent_lstm`` off."""
+        H = self.H
+        if not self.persistent_lstm:
+            return "step"
+        return "seq" if H % 128 == 0 and H <= 1024 else "seq_tc" if H == TC_HIDDEN else "step"
+
+    def _pack_rnn_tc(self):
+        """W_hh of every layer and direction in the fragment order of the tensor-core recurrence (masr_rnn_tc_pack_f16x2)."""
+        for l, ent in enumerate(self.w.rnn):
+            packed = []
+            for whh in ent["whh"]:
+                buf = torch.empty(whh.numel() * 4, device=self.device, dtype=torch.uint8)
+                call("masr_rnn_tc_pack_f16x2", _p(whh), _p(buf), self.G, self.H, self._stream())
+                packed.append(buf)
+            self._tcw[l, "whh_tc"] = packed
+        torch.cuda.synchronize(self.device)
 
     def _pack(self, sd, max_len):
         return pack_deepspeech2(sd, self.device)
@@ -195,7 +222,7 @@ class DeepSpeech2Engine(ConformerEngine):
                     c = None if stream.c is None else stream.c[l]
                 # the cell's per-unit operand: the LSTM's cell state c [B][H] (updated in place), the GRU's b_hn [H]
                 aux = ent["bhn"][di] if w.cell == "gru" else c
-                if self.persistent_lstm and H % 128 == 0 and H <= 1024:
+                if self.rnn_form == "seq":
                     # the whole recurrence of this layer / direction in one persistent launch (W_hh slices resident in shared memory).
                     # The state is updated in place (h0_T == hN_T), so it never changes buffers: a captured pool step reads in the
                     # next replay what it wrote in this one.
@@ -205,6 +232,15 @@ class DeepSpeech2Engine(ConformerEngine):
                         ws["lstm_ws"] = torch.empty(nbytes.value, device=self.device, dtype=torch.uint8)
                     self._k(f"{w.cell}_seq", self._seq_fn, _p(gx), GH, T, _p(ent["whh"][di]), _p(hT[cur]), _p(hT[cur]), _p(aux),
                             _p(out), None, None, D, di * H, _p(tlens), B, H, T, di, _p(ws["lstm_ws"]), ws["lstm_ws"].numel())
+                elif self.rnn_form == "seq_tc":
+                    # the same in-place persistent launch on the tensor cores (H = 2048)
+                    if ws.get("rnn_tc_ws") is None:
+                        nbytes = _lib.C.c_int64(0)
+                        call("masr_rnn_seq_tc_workspace_bytes", B, H, _lib.C.byref(nbytes))
+                        ws["rnn_tc_ws"] = torch.empty(nbytes.value, device=self.device, dtype=torch.uint8)
+                    self._k(f"{w.cell}_seq", self._seq_tc_fn, _p(gx), GH, T, _p(self._tcw[l, "whh_tc"][di]), _p(hT[cur]),
+                            _p(hT[cur]), _p(aux), _p(out), None, None, D, di * H, _p(tlens), B, H, T, di, _p(ws["rnn_tc_ws"]),
+                            ws["rnn_tc_ws"].numel())
                 else:
                     for s in range(T):
                         self._k(f"{w.cell}_step", self._step_fn, _p(gx), GH, T, _p(ent["whh"][di]), _p(hT[cur]), _p(hT[1 - cur]),

@@ -475,8 +475,10 @@ class DeepSpeech2StreamPool(_PoolBase):
     put across rounds, as a CUDA graph replay needs: the persistent recurrence updates it in place, and the per-step form
     (``MASR_LSTM_PERSISTENT=0``) ping-pongs 16 times per round, so it ends where it started.
 
-    The persistent recurrence needs all its H / 8 CTAs co-resident (a grid barrier per step).  The pool launches on the
-    engine's stream like every other engine call; do not run its steps on a second stream beside another persistent launch.
+    The persistent recurrences need all their CTAs co-resident (a grid barrier per step): H / 8 for the fp32 form at
+    H <= 1024, H / 16 = 128 with 216 KiB of shared memory each for the tensor-core form at H = 2048 (the host checks the
+    occupancy and refuses to launch a grid that cannot be resident).  The pool launches on the engine's stream like every
+    other engine call; do not run its steps on a second stream beside another persistent launch.
 
     There is no position table and the state has a constant size, so a greedy slot decodes any length; with a beam search
     attached, `max_frames` sizes each slot's prefix trie and bounds the slot.  A short chunk may be followed by more."""

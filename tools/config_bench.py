@@ -6,7 +6,7 @@ per-GPU shard of every BASELINE.json config that is not the headline — one JSO
     config 4lm / 4plm / 5lm  the same beam-search configs with a synthetic character 5-gram ARPA LM (alpha 2.2, beta 4.3, the
               shipped configs' values; a few million n-grams, generated into a temporary directory on first use)
     plus      squeezeformer.yml / deepspeech2.yml whole-utterance, 32 x 10 s, ctc_greedy; deepspeech2gru the same with
-              encoder_conf.use_gru: True (GRU recurrences)
+              encoder_conf.use_gru: True (GRU recurrences); deepspeech2wide: rnn_size 2048, LSTM and GRU, uni and bi
 Numbers printed here are dev measurements (CUDA-synchronised wall clock around the public engine call), not bench values."""
 import json
 import os
@@ -182,3 +182,15 @@ sdn = synth.deepspeech2_state_dict(0, use_gru=True)
 e = DeepSpeech2Engine(sdn, streaming=True)
 run("deepspeech2gru deepspeech2.yml use_gru=True 32x10s ctc_greedy (whole utterance)", e, tens, lambda w: e.transcribe(w),
     oracle=greedy_oracle(odg, synth.to_torch(sdn), ods.DS2Config()), sample=(0,))
+for use_gru in (False, True):         # encoder_conf.rnn_size: 2048 (tensor-core persistent recurrence), uni and bi
+    for streaming in (True, False):
+        if not want("deepspeech2wide"):
+            break
+        del e
+        torch.cuda.empty_cache()
+        sdn = synth.deepspeech2_state_dict(0, streaming=streaming, hidden=2048, use_gru=use_gru)
+        e = DeepSpeech2Engine(sdn, streaming=streaming)
+        run(f"deepspeech2wide deepspeech2.yml rnn_size=2048 use_gru={use_gru} streaming={streaming} 32x10s ctc_greedy "
+            "(whole utterance)", e, tens, lambda w: e.transcribe(w), reps=3,
+            oracle=greedy_oracle(odg if use_gru else ods, synth.to_torch(sdn), ods.DS2Config(hidden=2048, bidirectional=not streaming)),
+            sample=(0,))
