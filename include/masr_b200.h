@@ -543,12 +543,18 @@ int masr_ctc_prefix_beam_wordlm_pool(const int* cand_id, const float* cand_logp,
  * masr_silero_vad_encode_f32: every window in parallel, reflect pad -> STFT -> magnitude / log -> adaptive
  * normalisation -> first_layer -> encoder -> gates_x[N*T][256] = W_ih1 x + (Wb1 + Rb1) (gate rows i, f, g, o).
  * masr_silero_vad_recur_f32: one CTA runs both LSTM layers (state zero at the start) over all N*T steps, then the
- * decoder: logits[N*T] (workspace), probs[N] = mean over each window's steps of sigmoid(logit). */
+ * decoder: logits[N*T] (workspace), probs[N] = mean over each window's steps of sigmoid(logit).
+ * masr_silero_vad_recur_slots_f32: one CTA per slot; slot s runs windows [win_off[s], win_off[s+1]) of gates_x
+ * (win_off: device int32 [n_slots + 1], non-decreasing from 0) from its carried state[s] = (h1, c1, h2, c2), each [64],
+ * writes probs[w] for each of those windows (logits as above, same rows) and the final state back to state[s].  A
+ * slot without windows is not touched; with every state zero and one slot it computes masr_silero_vad_recur_f32. */
 int masr_silero_vad_layout(int64_t* floats);
 int masr_silero_vad_encode_f32(const float* audio, int64_t n_samples, int window, const float* basis, const float* enc,
                                float* gates_x, void* stream);
 int masr_silero_vad_recur_f32(const float* gates_x, int64_t n_windows, int window, const float* rec, float* logits,
                               float* probs, void* stream);
+int masr_silero_vad_recur_slots_f32(const float* gates_x, const int32_t* win_off, int n_slots, int window, const float* rec,
+                                    float* state, float* logits, float* probs, void* stream);
 
 #ifdef __cplusplus
 }

@@ -49,6 +49,7 @@ SIGNATURES = {
     "masr_silero_vad_layout": [C.POINTER(_i64)],
     "masr_silero_vad_encode_f32": [_vp, _i64, _i, _vp, _vp, _vp, _vp],
     "masr_silero_vad_recur_f32": [_vp, _i64, _i, _vp, _vp, _vp, _vp],
+    "masr_silero_vad_recur_slots_f32": [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp],
     "masr_fbank_workspace_bytes": [_i, _i64, C.POINTER(_i64)],
     "masr_wave_gain_f32": [_vp, _vp, _i, _i64, _f, _f, _vp, _vp, _vp, _vp],
     "masr_fbank_f32": [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp],

@@ -277,9 +277,13 @@ __device__ __forceinline__ float lstm_cell(const float* g, int j, float& c) {
     return o * tanhf(c);
 }
 
-__global__ void __launch_bounds__(kRecThreads, 1)
-vad_recur_kernel(const float* __restrict__ gx, int64_t steps, int T, const float* __restrict__ p,
-                 float* __restrict__ logits, float* __restrict__ probs) {
+// The recurrence over `steps` steps of one sequence.  kResume = false: from a zero state, nothing written back (the
+// whole-recording kernel).  kResume = true: from state = [h1, c1, h2, c2] (4 x 64 floats), and after the last step has
+// gone through both layers the final state is written back there.
+template <bool kResume>
+__device__ __forceinline__ void vad_recur_body(const float* __restrict__ gx, int64_t steps, int T,
+                                               const float* __restrict__ p, float* __restrict__ logits,
+                                               float* __restrict__ probs, float* __restrict__ state) {
     __shared__ __align__(16) float h1[kVadH];
     __shared__ __align__(16) float h2[kVadH];
     __shared__ float g1[kVadGates];
@@ -297,8 +301,18 @@ vad_recur_kernel(const float* __restrict__ gx, int64_t steps, int T, const float
     }
     const float b2 = __ldg(p + kB2 + r);
     const float dw0 = __ldg(p + kDecW + (tid & 31)), dw1 = __ldg(p + kDecW + 32 + (tid & 31)), db = __ldg(p + kDecB);
-    if (tid < kVadH) h1[tid] = h2[tid] = 0.f;
     float c = 0.f;                                     // c1 of unit tid (tid < 64) or c2 of unit tid - 64 (tid < 128)
+    if constexpr (kResume) {
+        if (tid < kVadH) {
+            h1[tid] = state[tid];
+            h2[tid] = state[2 * kVadH + tid];
+            c = state[kVadH + tid];
+        } else if (tid < 2 * kVadH) {
+            c = state[3 * kVadH + tid - kVadH];
+        }
+    } else {
+        if (tid < kVadH) h1[tid] = h2[tid] = 0.f;
+    }
     float g_next = (half == 0) ? __ldg(gx + r) : 0.f;
     __syncthreads();
 
@@ -347,6 +361,15 @@ vad_recur_kernel(const float* __restrict__ gx, int64_t steps, int T, const float
         v = warp_sum(v);
         if (l == 0) logits[steps - 1] = v + db;
     }
+    if constexpr (kResume) {                           // h1, c1 after step steps - 1 (layer 1 idles in the last iteration),
+        if (tid < kVadH) {                             // h2, c2 after the last iteration
+            state[tid] = h1[tid];
+            state[kVadH + tid] = c;
+            state[2 * kVadH + tid] = h2[tid];
+        } else if (tid < 2 * kVadH) {
+            state[3 * kVadH + tid - kVadH] = c;
+        }
+    }
     __syncthreads();
     // decoder sigmoid and the mean over each window's T steps
     const int64_t n_windows = steps / T;
@@ -355,6 +378,26 @@ vad_recur_kernel(const float* __restrict__ gx, int64_t steps, int T, const float
         for (int k = 0; k < T; ++k) acc += sigmoid_f(logits[n * T + k]);
         probs[n] = acc / (float)T;
     }
+}
+
+// One CTA: the whole recording from a zero state.
+__global__ void __launch_bounds__(kRecThreads, 1)
+vad_recur_kernel(const float* __restrict__ gx, int64_t steps, int T, const float* __restrict__ p,
+                 float* __restrict__ logits, float* __restrict__ probs) {
+    vad_recur_body<false>(gx, steps, T, p, logits, probs, nullptr);
+}
+
+// One CTA per slot: slot b = blockIdx.x runs windows [win_off[b], win_off[b + 1]) of gx (and of logits / probs) from its
+// carried state[b] and writes the state back.  A slot without windows returns at once and leaves its state untouched.
+// The CTAs share nothing, so any number of slots runs in waves.
+__global__ void __launch_bounds__(kRecThreads, 1)
+vad_recur_slots_kernel(const float* __restrict__ gx, const int32_t* __restrict__ win_off, int T,
+                       const float* __restrict__ p, float* __restrict__ state, float* __restrict__ logits,
+                       float* __restrict__ probs) {
+    const int b = blockIdx.x;
+    const int64_t w0 = win_off[b], nw = (int64_t)win_off[b + 1] - w0;
+    if (nw <= 0) return;
+    vad_recur_body<true>(gx + w0 * T * kVadGates, nw * T, T, p, logits + w0 * T, probs + w0, state + b * 4 * kVadH);
 }
 
 }  // namespace masr
@@ -401,4 +444,17 @@ extern "C" int masr_silero_vad_recur_f32(const float* gates_x, int64_t n_windows
     const int T = window / 512;
     vad_recur_kernel<<<1, kRecThreads, 0, (cudaStream_t)stream>>>(gates_x, n_windows * T, T, rec, logits, probs);
     return check_launch("vad_recur_kernel");
+}
+
+extern "C" int masr_silero_vad_recur_slots_f32(const float* gates_x, const int32_t* win_off, int n_slots, int window,
+                                               const float* rec, float* state, float* logits, float* probs,
+                                               void* stream) {
+    MASR_REQUIRE(gates_x && win_off && rec && state && logits && probs,
+                 "masr_silero_vad_recur_slots_f32: null pointer");
+    MASR_REQUIRE(vad_window_ok(window), "masr_silero_vad_recur_slots_f32: window = %d is not one of 512, 1024, 1536",
+                 window);
+    MASR_REQUIRE(n_slots > 0, "masr_silero_vad_recur_slots_f32: n_slots = %d", n_slots);
+    vad_recur_slots_kernel<<<n_slots, kRecThreads, 0, (cudaStream_t)stream>>>(gates_x, win_off, window / 512, rec, state,
+                                                                                logits, probs);
+    return check_launch("vad_recur_slots_kernel");
 }

@@ -364,16 +364,25 @@ class MASRPredictor:
             raise Exception("masr_b200: inverse text normalisation (is_itn) is outside the hot-path scope")
         return {'text': text, 'score': score}
 
-    def create_stream_pool(self, n_slots: int, max_frames: int = 3000):
+    def create_stream_pool(self, n_slots: int, max_frames: int = 3000, vad_model_path=None, vad_options=None):
         """Additive: a ``StreamPool`` of ``n_slots`` concurrent streams over this predictor's model, decoding as the YAML
         says — greedy, or the GPU prefix beam search with the character or word LM this predictor loaded (if any).  Each slot's
         ``push`` results equal ``predict_stream`` on that stream alone.  ``max_frames``: encoder frames one stream may reach
-        before it must be reset (40 ms each; 3000 = 2 minutes)."""
+        before it must be reset (40 ms each; 3000 = 2 minutes).
+
+        ``vad_model_path`` (the silero VAD model file): instead a ``SegmentingStreamPool`` over that pool, which cuts every
+        slot's live stream into utterances with ``GpuSileroVAD(vad_model_path, **vad_options)`` and decodes each one as a
+        fresh ``predict_stream`` (masr_b200/segment_pool.py), so a stream may run for any length."""
         if not self.configs.streaming:
             raise Exception(f"不支持改该模型流式识别，当前模型：{self.configs.use_model}，参数streaming为：{self.configs.streaming}")
         from .stream_pool import StreamPool
-        return StreamPool(self.predictor, self._text_featurizer.vocab_list, n_slots, use_db_normalization=self._use_db,
+        pool = StreamPool(self.predictor, self._text_featurizer.vocab_list, n_slots, use_db_normalization=self._use_db,
                           target_db=self._target_db, max_frames=max_frames, beam=self._beam_conf, resample=self._resample)
+        if vad_model_path is None:
+            return pool
+        from .segment_pool import SegmentingStreamPool
+        from .vad import GpuSileroVAD
+        return SegmentingStreamPool(pool, GpuSileroVAD(vad_model_path, device=self.predictor.device, **(vad_options or {})))
 
     def reset_stream(self):
         """predict.py:346-353."""
