@@ -120,7 +120,10 @@ int masr_gemm_f32(const float* A, int64_t lda, const float* W, const float* bias
 /* Tensor-core (wgmma/TMA) variant of masr_gemm_f32 with fp32-grade results: operands are fp16
  * (h, l) pairs, h = fp16(x), l = fp16((x - h) * 2^11) (masr_split_f16); C ~= Ah.Wh^T + 2^-11 (Ah.Wl^T + Al.Wh^T)
  * accumulated in fp32.  Output: fp32 C and/or the (Ch, Cl) pair the next GEMM consumes (either may be NULL,
- * not both).  K % 64 == 0, lda % 8 == 0, ldc % 8 == 0 (ldc % 4 when only fp32 is written); W is [N, K] dense. */
+ * not both).  Accuracy (the masr_split_f16 operand range): |C - A.W^T| <= c * (u (sqrt(K) |a_i o w_j| + |C|) +
+ * 2^-36 sqrt(K) (|a_i| + |w_j|)), u = 2^-24, the second term being the pairs' absolute floor; c < 8 is asserted with operand
+ * scales 2^-16 .. 2^12, and without the floor term where both scales are >= 2^-8 (DESIGN.md, precision policy).  An operand pair at +-inf (|x| >= 65520) makes its output row / column
+ * NaN in every epilogue (ReLU keeps NaN) and leaves every other output unchanged.  K % 64 == 0, lda % 8 == 0, ldc % 8 == 0 (ldc % 4 when only fp32 is written); W is [N, K] dense. */
 int masr_gemm_tc_f16x2(const void* Ah, const void* Al, int64_t lda, const void* Wh, const void* Wl,
                        const float* bias, const float* residual, int64_t ldr, float* C, void* Ch, void* Cl,
                        int64_t ldc, int M, int N, int K, int epilogue, float alpha, void* stream);
@@ -138,6 +141,9 @@ int masr_ffn_tc_f16x2(const void* Ah, const void* Al, int64_t lda, const void* W
 /* CTC head without the [M, V] logits: ctc_lo Linear (loss/ctc.py:70) with a GEMM epilogue that keeps, per frame and per
  * 32-column group, (max logit, first argmax, sum exp(x - max)), then a combine kernel -> per-frame argmax id (first
  * maximum, ctc_greedy_decoder.py:21) and max-probability 1 / sum_j exp(x_j - max) (the softmax value of the argmax).
+ * A frame whose softmax is undefined (a NaN or +inf logit, e.g. from an operand pair at +-inf) gets maxp = NaN and id 0,
+ * which is what np.argmax returns on the reference's all-NaN probability row.  Id 0 is the CTC blank, so such a frame
+ * decodes as silence: a caller that must detect poisoned input checks maxp for NaN.
  * workspace: 3 * ceil(V/32) * M * 4 bytes.  Same outputs as masr_gemm_tc_f16x2 + masr_ctc_frame_argmax_f32. */
 int masr_ctc_head_argmax_tc_f16x2(const void* Ah, const void* Al, int64_t lda, const void* Wh, const void* Wl,
                                   const float* bias, int M, int V, int K, void* workspace, int64_t workspace_bytes,
@@ -155,7 +161,12 @@ int masr_conv1_cmvn_relu_planes_f16(const float* feats, const float* mean, const
 int masr_conv2_tc_f16x2(const void* c1h, const void* c1l, const void* Wh, const void* Wl, const float* bias,
                         float* out, void* outh, void* outl, int B, int F1, int T2, int C, void* stream);
 
-/* fp32 -> fp16 (h, l) pair, elementwise over n contiguous values. */
+/* fp32 -> fp16 (h, l) pair, elementwise over n contiguous values: h = fp16_rn(x), l = fp16_rn((x - h) * 2^11), the form every
+ * pair producer of this header writes.  Operand range (derived from the fp16 format):
+ *   2^-14 <= |x| < 65520   h + 2^-11 l = x within 2^-22 |x|;
+ *   |x| < 2^-14            l is an fp16 subnormal: an absolute floor of 2^-36 (|error| <= 2^-22 |x| + 2^-36 everywhere);
+ *   |x| >= 65520           h = +-inf, l = -+inf (never a saturated finite value); a contraction that multiplies such a pair
+ *                          by anything yields NaN (inf - inf), so every output the operand enters is non-finite. */
 int masr_split_f16(const float* x, void* h, void* l, int64_t n, void* stream);
 
 /* torch.nn.LayerNorm(D, eps) over the last dimension (encoder.py:64-72; convolution.py:66).  D = 256, 512, 1024, 2048 or 4096
@@ -342,7 +353,8 @@ int masr_stream_shift_cache(void* x0, void* x1, int64_t rows_per_slot, int lorde
 
 /* softmax statistics of CTCLoss.softmax (masr/model_utils/loss/ctc.py:70) fused with the argmax of
  * greedy_decoder (masr/decoders/ctc_greedy_decoder.py:21-22): ids[m] = first argmax_v, maxp[m] =
- * softmax(logits[m])[ids[m]].  probs (optional, may be NULL): full posterior [M, ldp]. */
+ * softmax(logits[m])[ids[m]] (a frame with a NaN or +inf logit: maxp = NaN, id 0, as masr_ctc_head_argmax_tc_f16x2).
+ * probs (optional, may be NULL): full posterior [M, ldp]. */
 int masr_ctc_frame_argmax_f32(const float* logits, int64_t ldl, int M, int V, int* ids, float* maxp, float* probs,
                               int64_t ldp, void* stream);
 

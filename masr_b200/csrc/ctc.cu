@@ -54,7 +54,8 @@ __global__ void __launch_bounds__(256) ctc_frame_argmax_kernel(const float* __re
     float tot = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) tot += ssum[w];
-    if (threadIdx.x == 0) { ids[row] = mi; maxp[row] = 1.0f / tot; }
+    // a NaN or +inf logit makes the softmax row all NaN (tot is NaN): numpy's argmax of such a row is 0
+    if (threadIdx.x == 0) { ids[row] = tot == tot ? mi : 0; maxp[row] = 1.0f / tot; }
     if (probs) {
         float* pr = probs + (int64_t)row * ldp;
         for (int j = threadIdx.x; j < V; j += 256) pr[j] = expf(__ldg(x + j) - m) / tot;

@@ -292,8 +292,9 @@ __device__ __forceinline__ void store_chunk(const TcParams& p, const EpiCtx& c, 
             }
             break;
         case MASR_EPI_BIAS_RELU:
+            // torch.relu keeps NaN (an operand that overflowed fp16 must not come out as 0); fmaxf alone would drop it
 #pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
+            for (int j = 0; j < 32; ++j) v[j] = v[j] != v[j] ? v[j] : fmaxf(v[j], 0.f);
             break;
         case MASR_EPI_BIAS_SCALE:
 #pragma unroll
@@ -610,7 +611,8 @@ __global__ void __launch_bounds__(128) ctc_partial_combine_kernel(const float* _
             if (gm > m || (gm == m && gi < mi)) { s = s * expf(m - gm) + gs; m = gm; mi = gi; }
             else s += gs * expf(gm - m);
         }
-        ids[row] = mi;
+        // a NaN or +inf logit makes the reference's softmax row all NaN (s is NaN here too): np.argmax of it is 0
+        ids[row] = s == s ? mi : 0;
         maxp[row] = 1.0f / s;
     }
 }
