@@ -478,6 +478,26 @@ int masr_ctc_prefix_beam_lm_pool(const int* cand_id, const float* cand_logp, con
                                  int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int* fresh, int* out_tok,
                                  int64_t tok_stride, int* out_n, float* out_score, float* out_approx, void* stream);
 
+/* Token onsets of the prefix beam search (every form above and the word-LM forms below).
+ * Trie layout per slot (trie_cap ints each of trie_parent and trie_tok, nc = trie_cap / 5):
+ *   trie_parent [0, nc)       parent node of node id (root 0: -1)
+ *   trie_parent [nc, 5 nc)    the persistent (parent, token) -> node hash (-1 = empty)
+ *   trie_tok    [0, nc)       last token of node id (root: -1)
+ *   trie_tok    [nc, 2 nc)    word-LM forms: 1 = the node's lexicon state was reset after <space>
+ *   trie_tok    [2 nc, 3 nc)  the onset of node id: the frame at which the search allocated it, i.e. the first frame after
+ *                             whose selection its prefix was in the beam (nodes are allocated for survivors only, and a
+ *                             prefix that leaves the beam and comes back keeps its node, so onsets strictly increase
+ *                             along a prefix)
+ *   trie_tok    [4 nc]        frames searched since the slot started fresh (one-shot, resume = 0, or fresh[b]); frames
+ *                             count from there, so a stream fed in any chunking records the one-shot search's onsets.
+ * masr_ctc_prefix_beam_frames: after a search, for each slot b < B the onset frame of every token of the prefix it
+ * reported: out_frame[b * tok_stride_f + p] for p < out_n[b], found by walking the hash from the root along
+ * out_tok[b * tok_stride + p] (so it serves the word-LM forms, which may report an entry other than rank 0); -1 where
+ * the prefix has no node (the trie ran out of nodes, or the slot was reset since).  One CTA per slot; the search's own
+ * trie_parent / trie_tok / trie_cap / out_tok / out_n. */
+int masr_ctc_prefix_beam_frames(const int* trie_parent, const int* trie_tok, int64_t trie_cap, const int* out_tok,
+                                int64_t tok_stride, const int* out_n, int B, int* out_frame, int64_t tok_stride_f, void* stream);
+
 /* ---- word n-gram LM fusion (ARPA) with the lexicon constraint -------------------------------------------
  * The external Scorer for a WORD-based LM (English models: configs/english_example.yml): the LM scores a word once, when
  * the <space> after it is emitted, and every hypothesis is limited to words of a lexicon built from the LM's unigrams

@@ -100,6 +100,7 @@ SIGNATURES = {
     "masr_ctc_prefix_beam_workspace": [_i, _i, C.POINTER(_i64), C.POINTER(_i64)],
     "masr_ctc_prefix_beam": [_vp, _vp, _vp, _i64, _vp, _i, _i, _i, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _vp, _vp],
     "masr_ctc_prefix_beam_state_size": [C.POINTER(_i64), C.POINTER(_i64)],
+    "masr_ctc_prefix_beam_frames": [_vp, _vp, _i64, _vp, _i64, _vp, _i, _vp, _i64, _vp],
     "masr_ctc_prefix_beam_stream": [_vp, _vp, _vp, _i64, _vp, _i, _i, _i, _vp, _vp, _vp, _i64, _vp, _vp, _i, _vp, _i64, _vp, _vp, _vp],
     "masr_ctc_greedy_collapse": [_vp, _vp, _i64, _vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp],
     "masr_lm_load_arpa": [_vp, _vp, _i, C.POINTER(_vp)],

@@ -32,7 +32,7 @@ class BeamSearch:
     while ``fresh[b]`` != 0.
     Results: ``out_tok`` [slots, max_frames] and ``out`` [3, slots] = (``score``, ``count`` as int32 bits, fused score):
     ``score`` is what the search reports (approx_ctc with an LM), ``fused`` the score the beam was ranked by (``score``
-    itself without an LM)."""
+    itself without an LM).  ``frames`` reads out the onset frame of each reported token."""
 
     def __init__(self, device, form: str, slots: int, rows: int, max_frames: int, beam_size: int = 300,
                  cutoff_prob: float = 0.99, cutoff_top_n: int = 40, lm=None, alpha: float = 0.0, beta: float = 0.0):
@@ -68,6 +68,7 @@ class BeamSearch:
         self.out = torch.zeros(3, S, device=dev, dtype=f32)
         self.score, self.count = self.out[0], self.out[1].view(i32)
         self.fused = self.out[0] if lm is None else self.out[2]
+        self.out_frame = None
 
     @property
     def lm(self):
@@ -106,3 +107,14 @@ class BeamSearch:
         eng._k("prefix_beam", self.name, *cands, *blank, bstride, lens, B, self.beam, 0, *fusion, self.scratch.data_ptr(),
                self.trie_par.data_ptr(), self.trie_tok.data_ptr(), self.trie_cap, *state, self.out_tok.data_ptr(),
                self.max_frames, self.count.data_ptr(), *scores)
+
+    def frames(self, eng, B: int) -> torch.Tensor:
+        """The onset frame of every token that slots 0..B-1 reported in their last search -> ``out_frame`` [slots,
+        max_frames] int32 (row b valid up to ``count[b]``), frames counted since each slot's (fresh) start.  One launch
+        after ``search``, on the same stream, and never inside a graph capture: the buffer is allocated on first use."""
+        if self.out_frame is None:
+            self.out_frame = torch.zeros(self.slots, self.max_frames, device=self.device, dtype=torch.int32)
+        eng._k("beam_frames", "masr_ctc_prefix_beam_frames", self.trie_par.data_ptr(), self.trie_tok.data_ptr(), self.trie_cap,
+               self.out_tok.data_ptr(), self.max_frames, self.count.data_ptr(), B, self.out_frame.data_ptr(),
+               self.max_frames)
+        return self.out_frame

@@ -12,7 +12,9 @@
 //                          entries could spell the same prefix and split its mass (seen as a ln 2 score gap on a 12 s
 //                          utterance); selection = exact radix select + bitonic sort, so ties
 //                          resolve deterministically (existing prefixes by rank, then children in (parent rank, candidate)
-//                          order) and the result equals the CPU restatement.
+//                          order) and the result equals the CPU restatement.  Each node also records its onset, the frame
+//                          at which it was allocated (= the first frame its prefix survived selection).
+//   prefix_frames_kernel   after a search: the onset of every token of each slot's reported prefix (token timestamps).
 #include <math.h>
 
 #include <type_traits>
@@ -200,6 +202,19 @@ struct LmSearch {
     masr_word_lm_tables wlm;                     // BEAM_WORD_LM
 };
 
+// The persistent (parent, token) -> node hash of a slot's trie: the home slot of a key, and the node of a key (-1: none).
+// Keys are inserted with atomicCAS at their home slot and linear probing, so a probe stops at the first empty slot.
+__device__ __forceinline__ uint32_t trie_home(int par, int tok, uint32_t hcap) {
+    return (((uint32_t)par * 2654435761u) ^ ((uint32_t)tok * 40503u)) % hcap;
+}
+__device__ __forceinline__ int trie_find(const int* thash, const int* tpar, const int* ttok, uint32_t hcap, int par, int tok) {
+    for (uint32_t h = trie_home(par, tok, hcap);; h = h + 1 == hcap ? 0 : h + 1) {
+        const int id = thash[h];
+        if (id == -1) return -1;
+        if (tpar[id] == par && ttok[id] == tok) return id;
+    }
+}
+
 constexpr int LM_STATE_INTS = 3 * BEAM_CAP + 2 + BEAM_CAP * LM_CTX / 2;   // + the windows, two ids per int
 constexpr int WLM_STATE_INTS = 3 * BEAM_CAP + 2 + BEAM_CAP * (WLM_CTX + 1);   // + the word windows and lexicon states
 
@@ -247,6 +262,9 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
     const uint32_t hcap = (uint32_t)(trie_cap - node_cap);
     int* thash = tpar + node_cap;
     int* tflag = ttok + node_cap;                                   // WORD: per node, 1 = reset after <space>
+    // [2 node_cap, 3 node_cap) of `trie_tok`: per node, the frame it was allocated at; trie_tok[4 node_cap]: the frames
+    // searched since the slot's fresh start (the first frame of this launch is frame S.misc[2] of the slot)
+    int* tclock = ttok + 4 * node_cap;
     int nbeam = 1, nnodes = 1;
     int* st_i = state_i ? state_i + (int64_t)b * (WORD ? WLM_STATE_INTS : LM ? LM_STATE_INTS : 3 * BEAM_CAP + 2) : nullptr;
     float* st_f = state_f ? state_f + (int64_t)b * (3 * BEAM_CAP) : nullptr;
@@ -281,6 +299,7 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
         if (tid == 0) {
             S.node[0] = 0; S.par[0] = -1; S.last[0] = -1; S.pb[0] = 0.f; S.pnb[0] = -INFINITY; S.score[0] = 0.f;
             tpar[0] = -1; ttok[0] = -1;
+            *tclock = 0;
             if constexpr (WORD) {
 #pragma unroll
                 for (int j = 0; j < WLM_CTX; ++j) S.wctx[0][j] = (uint32_t)lms.wlm.bos;
@@ -297,6 +316,7 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
     if constexpr (POOL) {
         if (tid == 0 && !cont) fresh[b] = 0;                       // (every thread has read the flag: after the barrier)
     }
+    if (tid == 0) S.misc[2] = *tclock;                             // (the radix select uses misc[0..1] only)
     for (int t = 0; t < T; ++t) {
         const int64_t row = (int64_t)b * bstride + t;
         const int K = cand_cnt[row];
@@ -545,15 +565,7 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
         // new children: reuse the node of a prefix that existed before (persistent hash), else allocate ids in rank order
         int need_new = 0;
         if (tid < n_sel && S.s_src[tid] == 1) {
-            const int par = S.s_par[tid], tok = S.s_last[tid];
-            uint32_t h = (((uint32_t)par * 2654435761u) ^ ((uint32_t)tok * 40503u)) % hcap;
-            int found = -1;
-            for (;;) {
-                const int id = thash[h];
-                if (id == -1) break;
-                if (tpar[id] == par && ttok[id] == tok) { found = id; break; }
-                h = h + 1 == hcap ? 0 : h + 1;
-            }
+            const int found = trie_find(thash, tpar, ttok, hcap, S.s_par[tid], S.s_last[tid]);
             S.s_node[tid] = found;
             need_new = found < 0;
             if constexpr (WORD) {                     // a prefix that comes back keeps its reset
@@ -577,8 +589,9 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
             if (id < node_cap) {
                 const int par = S.s_par[tid], tok = S.s_last[tid];
                 tpar[id] = par; ttok[id] = tok;
+                ttok[2 * node_cap + id] = S.misc[2] + t;
                 if constexpr (WORD) tflag[id] = 0;
-                uint32_t h = (((uint32_t)par * 2654435761u) ^ ((uint32_t)tok * 40503u)) % hcap;
+                uint32_t h = trie_home(par, tok, hcap);
                 while (atomicCAS(&thash[h], -1, id) != -1) h = h + 1 == hcap ? 0 : h + 1;
             }
         }
@@ -601,6 +614,7 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
         __syncthreads();
         if (nbeam == 0) break;
     }
+    if (tid == 0) *tclock = S.misc[2] + T;
     if (st_i) {
         if (tid < nbeam) {
             st_i[tid] = S.node[tid]; st_i[BEAM_CAP + tid] = S.par[tid]; st_i[2 * BEAM_CAP + tid] = S.last[tid];
@@ -722,6 +736,28 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
             }
             lms.out_approx[b] = apx;
         }
+    }
+}
+
+// The onset frame of every token of the prefix each slot reports: a walk from the root through the slot's (parent, token)
+// hash along out_tok (so it finds the reported entry whatever its rank), one thread per slot.  -1 where the prefix has no
+// node (the trie ran out of node capacity, or the slot's hash was reset after the search).
+__global__ void __launch_bounds__(32) prefix_frames_kernel(const int* __restrict__ trie_parent, const int* __restrict__ trie_tok,
+                                                           int64_t trie_cap, const int* __restrict__ out_tok, int64_t tok_stride,
+                                                           const int* __restrict__ out_n, int* __restrict__ out_frame,
+                                                           int64_t tok_stride_f) {
+    const int b = blockIdx.x;
+    if (threadIdx.x != 0) return;
+    const int64_t node_cap = trie_cap / 5;
+    const int* tpar = trie_parent + (int64_t)b * trie_cap;
+    const int* ttok = trie_tok + (int64_t)b * trie_cap;
+    const int* tonset = ttok + 2 * node_cap;
+    const uint32_t hcap = (uint32_t)(trie_cap - node_cap);
+    const int n = out_n[b];
+    int node = 0;
+    for (int p = 0; p < n; ++p) {
+        if (node >= 0) node = trie_find(tpar + node_cap, tpar, ttok, hcap, node, out_tok[(int64_t)b * tok_stride + p]);
+        out_frame[(int64_t)b * tok_stride_f + p] = node >= 0 ? tonset[node] : -1;
     }
 }
 
@@ -953,4 +989,15 @@ extern "C" int masr_ctc_prefix_beam_wordlm_pool(const int* cand_id, const float*
     return launch_beam<BEAM_WORD_LM, true>("masr_ctc_prefix_beam_wordlm_pool", true,
         {cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
          state_i, state_f, 0, fresh, out_tok, tok_stride, out_n, out_score, out_approx}, lm_host, alpha, beta, stream);
+}
+
+extern "C" int masr_ctc_prefix_beam_frames(const int* trie_parent, const int* trie_tok, int64_t trie_cap, const int* out_tok,
+                                           int64_t tok_stride, const int* out_n, int B, int* out_frame, int64_t tok_stride_f,
+                                           void* stream) {
+    if (B == 0) return MASR_OK;
+    MASR_REQUIRE(trie_parent && trie_tok && out_tok && out_n && out_frame, "masr_ctc_prefix_beam_frames: null pointer");
+    MASR_REQUIRE(B > 0 && trie_cap >= 5, "masr_ctc_prefix_beam_frames: B=%d, trie_cap=%lld out of range", B, (long long)trie_cap);
+    prefix_frames_kernel<<<B, 32, 0, (cudaStream_t)stream>>>(trie_parent, trie_tok, trie_cap, out_tok, tok_stride, out_n,
+                                                              out_frame, tok_stride_f);
+    return check_launch("prefix_frames_kernel");
 }

@@ -688,11 +688,11 @@ class ConformerEngine:
 
     def transcribe_beam(self, waves: Sequence[np.ndarray], beam_size: int = 300, cutoff_prob: float = 0.99,
                         cutoff_top_n: int = 40, use_db_normalization: bool = True, target_db: float = -20.0, lm=None,
-                        alpha: float = 0.0, beta: float = 0.0, rates: Optional[Sequence[int]] = None):
+                        alpha: float = 0.0, beta: float = 0.0, rates: Optional[Sequence[int]] = None, onsets: bool = False):
         """Host waveforms -> (token ids per utterance, log-scores) with the GPU prefix beam search (``lm``: see ctc_beam;
-        ``rates``: see transcribe)."""
+        ``rates``: see transcribe; ``onsets``: see beam_features)."""
         feats, frames, status = self.fbank(waves, use_db_normalization, target_db, rates=rates)
-        return self.beam_features(feats, frames, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta)
+        return self.beam_features(feats, frames, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta, onsets)
 
     def transcribe_beam_pipelined(self, batches, beam_size: int = 300, cutoff_prob: float = 0.99, cutoff_top_n: int = 40,
                                   use_db_normalization: bool = True, target_db: float = -20.0, lm=None, alpha: float = 0.0,
@@ -767,15 +767,19 @@ class ConformerEngine:
             yield finish(prev)
 
     def beam_features(self, feats, frames, beam_size: int = 300, cutoff_prob: float = 0.99, cutoff_top_n: int = 40, lm=None,
-                      alpha: float = 0.0, beta: float = 0.0):
+                      alpha: float = 0.0, beta: float = 0.0, onsets: bool = False):
+        """-> (token ids per utterance, log-scores); ``onsets``: also the onset frame of every token per utterance
+        (BeamSearch.frames), as a third element."""
         B = feats.shape[0]
         enc, tl, T, ws = self.encode(feats, frames)
         if T == 0:
-            return [[] for _ in range(B)], [0.0] * B
+            return ([[] for _ in range(B)], [0.0] * B) + (([[] for _ in range(B)],) if onsets else ())
         tok, n, sc = self.ctc_beam(enc, tl, T, ws, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta)
+        fr = ws["beam"].frames(self, B).cpu().numpy() if onsets else None
         tok, n, sc = tok.cpu().numpy(), n.cpu().numpy(), sc.cpu().numpy()
-        self.d2h_bytes += tok.nbytes + n.nbytes + sc.nbytes
-        return [tok[b, :n[b]].tolist() for b in range(B)], [float(s) for s in sc]
+        self.d2h_bytes += tok.nbytes + n.nbytes + sc.nbytes + (0 if fr is None else fr.nbytes)
+        out = [tok[b, :n[b]].tolist() for b in range(B)], [float(s) for s in sc]
+        return out + (([fr[b, :n[b]].tolist() for b in range(B)],) if onsets else ())
 
     # ---- public batched entry points -----------------------------------------------------------
     def transcribe(self, waves: Sequence[np.ndarray], use_db_normalization: bool = True, target_db: float = -20.0,
@@ -1252,28 +1256,35 @@ class StreamBeam(BeamSearch):
         self.eng, self._own_lm = eng, lm                         # (the search itself holds the LM only weakly)
         self.max_chunk = int(max_chunk)
         self.lens = torch.zeros(1, device=eng.device, dtype=torch.int32)
-        self.frames = 0
+        self.seen = 0
 
     def reset(self):
         """``reset_decoder`` (beam_search_decoder.py:93-96)."""
-        self.frames = 0
+        self.seen = 0
 
     def push(self, logits: torch.Tensor, rows: int):
-        """CTC-head logits [>= rows, ld] of the new chunk's frames -> (token ids of the best prefix so far, its log score)."""
+        """CTC-head logits [>= rows, ld] of the new chunk's frames -> (token ids of the best prefix so far, its log score);
+        ``onsets()`` reads out the frames of those tokens."""
         if rows > self.max_chunk:
             raise ValueError(f"a chunk has at most {self.max_chunk} frames")
-        if self.frames + rows > self.max_frames:
+        if self.seen + rows > self.max_frames:
             raise AssertionError(f"stream longer than {self.max_frames} frames: create the StreamBeam with a larger max_frames")
         if rows > 0:
             self.topk(self.eng, logits, logits.stride(0), rows)
         self.lens.fill_(rows)
-        self.search(self.eng, _p(self.lens), 1, self.max_chunk, resume=1 if self.frames else 0)
-        self.frames += rows
+        self.search(self.eng, _p(self.lens), 1, self.max_chunk, resume=1 if self.seen else 0)
+        self.seen += rows
         oh = self.out[:2].cpu()                                     # [score, count (int32 bits)]
         n = int(oh[1].view(torch.int32).item())
         toks = self.out_tok[0, :n].cpu().tolist() if n else []
         self.eng.d2h_bytes += 8 + 4 * n
         return toks, float(oh[0].item())
+
+    def onsets(self) -> List[int]:
+        """The onset frame (since the last ``reset``) of every token of the best prefix the last ``push`` reported."""
+        n = int(self.count[0].item())
+        self.eng.d2h_bytes += 4 * n
+        return self.frames(self.eng, 1)[0, :n].cpu().tolist() if n else []
 
 
 def greedy_score(psum: np.float32, pcount: int) -> float:

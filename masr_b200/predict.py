@@ -28,6 +28,7 @@ from .audio import load_audio, pcm_bytes_to_float32, samples_to_float32
 from .engine import ConformerEngine, EfficientConformerEngine, greedy_score, subsampled_len
 from .resample import MODEL_RATE, needs_resampling
 from .text import TextFeaturizer, ids_to_text
+from . import timestamps as ts
 
 logger = logging.getLogger(__name__)
 
@@ -191,32 +192,40 @@ class MASRPredictor:
             raise Exception("masr_b200: inverse text normalisation (is_itn) is outside the hot-path scope")
         return text
 
-    def predict(self, audio_data, use_pun=False, is_itn=False, sample_rate=16000):
-        """Whole-utterance recognition (predict.py:167-192)."""
-        waves, rates = self._load_batch([audio_data], sample_rate)
-        if self._beam_conf is not None:
-            toks, scores = self.predictor.transcribe_beam(waves, use_db_normalization=self._use_db,
-                                                          target_db=self._target_db, rates=rates, **self._beam_conf)
-            text = ids_to_text(toks[0], self._text_featurizer.vocab_list)
-            return {'text': self._finish(text, use_pun, is_itn), 'score': scores[0]}
-        res = self.predictor.transcribe(waves, self._use_db, self._target_db, rates=rates)
-        self._raise_status(res.status)
-        text = ids_to_text(res.tokens[0], self._text_featurizer.vocab_list)
-        return {'text': self._finish(text, use_pun, is_itn), 'score': res.scores[0]}
+    def predict(self, audio_data, use_pun=False, is_itn=False, sample_rate=16000, timestamps=False):
+        """Whole-utterance recognition (predict.py:167-192).  ``timestamps``: the result also carries ``'tokens'``
+        (``[{'token', 'start', 'end'}]``, seconds) and, when the vocabulary has ``<space>``, ``'words'``
+        (masr_b200/timestamps.py)."""
+        r = self._recognise(*self._load_batch([audio_data], sample_rate), timestamps)[0]
+        r['text'] = self._finish(r['text'], use_pun, is_itn)
+        return r
 
-    def predict_batch(self, audio_list: Sequence, sample_rate=16000):
+    def predict_batch(self, audio_list: Sequence, sample_rate=16000, timestamps=False):
         """Additive: a list of utterances in one GPU pass; element i equals ``predict(audio_list[i])``.  With
-        ``resample=True`` the rows may have different rates (WAV files carry their own)."""
-        waves, rates = self._load_batch(audio_list, sample_rate)
-        if self._beam_conf is not None:
-            toks, scores = self.predictor.transcribe_beam(waves, use_db_normalization=self._use_db,
-                                                          target_db=self._target_db, rates=rates, **self._beam_conf)
-            vocab = self._text_featurizer.vocab_list
-            return [{'text': ids_to_text(t, vocab), 'score': s} for t, s in zip(toks, scores)]
-        res = self.predictor.transcribe(waves, self._use_db, self._target_db, rates=rates)
-        self._raise_status(res.status)
+        ``resample=True`` the rows may have different rates (WAV files carry their own).  ``timestamps``: as in predict."""
+        return self._recognise(*self._load_batch(audio_list, sample_rate), timestamps)
+
+    def _recognise(self, waves, rates, timestamps=False, offsets=None):
+        """Waveforms -> ``[{'text', 'score'}]`` (+ token and word times, shifted by ``offsets[i]`` seconds)."""
         vocab = self._text_featurizer.vocab_list
-        return [{'text': ids_to_text(t, vocab), 'score': s} for t, s in zip(res.tokens, res.scores)]
+        dt = ts.frame_seconds(self.predictor)
+        offsets = offsets or [0.0] * len(waves)
+        if self._beam_conf is not None:
+            out = self.predictor.transcribe_beam(waves, use_db_normalization=self._use_db, target_db=self._target_db,
+                                                 rates=rates, onsets=timestamps, **self._beam_conf)
+            res = [{'text': ids_to_text(t, vocab), 'score': s} for t, s in zip(out[0], out[1])]
+            if timestamps:
+                for r, t, f, off in zip(res, out[0], out[2], offsets):
+                    ts.beam_result(r, t, f, vocab, dt, off)
+            return res
+        g = self.predictor.transcribe(waves, self._use_db, self._target_db, return_frames=timestamps, rates=rates)
+        self._raise_status(g.status)
+        res = [{'text': ids_to_text(t, vocab), 'score': s} for t, s in zip(g.tokens, g.scores)]
+        if timestamps:
+            for b, (r, off) in enumerate(zip(res, offsets)):
+                ids = g.frame_ids[b, :g.frame_lens[b]] if g.frame_ids is not None else []
+                ts.greedy_result(r, ids, vocab, dt, off)
+        return res
 
     def predict_batches(self, batches, sample_rate=16000, device_hook=None):
         """Additive: a stream of batches (iterable of lists of utterances) -> one list of ``{'text','score'}`` per batch, in
@@ -257,10 +266,14 @@ class MASRPredictor:
             from .vad import GpuSileroVAD
             self.vad_predictor = GpuSileroVAD(vad_model_path, device=self.predictor.device)
 
-    def predict_long(self, audio_data, use_pun=False, is_itn=False, sample_rate=16000, vad_predictor=None, vad_model_path=None):
+    def predict_long(self, audio_data, use_pun=False, is_itn=False, sample_rate=16000, vad_predictor=None, vad_model_path=None,
+                     timestamps=False):
         """Long-form recognition (predict.py:195-234): VAD segments -> recognise -> join with '，' and average the scores.
         All segments of the recording go through ONE batched GPU pass (``predict_batch``) instead of the reference's
-        one-``predict``-per-segment loop; each segment's result equals ``predict(segment)`` (B=1 semantics)."""
+        one-``predict``-per-segment loop; each segment's result equals ``predict(segment)`` (B=1 semantics).
+        ``timestamps``: the result also carries ``'sentences'``, one ``{'text', 'score', 'start', 'end', 'tokens'}`` (+
+        ``'words'``) per segment with non-empty text: the segment's bounds and its token times, in seconds of the
+        recording."""
         self.init_vad(vad_predictor, vad_model_path)
         samples, sr = load_audio(audio_data, sample_rate)
         self._check_rate(sr)
@@ -269,7 +282,8 @@ class MASRPredictor:
             samples, sr = self.predictor.resample([samples], [sr])[0], self._sample_rate
         stamps = self.vad_predictor.get_speech_timestamps(samples, sr)
         segs = [samples[t['start']:t['end']] for t in stamps]
-        results = self.predict_batch(segs, sample_rate=sr) if segs else []
+        offsets = [t['start'] / sr for t in stamps]
+        results = self._recognise(*self._load_batch(segs, sr), timestamps, offsets) if segs else []
         texts, scores = '', []
         for r in results:
             if r['text'] != '':
@@ -281,13 +295,17 @@ class MASRPredictor:
             logger.warning('标点符号模型没有初始化！')
         if is_itn:
             raise Exception("masr_b200: inverse text normalisation (is_itn) is outside the hot-path scope")
-        return {'text': texts, 'score': round(sum(scores) / len(scores), 2) if scores else 0}
+        out = {'text': texts, 'score': round(sum(scores) / len(scores), 2) if scores else 0}
+        if timestamps:
+            out['sentences'] = ts.sentences([(t['start'], t['end']) for t in stamps], results, sr)
+        return out
 
     # ---------------------------------------------------------------------------------------------
     def predict_stream(self, audio_data, is_end=False, use_pun=False, is_itn=False, channels=1, samp_width=2,
-                       sample_rate=16000):
+                       sample_rate=16000, timestamps=False):
         """Streaming recognition, one push of audio per call (predict.py:237-343).  Returns ``None``
-        while fewer than 67 feature frames are buffered, else the running ``{'text','score'}``."""
+        while fewer than 67 feature frames are buffered, else the running ``{'text','score'}``; ``timestamps``: with
+        ``'tokens'`` (+ ``'words'``) as in predict, timed since the last ``reset_stream``."""
         if not self.configs.streaming:
             raise Exception(
                 f"不支持改该模型流式识别，当前模型：{self.configs.use_model}，参数streaming为：{self.configs.streaming}")
@@ -342,11 +360,13 @@ class MASRPredictor:
             self._hist_ids.extend(int(i) for i in ids_h)
             self._hist_probs.extend(mp_h[t] for t in range(len(ids_h)) if ids_h[t] != 0)
         self.cached_feat = self.cached_feat[end - CACHED_FEATURE_NUM:]
+        vocab, dt = self._text_featurizer.vocab_list, ts.frame_seconds(eng)
         if self._beam_conf is not None:
             toks, score = self._sbeam_result
             if is_itn:
                 raise Exception("masr_b200: inverse text normalisation (is_itn) is outside the hot-path scope")
-            return {'text': ids_to_text(toks, self._text_featurizer.vocab_list), 'score': score}
+            r = {'text': ids_to_text(toks, vocab), 'score': score}
+            return ts.beam_result(r, toks, self._sbeam.onsets() if toks else [], vocab, dt) if timestamps else r
         # greedy_decoder_chunk re-collapses the whole history (ctc_greedy_decoder.py:81-88)
         toks, prev = [], None
         for i in self._hist_ids:
@@ -357,14 +377,16 @@ class MASRPredictor:
         for p in self._hist_probs:
             acc = np.float32(acc + p)
         score = greedy_score(acc, len(self._hist_probs))
-        text = ids_to_text(toks, self._text_featurizer.vocab_list)
+        text = ids_to_text(toks, vocab)
         if use_pun and is_end and len(text) > 0:
             logger.warning('标点符号模型没有初始化！')
         if is_itn:
             raise Exception("masr_b200: inverse text normalisation (is_itn) is outside the hot-path scope")
-        return {'text': text, 'score': score}
+        r = {'text': text, 'score': score}
+        return ts.greedy_result(r, self._hist_ids, vocab, dt) if timestamps else r
 
-    def create_stream_pool(self, n_slots: int, max_frames: int = 3000, vad_model_path=None, vad_options=None):
+    def create_stream_pool(self, n_slots: int, max_frames: int = 3000, vad_model_path=None, vad_options=None,
+                           timestamps=False):
         """Additive: a ``StreamPool`` of ``n_slots`` concurrent streams over this predictor's model, decoding as the YAML
         says — greedy, or the GPU prefix beam search with the character or word LM this predictor loaded (if any).  Each slot's
         ``push`` results equal ``predict_stream`` on that stream alone.  ``max_frames``: encoder frames one stream may reach
@@ -372,12 +394,16 @@ class MASRPredictor:
 
         ``vad_model_path`` (the silero VAD model file): instead a ``SegmentingStreamPool`` over that pool, which cuts every
         slot's live stream into utterances with ``GpuSileroVAD(vad_model_path, **vad_options)`` and decodes each one as a
-        fresh ``predict_stream`` (masr_b200/segment_pool.py), so a stream may run for any length."""
+        fresh ``predict_stream`` (masr_b200/segment_pool.py), so a stream may run for any length.
+
+        ``timestamps``: every result also carries ``'tokens'`` (+ ``'words'``) as ``predict_stream(..., timestamps=True)``,
+        timed since the slot's reset; with the VAD, segments and partials are timed since the slot's stream started."""
         if not self.configs.streaming:
             raise Exception(f"不支持改该模型流式识别，当前模型：{self.configs.use_model}，参数streaming为：{self.configs.streaming}")
         from .stream_pool import StreamPool
         pool = StreamPool(self.predictor, self._text_featurizer.vocab_list, n_slots, use_db_normalization=self._use_db,
-                          target_db=self._target_db, max_frames=max_frames, beam=self._beam_conf, resample=self._resample)
+                          target_db=self._target_db, max_frames=max_frames, beam=self._beam_conf, resample=self._resample,
+                          timestamps=timestamps)
         if vad_model_path is None:
             return pool
         from .segment_pool import SegmentingStreamPool

@@ -127,6 +127,8 @@ class SegmentingStreamPool:
 
     ``push(audio, is_end=False)`` -> per pushed slot ``{'segments': [{'start', 'end', 'text', 'score'}, ...] (closed
     during this push), 'partial': {'start', 'text', 'score'} | None (the open segment's latest result), 'speech': bool}``.
+    With a pool made with ``timestamps=True`` segments and partials also carry ``'tokens'`` (+ ``'words'``), timed in
+    seconds since the slot's stream started.
     ``is_end`` (one bool or ``{slot: bool}``) ends a slot's stream: its open segment closes at the last received sample and
     the slot starts a new stream (with an empty transcript) on its next push.  ``transcript(slot)`` joins the closed
     segments as ``predict_long`` does.  Per-slot errors (undecodable input, a rate other than 16 kHz, a failure of the slot's recognition) fail only
@@ -222,6 +224,10 @@ class SegmentingStreamPool:
                 if not grp[end]:
                     continue
                 pieces = {s: self.ring[s][a - self.ring_base[s]:b - self.ring_base[s]] for s, (a, b) in grp[end].items()}
+                for s in grp[end]:                    # the recogniser's stream starts at the segment's start
+                    pl = self.planners[s]
+                    k = len(self.closed[s])
+                    self.pool.t0[s] = (pl.segments[k][0] if k < len(pl.segments) else pl.open) / MODEL_RATE
                 res = self.pool.push(pieces, is_end=end, on_error="return")
                 for s, e in self.pool.last_errors.items():
                     errors[s] = e
@@ -234,12 +240,16 @@ class SegmentingStreamPool:
                         seg_start = self.planners[s].segments[len(self.closed[s])][0]
                         text, score = (got["text"], got["score"]) if got is not None else ("", 0.0)
                         rec = {"start": seg_start, "end": b, "text": text, "score": score}
+                        if self.pool.timestamps:
+                            rec.update({k: v for k, v in got.items() if k in ("tokens", "words")} if got is not None
+                                       else {"tokens": []})
                         self.closed[s].append(rec)
                         seg_out[s].append(rec)
                         self.partial[s] = None
                         self.pool.reset_stream(s)
                     elif got is not None:
                         self.partial[s] = {"start": self.planners[s].open, "text": got["text"], "score": got["score"]}
+                        self.partial[s].update({k: got[k] for k in ("tokens", "words") if k in got})
         for s in failed:                              # the slot's stream is abandoned: start it over
             self._clear([s])
         out: Dict[int, dict] = {}

@@ -26,6 +26,7 @@ from .engine import ConformerEngine, _p, greedy_score, subsampled_len
 from .predict import CACHED_FEATURE_NUM, DECODING_WINDOW, FRAME_SHIFT, chunk_starts
 from .resample import MODEL_RATE, output_length
 from .text import ids_to_text
+from . import timestamps as ts
 
 CHUNK_FRAMES = DECODING_WINDOW          # 67 feature frames -> 16 encoder frames
 CHUNK_OUT = 16
@@ -592,10 +593,11 @@ class PoolBeam(BeamSearch):
         self.topk(self.eng, self.logits, self.eng.Vpad, self.slots * self.R)
         self.search(self.eng, self.lens, self.slots, self.R)
 
-    def results(self, slots: Sequence[int], frames: Sequence[int]) -> Dict[int, tuple]:
+    def results(self, slots: Sequence[int], frames: Sequence[int], onsets: bool = False) -> Dict[int, tuple]:
         """slot -> (token ids of its best prefix, score) after the last step: one D2H copy of every slot's count and score,
         then one of the token rows spanning `slots`.  ``frames[slot]``: the slot's encoder frames since its reset; a slot
-        without any gets ([], 0.0), as ``predict_stream`` does."""
+        without any gets ([], 0.0), as ``predict_stream`` does.  ``onsets``: each with a third element, the tokens' onset
+        frames since the slot's reset (one read-out launch here, outside the step graph, and one more copy)."""
         slots = list(slots)
         if not slots:
             return {}
@@ -607,13 +609,16 @@ class PoolBeam(BeamSearch):
         nmax = max((int(n[s]) for s in had), default=0)
         lo, hi = (min(had), max(had) + 1) if had else (0, 0)
         toks = self.out_tok[lo:hi, :nmax].cpu().numpy() if nmax else None
-        eng.d2h_bytes += oh.numel() * 4 + (0 if toks is None else toks.size * 4)
+        fr = self.frames(eng, hi)[lo:hi, :nmax].cpu().numpy() if onsets and nmax else None
+        eng.d2h_bytes += oh.numel() * 4 + (0 if toks is None else toks.size * 4) + (0 if fr is None else fr.size * 4)
         out = {}
         for s in slots:
             if frames[s] == 0:
                 out[s] = ([], 0.0)
             else:
                 out[s] = (toks[s - lo, :n[s]].tolist() if n[s] else [], float(score[s]))
+            if onsets:
+                out[s] += (fr[s - lo, :len(out[s][0])].tolist() if out[s][0] else [],)
         return out
 
 
@@ -629,14 +634,18 @@ class StreamPool:
 
     def __init__(self, eng: ConformerEngine, vocab: Sequence[str], n_slots: int, use_db_normalization: bool = True,
                  target_db: float = -20.0, max_frames: int = 3000, beam: Optional[dict] = None, use_graph: bool = True,
-                 resample: bool = False):
+                 resample: bool = False, timestamps: bool = False):
         """``beam``: None decodes greedily (``ctc_greedy``); a dict ``{beam_size, cutoff_prob, cutoff_top_n, lm, alpha,
         beta}`` (``MASRPredictor``'s ``ctc_beam_search`` settings; ``lm`` a ``CharLM``, ``WordLM`` or None) runs the streaming prefix
         beam search of every slot on the GPU (``PoolBeam``), and every result is the beam's, as ``predict_stream`` with
         ``decoder: ctc_beam_search`` returns it.  ``use_graph=False`` launches every step eagerly instead of replaying
         its CUDA graph (same results).  ``resample``: accept pushes at other sample rates (``push(..., sample_rate=)``) and
-        resample them on the GPU as ``predict_stream`` does; False makes such a push a per-slot error."""
+        resample them on the GPU as ``predict_stream`` does; False makes such a push a per-slot error.  ``timestamps``:
+        every result also carries ``'tokens'`` (+ ``'words'``) timed since the slot's reset, as ``predict_stream(...,
+        timestamps=True)`` returns them, plus ``t0[slot]`` seconds (0 after a reset; a caller that cuts a longer stream
+        into utterances sets it to the utterance's start)."""
         self.eng, self.vocab, self.S = eng, list(vocab), n_slots
+        self.timestamps, self.dt, self.t0 = bool(timestamps), ts.frame_seconds(eng), [0.0] * n_slots
         self.resample = bool(resample)
         self.pool = make_pool(eng, n_slots, max_frames)
         if not use_graph:
@@ -660,9 +669,12 @@ class StreamPool:
             self.prev = np.full(self.S, -1, np.int64)          # last frame id per slot (-1: none yet)
             self.acc = np.zeros(self.S, np.float32)            # left-to-right float32 sum of the non-blank max-probabilities
             self.nprob = np.zeros(self.S, np.int64)
+            self.seen = np.zeros(self.S, np.int64)             # encoder frames since the reset
+            self.t_start = [[] for _ in range(self.S)]         # per token: its first frame, and the end of its run so far
+            self.t_end = [[] for _ in range(self.S)]
         for s in slots:
-            self.toks[s] = []
-            self.prev[s], self.acc[s], self.nprob[s] = -1, np.float32(0.0), 0
+            self.toks[s], self.t_start[s], self.t_end[s] = [], [], []
+            self.prev[s], self.acc[s], self.nprob[s], self.seen[s] = -1, np.float32(0.0), 0, 0
 
     def _fold(self, ids_h: np.ndarray, mp_h: np.ndarray, tout: Sequence[int]):
         """Incremental ``greedy_decoder_chunk`` (ctc_greedy_decoder.py:70-89) for every slot at once: collapse repeats against
@@ -687,6 +699,16 @@ class StreamPool:
         self.nprob += nonblank.sum(1)
         for s in np.nonzero(new_tok.any(1))[0]:
             self.toks[s].extend(ids[s, new_tok[s]].tolist())
+        if self.timestamps:                      # a non-blank frame starts a token or continues the last token's run
+            for s in np.nonzero(nonblank.any(1))[0]:
+                base = int(self.seen[s])
+                for t in np.nonzero(nonblank[s])[0]:
+                    if new_tok[s, t]:
+                        self.t_start[s].append(base + int(t))
+                        self.t_end[s].append(base + int(t) + 1)
+                    else:
+                        self.t_end[s][-1] = base + int(t) + 1
+        self.seen += tout
         has = tout > 0
         last = np.take_along_axis(ids, np.maximum(tout - 1, 0)[:, None], axis=1)[:, 0]
         self.prev = np.where(has, last, self.prev)
@@ -696,7 +718,7 @@ class StreamPool:
         if self.beam is not None:
             self.beam.reset(slot)
         self.remained[slot] = None
-        self.head[slot], self.count[slot] = 0, 0
+        self.head[slot], self.count[slot], self.t0[slot] = 0, 0, 0.0
         self._reset_hist([slot])
 
     def _dev_index(self, idx: np.ndarray) -> torch.Tensor:
@@ -839,7 +861,8 @@ class StreamPool:
                 ids, maxp, tout = self.pool.step(batch, nfr)
                 if self.beam is None:                # (the beam's state stays on the device: no copy per round)
                     self._fold(ids.cpu().numpy(), maxp.cpu().numpy(), tout)
-            beam_out = self.beam.results([s for s in live if pending[s]], self.pool.lens_host) if self.beam is not None else None
+            beam_out = self.beam.results([s for s in live if pending[s]], self.pool.lens_host, self.timestamps) \
+                if self.beam is not None else None
             for s in live:
                 if not pending[s]:
                     out[s] = None
@@ -848,10 +871,14 @@ class StreamPool:
                 self.head[s] = (self.head[s] + consumed) % R
                 self.count[s] -= consumed
                 if beam_out is not None:
-                    toks, score = beam_out[s]
+                    toks, score = beam_out[s][:2]
                     out[s] = {"text": ids_to_text(toks, self.vocab), "score": score}
+                    if self.timestamps:
+                        ts.beam_result(out[s], toks, beam_out[s][2], self.vocab, self.dt, self.t0[s])
                 else:
                     out[s] = {"text": ids_to_text(self.toks[s], self.vocab), "score": greedy_score(self.acc[s], int(self.nprob[s]))}
+                    if self.timestamps:
+                        ts.attach(out[s], self.toks[s], self.t_start[s], self.t_end[s], self.vocab, self.dt, self.t0[s])
         if errors and on_error == "raise":
             raise StreamSlotError(errors, out)
         return out
