@@ -567,6 +567,88 @@ int masr_ctc_prefix_beam_wordlm_pool(const int* cand_id, const float* cand_logp,
                                      int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int* fresh, int* out_tok,
                                      int64_t tok_stride, int* out_n, float* out_score, float* out_approx, void* stream);
 
+/* ---- hotword biasing ------------------------------------------------------------------------------------------------
+ * Boosts user hotwords inside the prefix beam search (semantics: oracle/hotwords.py, masr_b200/hotwords.py).  The
+ * hotwords' token sequences form an Aho-Corasick automaton; one buffer may hold several graphs (one per stream-pool
+ * slot), each a contiguous node range whose first node is its root.  Node ids, arc targets, fail and tail are indices of
+ * the whole buffer.  Per node n: acc = float32(w) * depth, leaf = no hotword extends str(n), fail = the longest proper
+ * suffix of str(n) that is a node, tail = -1 if no prefix of str(n) (itself included) is a whole hotword, else the state
+ * reached from the root by what follows the deepest such prefix ta(n), whose credit is ta_acc; fin = the credit banked
+ * when a token that extends nothing follows n.  Arcs in CSR form, ascending token within a node. */
+typedef struct masr_hotword_graph {
+    const int* arc_off;       /* device [nodes + 1]: first arc of each node                                     */
+    const int* arc_tok;       /* device [arcs]: token of each arc                                               */
+    const int* arc_next;      /* device [arcs]: node each arc leads to                                          */
+    const int* fail;          /* device [nodes]                                                                 */
+    const int* tail;          /* device [nodes]: -1 = no whole hotword in the match                             */
+    const int* leaf;          /* device [nodes]: 1 = no hotword extends the match                               */
+    const float* acc;         /* device [nodes]                                                                 */
+    const float* ta_acc;      /* device [nodes]: acc of the deepest whole hotword in the match                  */
+    const float* fin;         /* device [nodes]                                                                 */
+    int nodes;                /* nodes of the buffer                                                            */
+} masr_hotword_graph;
+
+/* The nine prefix beam searches above with hotword biasing: the same arguments, then hot_host (the graph) and slot_root
+ * [B] (device: slot b's root node, -1 = no hotwords for that slot, which searches exactly as without).  Every extension
+ * by a non-blank token with a finite base adds the automaton's credit delta after the LM terms; the reported entry is the
+ * best after adding each entry's read-out fin(s) - acc(s), and out_score (and out_approx) exclude every credit: they
+ * are the reported entry's selection score minus the float32 sum of its tokens' deltas and read-out.  The streaming and
+ * pool forms size their state with the *_hot_state_size answers (BEAM_CAP ints more than without). */
+int masr_ctc_prefix_beam_hot_state_size(int64_t* ints_per_utt, int64_t* floats_per_utt);
+int masr_ctc_prefix_beam_lm_hot_state_size(int64_t* ints_per_utt, int64_t* floats_per_utt);
+int masr_ctc_prefix_beam_wordlm_hot_state_size(int64_t* ints_per_utt, int64_t* floats_per_utt);
+int masr_ctc_prefix_beam_hot(const int* cand_id, const float* cand_logp, const int* cand_cnt, int64_t bstride, const int* lens,
+                             int B, int beam_size, int blank, float* pool, int* trie_parent, int* trie_tok, int64_t trie_cap,
+                             int* out_tok, int64_t tok_stride, int* out_n, float* out_score,
+                             const masr_hotword_graph* hot_host, const int* slot_root, void* stream);
+int masr_ctc_prefix_beam_hot_stream(const int* cand_id, const float* cand_logp, const int* cand_cnt, int64_t bstride,
+                                    const int* lens, int B, int beam_size, int blank, float* pool, int* trie_parent,
+                                    int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int resume, int* out_tok,
+                                    int64_t tok_stride, int* out_n, float* out_score, const masr_hotword_graph* hot_host,
+                                    const int* slot_root, void* stream);
+int masr_ctc_prefix_beam_hot_pool(const int* cand_id, const float* cand_logp, const int* cand_cnt, int64_t bstride,
+                                  const int* lens, int B, int beam_size, int blank, float* pool, int* trie_parent,
+                                  int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int* fresh, int* out_tok,
+                                  int64_t tok_stride, int* out_n, float* out_score, const masr_hotword_graph* hot_host,
+                                  const int* slot_root, void* stream);
+int masr_ctc_prefix_beam_lm_hot(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
+                                int64_t bstride, const int* lens, int B, int beam_size, int blank, const masr_lm_tables* lm_host,
+                                float alpha, float beta, float* pool, int* trie_parent, int* trie_tok, int64_t trie_cap,
+                                int* out_tok, int64_t tok_stride, int* out_n, float* out_score, float* out_approx,
+                                const masr_hotword_graph* hot_host, const int* slot_root, void* stream);
+int masr_ctc_prefix_beam_lm_hot_stream(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
+                                       int64_t bstride, const int* lens, int B, int beam_size, int blank,
+                                       const masr_lm_tables* lm_host, float alpha, float beta, float* pool, int* trie_parent,
+                                       int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int resume, int* out_tok,
+                                       int64_t tok_stride, int* out_n, float* out_score, float* out_approx,
+                                       const masr_hotword_graph* hot_host, const int* slot_root, void* stream);
+int masr_ctc_prefix_beam_lm_hot_pool(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
+                                     int64_t bstride, const int* lens, int B, int beam_size, int blank,
+                                     const masr_lm_tables* lm_host, float alpha, float beta, float* pool, int* trie_parent,
+                                     int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int* fresh, int* out_tok,
+                                     int64_t tok_stride, int* out_n, float* out_score, float* out_approx,
+                                     const masr_hotword_graph* hot_host, const int* slot_root, void* stream);
+int masr_ctc_prefix_beam_wordlm_hot(const int* cand_id, const float* cand_logp, const int* cand_cnt, const float* blank_logp,
+                                    int64_t bstride, const int* lens, int B, int beam_size, int blank,
+                                    const masr_word_lm_tables* lm_host, float alpha, float beta, float* pool, int* trie_parent,
+                                    int* trie_tok, int64_t trie_cap, int* out_tok, int64_t tok_stride, int* out_n,
+                                    float* out_score, float* out_approx, const masr_hotword_graph* hot_host,
+                                    const int* slot_root, void* stream);
+int masr_ctc_prefix_beam_wordlm_hot_stream(const int* cand_id, const float* cand_logp, const int* cand_cnt,
+                                           const float* blank_logp, int64_t bstride, const int* lens, int B, int beam_size,
+                                           int blank, const masr_word_lm_tables* lm_host, float alpha, float beta, float* pool,
+                                           int* trie_parent, int* trie_tok, int64_t trie_cap, int* state_i, float* state_f,
+                                           int resume, int* out_tok, int64_t tok_stride, int* out_n, float* out_score,
+                                           float* out_approx, const masr_hotword_graph* hot_host, const int* slot_root,
+                                           void* stream);
+int masr_ctc_prefix_beam_wordlm_hot_pool(const int* cand_id, const float* cand_logp, const int* cand_cnt,
+                                         const float* blank_logp, int64_t bstride, const int* lens, int B, int beam_size,
+                                         int blank, const masr_word_lm_tables* lm_host, float alpha, float beta, float* pool,
+                                         int* trie_parent, int* trie_tok, int64_t trie_cap, int* state_i, float* state_f,
+                                         int* fresh, int* out_tok, int64_t tok_stride, int* out_n, float* out_score,
+                                         float* out_approx, const masr_hotword_graph* hot_host, const int* slot_root,
+                                         void* stream);
+
 /* The silero VAD network (16 kHz branch of silero_vad.onnx, weights packed by masr_b200/silero.py) over one recording
  * of n_samples 16 kHz samples in windows of `window` samples (512, 1024 or 1536; the last window zero-padded),
  * T = window / 512 recurrent steps per window, N = ceil(n_samples / window) windows.

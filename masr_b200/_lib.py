@@ -36,6 +36,15 @@ class WordLmTables(C.Structure):
 
 
 _wlmp = C.POINTER(WordLmTables)
+
+
+class HotwordGraph(C.Structure):
+    """``masr_hotword_graph`` of include/masr_b200.h."""
+    _fields_ = [("arc_off", _vp), ("arc_tok", _vp), ("arc_next", _vp), ("fail", _vp), ("tail", _vp), ("leaf", _vp),
+                ("acc", _vp), ("ta_acc", _vp), ("fin", _vp), ("nodes", _i)]
+
+
+_hgp = C.POINTER(HotwordGraph)
 LM_INFO_ORDER, LM_INFO_CHAR_BASED, LM_INFO_DICT_SIZE, LM_INFO_VOCAB, LM_INFO_KEY_WORDS, LM_INFO_VAL_FLOATS = range(6)
 LM_INFO_READ, LM_INFO_KEPT, LM_INFO_SLOTS, LM_INFO_TABLE_BYTES = 8, 14, 20, 26
 WORD_LM_INFO_NODES, WORD_LM_INFO_ARCS, WORD_LM_INFO_SPACE = 27, 28, 29
@@ -129,6 +138,26 @@ SIGNATURES = {
                                            _i, _vp, _i64, _vp, _vp, _vp, _vp],
     "masr_ctc_prefix_beam_wordlm_pool": [_vp, _vp, _vp, _vp, _i64, _vp, _i, _i, _i, _wlmp, _f, _f, _vp, _vp, _vp, _i64, _vp, _vp,
                                          _vp, _vp, _i64, _vp, _vp, _vp, _vp],
+    "masr_ctc_prefix_beam_hot_state_size": [C.POINTER(_i64), C.POINTER(_i64)],
+    "masr_ctc_prefix_beam_lm_hot_state_size": [C.POINTER(_i64), C.POINTER(_i64)],
+    "masr_ctc_prefix_beam_wordlm_hot_state_size": [C.POINTER(_i64), C.POINTER(_i64)],
+    "masr_ctc_prefix_beam_hot": [_vp, _vp, _vp, _i64, _vp, _i, _i, _i, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _vp, _hgp, _vp, _vp],
+    "masr_ctc_prefix_beam_hot_stream": [_vp, _vp, _vp, _i64, _vp, _i, _i, _i, _vp, _vp, _vp, _i64, _vp, _vp, _i, _vp, _i64, _vp,
+                                        _vp, _hgp, _vp, _vp],
+    "masr_ctc_prefix_beam_hot_pool": [_vp, _vp, _vp, _i64, _vp, _i, _i, _i, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _vp,
+                                      _vp, _hgp, _vp, _vp],
+    "masr_ctc_prefix_beam_lm_hot": [_vp, _vp, _vp, _vp, _i64, _vp, _i, _i, _i, _lmp, _f, _f, _vp, _vp, _vp, _i64, _vp, _i64, _vp,
+                                    _vp, _vp, _hgp, _vp, _vp],
+    "masr_ctc_prefix_beam_lm_hot_stream": [_vp, _vp, _vp, _vp, _i64, _vp, _i, _i, _i, _lmp, _f, _f, _vp, _vp, _vp, _i64, _vp, _vp,
+                                           _i, _vp, _i64, _vp, _vp, _vp, _hgp, _vp, _vp],
+    "masr_ctc_prefix_beam_lm_hot_pool": [_vp, _vp, _vp, _vp, _i64, _vp, _i, _i, _i, _lmp, _f, _f, _vp, _vp, _vp, _i64, _vp, _vp,
+                                         _vp, _vp, _i64, _vp, _vp, _vp, _hgp, _vp, _vp],
+    "masr_ctc_prefix_beam_wordlm_hot": [_vp, _vp, _vp, _vp, _i64, _vp, _i, _i, _i, _wlmp, _f, _f, _vp, _vp, _vp, _i64, _vp, _i64,
+                                        _vp, _vp, _vp, _hgp, _vp, _vp],
+    "masr_ctc_prefix_beam_wordlm_hot_stream": [_vp, _vp, _vp, _vp, _i64, _vp, _i, _i, _i, _wlmp, _f, _f, _vp, _vp, _vp, _i64, _vp,
+                                               _vp, _i, _vp, _i64, _vp, _vp, _vp, _hgp, _vp, _vp],
+    "masr_ctc_prefix_beam_wordlm_hot_pool": [_vp, _vp, _vp, _vp, _i64, _vp, _i, _i, _i, _wlmp, _f, _f, _vp, _vp, _vp, _i64, _vp,
+                                             _vp, _vp, _vp, _i64, _vp, _vp, _vp, _hgp, _vp, _vp],
 }
 
 

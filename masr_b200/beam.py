@@ -1,7 +1,8 @@
 """The GPU CTC prefix beam search (csrc/beam.cu) from the host: its device buffers and its two launches, for each of its
 three forms — one-shot (a batch of whole utterances), streaming (one stream fed chunk by chunk) and pool (every slot of a
-stream pool, launched inside the pool's CUDA graph) — without an LM, with a character LM or with a word LM.  Which entry
-point, which argument order and which buffers go with a (form, LM kind) is decided here and nowhere else."""
+stream pool, launched inside the pool's CUDA graph) — without an LM, with a character LM or with a word LM, each with or
+without hotwords.  Which entry point, which argument order and which buffers go with a (form, LM kind, hotwords) is decided
+here and nowhere else."""
 from __future__ import annotations
 
 import ctypes as C
@@ -32,14 +33,19 @@ class BeamSearch:
     while ``fresh[b]`` != 0.
     Results: ``out_tok`` [slots, max_frames] and ``out`` [3, slots] = (``score``, ``count`` as int32 bits, fused score):
     ``score`` is what the search reports (approx_ctc with an LM), ``fused`` the score the beam was ranked by (``score``
-    itself without an LM).  ``frames`` reads out the onset frame of each reported token."""
+    itself without an LM).  ``frames`` reads out the onset frame of each reported token.
+    ``hot``: None, or hotwords (a ``hotwords.HotwordGraph``, or for POOL a ``hotwords.HotwordBuffer``) searched by the
+    ``*_hot`` entry points; ``slot_root`` [slots] (device int32) is each slot's root node in it (-1: no hotwords for that
+    slot), all 0 (the graph's root) unless given.  Scores are reported without the hotword credit."""
 
     def __init__(self, device, form: str, slots: int, rows: int, max_frames: int, beam_size: int = 300,
-                 cutoff_prob: float = 0.99, cutoff_top_n: int = 40, lm=None, alpha: float = 0.0, beta: float = 0.0):
+                 cutoff_prob: float = 0.99, cutoff_top_n: int = 40, lm=None, alpha: float = 0.0, beta: float = 0.0,
+                 hot=None, slot_root: torch.Tensor = None):
         self.device, self.form, self.slots, self.max_frames = torch.device(device), form, int(slots), int(max_frames)
         self.beam, self.cutoff, self.top_n = int(beam_size), float(cutoff_prob), int(cutoff_top_n)
         self._lm, self.alpha, self.beta = None if lm is None else weakref.ref(lm), float(alpha), float(beta)
-        base = "masr_ctc_prefix_beam" if lm is None else lm.BEAM
+        self.hot = hot
+        base = ("masr_ctc_prefix_beam" if lm is None else lm.BEAM) + ("" if hot is None else "_hot")
         self.name = base + form
         dev, i32, f32, S = self.device, torch.int32, torch.float32, self.slots
         pool_n, trie_n = C.c_int64(0), C.c_int64(0)
@@ -51,6 +57,10 @@ class BeamSearch:
         self.blank_lp = None if lm is None else torch.zeros(rows, device=dev, dtype=f32)
         if lm is not None:
             lm.tables(dev)                                 # (uploaded here, never inside a graph capture)
+        self.slot_root = None
+        if hot is not None:
+            hot.tables(dev)
+            self.slot_root = torch.zeros(S, device=dev, dtype=i32) if slot_root is None else slot_root
         self.scratch = torch.empty(pool_n.value, device=dev, dtype=f32)
         if form == POOL:
             self.trie_par = torch.full((S * self.trie_cap,), -1, device=dev, dtype=i32)
@@ -75,9 +85,10 @@ class BeamSearch:
         """The LM this search fuses (None without one, or once its owner has dropped it)."""
         return None if self._lm is None else self._lm()
 
-    def fits(self, slots: int, frames: int, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta) -> bool:
+    def fits(self, slots: int, frames: int, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta, hot=None) -> bool:
         """Whether this search has room for ``slots`` utterances of ``frames`` frames and was built with these settings."""
         return (self.slots >= slots and self.max_frames >= frames and (self._lm is None) == (lm is None) and self.lm is lm
+                and self.hot is hot
                 and (self.beam, self.cutoff, self.top_n, self.alpha, self.beta)
                 == (int(beam_size), float(cutoff_prob), int(cutoff_top_n), float(alpha), float(beta)))
 
@@ -104,9 +115,10 @@ class BeamSearch:
         if self.form != ONE_SHOT:
             state = (self.state_i.data_ptr(), self.state_f.data_ptr(),
                      self.fresh.data_ptr() if self.form == POOL else int(resume))
+        hot = () if self.hot is None else (C.byref(self.hot.tables(self.device)), self.slot_root.data_ptr())
         eng._k("prefix_beam", self.name, *cands, *blank, bstride, lens, B, self.beam, 0, *fusion, self.scratch.data_ptr(),
                self.trie_par.data_ptr(), self.trie_tok.data_ptr(), self.trie_cap, *state, self.out_tok.data_ptr(),
-               self.max_frames, self.count.data_ptr(), *scores)
+               self.max_frames, self.count.data_ptr(), *scores, *hot)
 
     def frames(self, eng, B: int) -> torch.Tensor:
         """The onset frame of every token that slots 0..B-1 reported in their last search -> ``out_frame`` [slots,

@@ -189,10 +189,18 @@ struct BeamSharedWord : BeamShared {
     int lex[BEAM_CAP], s_lex[BEAM_CAP], k0[BEAM_CAP];
 };
 
+// The hotword instantiations: each beam entry and each staged entry carries its hotword automaton state (a node id of
+// the graph buffer; -1 while the slot has no hotwords).
+template <class Base> struct BeamSharedHot : Base {
+    int hs[BEAM_CAP], s_hs[BEAM_CAP];
+};
+
 enum : int { BEAM_PLAIN = 0, BEAM_CHAR_LM = 1, BEAM_WORD_LM = 2 };
 template <int MODE> struct BeamSmem { using type = BeamShared; };
 template <> struct BeamSmem<BEAM_CHAR_LM> { using type = BeamSharedLm; };
 template <> struct BeamSmem<BEAM_WORD_LM> { using type = BeamSharedWord; };
+template <int MODE, bool HOT>
+using BeamSmemT = std::conditional_t<HOT, BeamSharedHot<typename BeamSmem<MODE>::type>, typename BeamSmem<MODE>::type>;
 
 struct LmSearch {
     masr_lm_tables lm;
@@ -215,19 +223,59 @@ __device__ __forceinline__ int trie_find(const int* thash, const int* tpar, cons
     }
 }
 
+// Hotword biasing (per masr_b200/hotwords.py, oracle/hotwords.py): an Aho-Corasick automaton over the hotwords' token
+// sequences; HotArg<true> = the graph and each slot's root node (-1: the slot has no hotwords and searches as without).
+constexpr int HOT_MAX_LEN = 32;                 // tokens per hotword: bounds the automaton's fall-back walk
+template <bool HOT> struct HotArg {};
+template <> struct HotArg<true> { masr_hotword_graph g; const int* slot_root; };
+
+// the child of node n by token c (-1: none): binary search over n's arcs, ascending by token
+__device__ __forceinline__ int hot_child(const masr_hotword_graph& g, int n, int c) {
+    int lo = __ldg(g.arc_off + n), hi = __ldg(g.arc_off + n + 1) - 1;
+    while (lo <= hi) {
+        const int mid = (lo + hi) >> 1;
+        const int t = __ldg(g.arc_tok + mid);
+        if (t == c) return __ldg(g.arc_next + mid);
+        if (t < c) lo = mid + 1;
+        else hi = mid - 1;
+    }
+    return -1;
+}
+// One step of the automaton from state s by token c (slot root r) -> the credit delta; *next = the next state.  Leaving a
+// match banks the deepest whole hotword inside it (ta_acc, then on from tail) or withdraws it (fail); every turn moves to
+// a shallower node, so the walk ends within HOT_MAX_LEN + 1 turns.  A match that cannot grow (leaf) is committed: root.
+__device__ __forceinline__ float hot_step(const masr_hotword_graph& g, int r, int s, int c, int* next) {
+    float bank = 0.f;
+    int cur = s, nxt = r;
+    for (int it = 0; it <= HOT_MAX_LEN; ++it) {
+        const int ch = hot_child(g, cur, c);
+        if (ch >= 0) { nxt = ch; break; }
+        if (cur == r) break;
+        const int tl = __ldg(g.tail + cur);
+        if (tl >= 0) { bank = __fadd_rn(bank, __ldg(g.ta_acc + cur)); cur = tl; }
+        else cur = __ldg(g.fail + cur);
+    }
+    *next = __ldg(g.leaf + nxt) ? r : nxt;
+    return __fsub_rn(__fadd_rn(bank, __ldg(g.acc + nxt)), __ldg(g.acc + s));
+}
+// the read-out term of a state at the end of a search: fin(s) - acc(s) (an unfinished match earns nothing)
+__device__ __forceinline__ float hot_readout(const masr_hotword_graph& g, int s) {
+    return __fsub_rn(__ldg(g.fin + s), __ldg(g.acc + s));
+}
+
 constexpr int LM_STATE_INTS = 3 * BEAM_CAP + 2 + BEAM_CAP * LM_CTX / 2;   // + the windows, two ids per int
 constexpr int WLM_STATE_INTS = 3 * BEAM_CAP + 2 + BEAM_CAP * (WLM_CTX + 1);   // + the word windows and lexicon states
 
 // pool layout: [0, BEAM_CAP) existing prefixes (rank order), then BEAM_CAP + i*K + k children of (rank i, candidate k);
 // K = this frame's candidate count (usually a handful, cutoff_prob 0.99), so the pool the selection scans is 512 + beam*K
 // entries, not 512 + beam*40
-template <int MODE, bool POOL = false>
+template <int MODE, bool POOL = false, bool HOT = false>
 __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
     const int* __restrict__ cand_id, const float* __restrict__ cand_logp, const int* __restrict__ cand_cnt, int64_t bstride,
     const int* __restrict__ lens, int beam, int blank, float* __restrict__ pool_all, int* __restrict__ trie_parent,
     int* __restrict__ trie_tok, int64_t trie_cap, int* __restrict__ out_tok, int64_t tok_stride, int* __restrict__ out_n,
     float* __restrict__ out_score, int* __restrict__ state_i, float* __restrict__ state_f, int resume, const LmSearch lms,
-    int* __restrict__ fresh) {
+    int* __restrict__ fresh, const HotArg<HOT> hot) {
     // state_i / state_f (optional, per utterance 3*BEAM_CAP+2 ints / 3*BEAM_CAP floats; LM: LM_STATE_INTS ints): the beam
     // after the last frame, so the search can be resumed with the next chunk of frames (`resume` != 0) —
     // CTCBeamSearchDecoder.next()/decode() of the reference's streaming path (beam_search_decoder.py:75-91); the trie and
@@ -244,8 +292,12 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
     // the lexicon rejects extensions (pool entry -inf); an entry in LEX_AFTER_SPACE loses its first attempt of a frame
     // and is reset to the root, a flag kept with its trie node (tflag) so the reset persists if the node drops out of the
     // beam and comes back; after the last frame a read-out term is added on the side to pick and report the best entry.
+    // HOT (per oracle/hotwords.py): every extension by a non-blank token whose base is finite adds the automaton's credit
+    // delta last, ((base + alpha lnP) + beta) + delta; each entry carries its automaton state (state_i: BEAM_CAP more ints
+    // after the form's own).  The entry reported is the best after adding fin(s) - acc(s) (and the word read-out), and
+    // its reported score is that minus the credit of its tokens, replayed, so scores mean what they mean without hotwords.
     constexpr bool LM = MODE != BEAM_PLAIN, CHAR = MODE == BEAM_CHAR_LM, WORD = MODE == BEAM_WORD_LM;
-    using Shared = typename BeamSmem<MODE>::type;
+    using Shared = BeamSmemT<MODE, HOT>;
     extern __shared__ __align__(16) uint8_t smem_beam[];
     Shared& S = *reinterpret_cast<Shared*>(smem_beam);
     const int b = blockIdx.x, tid = threadIdx.x;
@@ -266,7 +318,10 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
     // searched since the slot's fresh start (the first frame of this launch is frame S.misc[2] of the slot)
     int* tclock = ttok + 4 * node_cap;
     int nbeam = 1, nnodes = 1;
-    int* st_i = state_i ? state_i + (int64_t)b * (WORD ? WLM_STATE_INTS : LM ? LM_STATE_INTS : 3 * BEAM_CAP + 2) : nullptr;
+    constexpr int ST_INTS = WORD ? WLM_STATE_INTS : LM ? LM_STATE_INTS : 3 * BEAM_CAP + 2;   // (HOT: + BEAM_CAP states)
+    int* st_i = state_i ? state_i + (int64_t)b * (ST_INTS + (HOT ? BEAM_CAP : 0)) : nullptr;
+    int hroot = -1;
+    if constexpr (HOT) hroot = hot.slot_root[b];
     float* st_f = state_f ? state_f + (int64_t)b * (3 * BEAM_CAP) : nullptr;
     bool cont;
     if constexpr (POOL) cont = fresh[b] == 0;
@@ -291,6 +346,7 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
                     S.ctx[tid][2 * j + 1] = (uint16_t)((unsigned)w[j] >> 16);
                 }
             }
+            if constexpr (HOT) S.hs[tid] = st_i[ST_INTS + tid];
         }
     } else {
         if constexpr (!POOL) {
@@ -310,6 +366,7 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
 #pragma unroll
                 for (int j = 0; j < LM_CTX; ++j) S.ctx[0][j] = (uint16_t)lms.lm.bos;
             }
+            if constexpr (HOT) S.hs[0] = hroot;
         }
     }
     __syncthreads();
@@ -381,6 +438,12 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
                 if (add != -INFINITY) {
                     const float lnp = lm_lnp(lms.lm, S.ctx[i], lm_word(lms.lm, c));
                     add = __fadd_rn(__fadd_rn(add, __fmul_rn(lms.alpha, lnp)), lms.beta);
+                }
+            }
+            if constexpr (HOT) {
+                if (hroot >= 0 && add != -INFINITY) {
+                    int nx;
+                    add = __fadd_rn(add, hot_step(hot.g, hroot, S.hs[i], c, &nx));
                 }
             }
             pool[BEAM_CAP + i * K + k] = add;
@@ -536,6 +599,7 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
 #pragma unroll
                     for (int j = 0; j < LM_CTX; ++j) S.s_ctx[tid][j] = S.ctx[src][j];
                 }
+                if constexpr (HOT) S.s_hs[tid] = S.hs[src];
             } else {                                  // a new child: gets a trie node below
                 const int i = (src - BEAM_CAP) / K, k = (src - BEAM_CAP) - i * K;
                 S.s_node[tid] = -1; S.s_par[tid] = S.node[i]; S.s_last[tid] = S.cid[k];
@@ -558,6 +622,11 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
                     const int n1 = lms.lm.order - 1;
                     for (int j = 0; j + 1 < n1; ++j) S.s_ctx[tid][j] = S.ctx[i][j + 1];
                     if (n1 > 0) S.s_ctx[tid][n1 - 1] = lm_word(lms.lm, S.cid[k]);
+                }
+                if constexpr (HOT) {
+                    int nx = -1;
+                    if (hroot >= 0) hot_step(hot.g, hroot, S.hs[i], S.cid[k], &nx);
+                    S.s_hs[tid] = nx;
                 }
             }
         }
@@ -609,6 +678,7 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
 #pragma unroll
                 for (int j = 0; j < LM_CTX; ++j) S.ctx[tid][j] = S.s_ctx[tid][j];
             }
+            if constexpr (HOT) S.hs[tid] = S.s_hs[tid];
         }
         nbeam = n_sel;
         __syncthreads();
@@ -630,24 +700,31 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
 #pragma unroll
                 for (int j = 0; j < LM_CTX / 2; ++j) w[j] = (int)((unsigned)S.ctx[tid][2 * j] | ((unsigned)S.ctx[tid][2 * j + 1] << 16));
             }
+            if constexpr (HOT) st_i[ST_INTS + tid] = S.hs[tid];
         }
         if (tid == 0) { st_i[3 * BEAM_CAP] = nbeam; st_i[3 * BEAM_CAP + 1] = nnodes; }
     }
     // the entry to report: rank 0, or (WORD) the best after the read-out term, which is computed on the side (the state
-    // saved above never sees it): alpha lnP(last word | h) + beta for every non-empty entry not ending in <space>
+    // saved above never sees it): alpha lnP(last word | h) + beta for every non-empty entry not ending in <space>;
+    // (HOT) plus the hotword read-out fin(s) - acc(s)
     int best = 0;
     float best_sc = nbeam > 0 ? S.score[0] : -INFINITY;
-    if constexpr (WORD) {
+    if constexpr (WORD || HOT) {
         float a = -INFINITY;
         int ai = 0x7fffffff;
         if (tid < nbeam) {
             a = S.score[tid];
             ai = tid;
-            if (S.par[tid] >= 0 && S.last[tid] != lms.wlm.space) {
-                const int st = S.lex[tid];
-                const int wid = st > 0 ? __ldg(lms.wlm.lex_word + st) : -1;
-                const float lnp = wlm_lnp(lms.wlm, S.wctx[tid], wid < 0 ? WLM_OOV : (uint32_t)wid);
-                a = __fadd_rn(a, __fadd_rn(__fmul_rn(lms.alpha, lnp), lms.beta));
+            if constexpr (WORD) {
+                if (S.par[tid] >= 0 && S.last[tid] != lms.wlm.space) {
+                    const int st = S.lex[tid];
+                    const int wid = st > 0 ? __ldg(lms.wlm.lex_word + st) : -1;
+                    const float lnp = wlm_lnp(lms.wlm, S.wctx[tid], wid < 0 ? WLM_OOV : (uint32_t)wid);
+                    a = __fadd_rn(a, __fadd_rn(__fmul_rn(lms.alpha, lnp), lms.beta));
+                }
+            }
+            if constexpr (HOT) {
+                if (hroot >= 0) a = __fadd_rn(a, hot_readout(hot.g, S.hs[tid]));
             }
         }
 #pragma unroll
@@ -678,6 +755,14 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
             n = len;
             int pos = len - 1;
             for (int x = node; x > 0 && x < node_cap && pos >= 0; x = tpar[x]) out_tok[(int64_t)b * tok_stride + pos--] = ttok[x];
+            if constexpr (HOT) {                   // the score without credit: minus the replayed deltas and read-out
+                if (hroot >= 0) {
+                    float cr = 0.f;
+                    int s = hroot;
+                    for (int p = 0; p < n; ++p) cr = __fadd_rn(cr, hot_step(hot.g, hroot, s, out_tok[(int64_t)b * tok_stride + p], &s));
+                    sc = __fsub_rn(sc, __fadd_rn(cr, hot_readout(hot.g, s)));
+                }
+            }
         }
         out_n[b] = n;
         out_score[b] = sc;
@@ -857,26 +942,27 @@ static int check_tables(const char* what, const masr_word_lm_tables* lm, int bla
 
 // The dynamic shared memory attribute of one instantiation, set once per device (never while a graph is being captured:
 // the pool forms are launched eagerly once before their capture).
-template <int MODE, bool POOL>
+template <int MODE, bool POOL, bool HOT>
 static int smem_attr() {
     static bool done[64] = {};
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) dev = 0;
     if (!done[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<MODE, POOL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)sizeof(typename BeamSmem<MODE>::type));
+        cudaError_t e = cudaFuncSetAttribute(prefix_beam_kernel<MODE, POOL, HOT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)sizeof(BeamSmemT<MODE, HOT>));
         if (e != cudaSuccess) { set_last_error("prefix_beam smem attr: %s", cudaGetErrorString(e)); return (int)e; }
         done[dev] = true;
     }
     return MASR_OK;
 }
 
-// `stateful`: the streaming and pool forms, which need state_i / state_f.  `lm`: null without an LM.
-template <int MODE, bool POOL>
+// `stateful`: the streaming and pool forms, which need state_i / state_f.  `lm`: null without an LM.  HOT: `hot` (the
+// graph) and `slot_root` [B] are required.
+template <int MODE, bool POOL, bool HOT = false>
 static int launch_beam(const char* what, bool stateful, const BeamArgs& a,
                        const std::conditional_t<MODE == BEAM_WORD_LM, masr_word_lm_tables, masr_lm_tables>* lm, float alpha,
-                       float beta, void* stream) {
+                       float beta, void* stream, const masr_hotword_graph* hot = nullptr, const int* slot_root = nullptr) {
     constexpr bool LM = MODE != BEAM_PLAIN;
     if (a.B == 0) return MASR_OK;
     MASR_REQUIRE(a.cand_id && a.cand_logp && a.cand_cnt && a.lens && a.pool && a.trie_parent && a.trie_tok && a.out_tok &&
@@ -890,15 +976,23 @@ static int launch_beam(const char* what, bool stateful, const BeamArgs& a,
         else lms.wlm = *lm;
     }
     MASR_REQUIRE(a.beam_size >= 1 && a.beam_size <= BEAM_CAP, "%s: beam_size=%d out of range (1..%d)", what, a.beam_size, BEAM_CAP);
-    const int rc = smem_attr<MODE, POOL>();
+    HotArg<HOT> ha{};
+    if constexpr (HOT) {
+        MASR_REQUIRE(hot && slot_root, "%s: null hotword graph or slot roots", what);
+        MASR_REQUIRE(hot->arc_off && hot->arc_tok && hot->arc_next && hot->fail && hot->tail && hot->leaf && hot->acc &&
+                     hot->ta_acc && hot->fin && hot->nodes >= 1, "%s: hotword graph not set", what);
+        ha.g = *hot;
+        ha.slot_root = slot_root;
+    }
+    const int rc = smem_attr<MODE, POOL, HOT>();
     if (rc) return rc;
     lms.blank_lp = a.blank_logp;
     lms.alpha = alpha;
     lms.beta = beta;
     lms.out_approx = a.out_approx;
-    prefix_beam_kernel<MODE, POOL><<<a.B, BEAM_THREADS, sizeof(typename BeamSmem<MODE>::type), (cudaStream_t)stream>>>(
+    prefix_beam_kernel<MODE, POOL, HOT><<<a.B, BEAM_THREADS, sizeof(BeamSmemT<MODE, HOT>), (cudaStream_t)stream>>>(
         a.cand_id, a.cand_logp, a.cand_cnt, a.bstride, a.lens, a.beam_size, a.blank, a.pool, a.trie_parent, a.trie_tok,
-        a.trie_cap, a.out_tok, a.tok_stride, a.out_n, a.out_score, a.state_i, a.state_f, a.resume, lms, a.fresh);
+        a.trie_cap, a.out_tok, a.tok_stride, a.out_n, a.out_score, a.state_i, a.state_f, a.resume, lms, a.fresh, ha);
     return check_launch(what);
 }
 
@@ -989,6 +1083,139 @@ extern "C" int masr_ctc_prefix_beam_wordlm_pool(const int* cand_id, const float*
     return launch_beam<BEAM_WORD_LM, true>("masr_ctc_prefix_beam_wordlm_pool", true,
         {cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
          state_i, state_f, 0, fresh, out_tok, tok_stride, out_n, out_score, out_approx}, lm_host, alpha, beta, stream);
+}
+
+// ---- the nine hotword entry points: the nine above with the hotword graph (device arrays, masr_hotword_graph) and
+// each slot's root node in it, slot_root [B] (device; -1: that slot searches without hotwords).  Each form's state
+// carries BEAM_CAP more ints (the automaton state of every beam entry): *_hot_state_size.
+extern "C" int masr_ctc_prefix_beam_hot_state_size(int64_t* ints_per_utt, int64_t* floats_per_utt) {
+    MASR_REQUIRE(ints_per_utt && floats_per_utt, "masr_ctc_prefix_beam_hot_state_size: null pointer");
+    *ints_per_utt = 3 * BEAM_CAP + 2 + BEAM_CAP;
+    *floats_per_utt = 3 * BEAM_CAP;
+    return MASR_OK;
+}
+
+extern "C" int masr_ctc_prefix_beam_lm_hot_state_size(int64_t* ints_per_utt, int64_t* floats_per_utt) {
+    MASR_REQUIRE(ints_per_utt && floats_per_utt, "masr_ctc_prefix_beam_lm_hot_state_size: null pointer");
+    *ints_per_utt = LM_STATE_INTS + BEAM_CAP;
+    *floats_per_utt = 3 * BEAM_CAP;
+    return MASR_OK;
+}
+
+extern "C" int masr_ctc_prefix_beam_wordlm_hot_state_size(int64_t* ints_per_utt, int64_t* floats_per_utt) {
+    MASR_REQUIRE(ints_per_utt && floats_per_utt, "masr_ctc_prefix_beam_wordlm_hot_state_size: null pointer");
+    *ints_per_utt = WLM_STATE_INTS + BEAM_CAP;
+    *floats_per_utt = 3 * BEAM_CAP;
+    return MASR_OK;
+}
+
+extern "C" int masr_ctc_prefix_beam_hot(const int* cand_id, const float* cand_logp, const int* cand_cnt, int64_t bstride,
+                                        const int* lens, int B, int beam_size, int blank, float* pool, int* trie_parent,
+                                        int* trie_tok, int64_t trie_cap, int* out_tok, int64_t tok_stride, int* out_n,
+                                        float* out_score, const masr_hotword_graph* hot_host, const int* slot_root,
+                                        void* stream) {
+    return launch_beam<BEAM_PLAIN, false, true>("masr_ctc_prefix_beam_hot", false,
+        {cand_id, cand_logp, cand_cnt, nullptr, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
+         nullptr, nullptr, 0, nullptr, out_tok, tok_stride, out_n, out_score, nullptr}, nullptr, 0.f, 0.f, stream, hot_host,
+        slot_root);
+}
+
+extern "C" int masr_ctc_prefix_beam_hot_stream(const int* cand_id, const float* cand_logp, const int* cand_cnt, int64_t bstride,
+                                               const int* lens, int B, int beam_size, int blank, float* pool, int* trie_parent,
+                                               int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int resume,
+                                               int* out_tok, int64_t tok_stride, int* out_n, float* out_score,
+                                               const masr_hotword_graph* hot_host, const int* slot_root, void* stream) {
+    return launch_beam<BEAM_PLAIN, false, true>("masr_ctc_prefix_beam_hot_stream", true,
+        {cand_id, cand_logp, cand_cnt, nullptr, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
+         state_i, state_f, resume, nullptr, out_tok, tok_stride, out_n, out_score, nullptr}, nullptr, 0.f, 0.f, stream, hot_host,
+        slot_root);
+}
+
+extern "C" int masr_ctc_prefix_beam_hot_pool(const int* cand_id, const float* cand_logp, const int* cand_cnt, int64_t bstride,
+                                             const int* lens, int B, int beam_size, int blank, float* pool, int* trie_parent,
+                                             int* trie_tok, int64_t trie_cap, int* state_i, float* state_f, int* fresh,
+                                             int* out_tok, int64_t tok_stride, int* out_n, float* out_score,
+                                             const masr_hotword_graph* hot_host, const int* slot_root, void* stream) {
+    return launch_beam<BEAM_PLAIN, true, true>("masr_ctc_prefix_beam_hot_pool", true,
+        {cand_id, cand_logp, cand_cnt, nullptr, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
+         state_i, state_f, 0, fresh, out_tok, tok_stride, out_n, out_score, nullptr}, nullptr, 0.f, 0.f, stream, hot_host,
+        slot_root);
+}
+
+extern "C" int masr_ctc_prefix_beam_lm_hot(const int* cand_id, const float* cand_logp, const int* cand_cnt,
+                                           const float* blank_logp, int64_t bstride, const int* lens, int B, int beam_size,
+                                           int blank, const masr_lm_tables* lm_host, float alpha, float beta, float* pool,
+                                           int* trie_parent, int* trie_tok, int64_t trie_cap, int* out_tok, int64_t tok_stride,
+                                           int* out_n, float* out_score, float* out_approx, const masr_hotword_graph* hot_host,
+                                           const int* slot_root, void* stream) {
+    return launch_beam<BEAM_CHAR_LM, false, true>("masr_ctc_prefix_beam_lm_hot", false,
+        {cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
+         nullptr, nullptr, 0, nullptr, out_tok, tok_stride, out_n, out_score, out_approx}, lm_host, alpha, beta, stream,
+        hot_host, slot_root);
+}
+
+extern "C" int masr_ctc_prefix_beam_lm_hot_stream(const int* cand_id, const float* cand_logp, const int* cand_cnt,
+                                                  const float* blank_logp, int64_t bstride, const int* lens, int B, int beam_size,
+                                                  int blank, const masr_lm_tables* lm_host, float alpha, float beta, float* pool,
+                                                  int* trie_parent, int* trie_tok, int64_t trie_cap, int* state_i, float* state_f,
+                                                  int resume, int* out_tok, int64_t tok_stride, int* out_n, float* out_score,
+                                                  float* out_approx, const masr_hotword_graph* hot_host, const int* slot_root,
+                                                  void* stream) {
+    return launch_beam<BEAM_CHAR_LM, false, true>("masr_ctc_prefix_beam_lm_hot_stream", true,
+        {cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
+         state_i, state_f, resume, nullptr, out_tok, tok_stride, out_n, out_score, out_approx}, lm_host, alpha, beta, stream,
+        hot_host, slot_root);
+}
+
+extern "C" int masr_ctc_prefix_beam_lm_hot_pool(const int* cand_id, const float* cand_logp, const int* cand_cnt,
+                                                const float* blank_logp, int64_t bstride, const int* lens, int B, int beam_size,
+                                                int blank, const masr_lm_tables* lm_host, float alpha, float beta, float* pool,
+                                                int* trie_parent, int* trie_tok, int64_t trie_cap, int* state_i, float* state_f,
+                                                int* fresh, int* out_tok, int64_t tok_stride, int* out_n, float* out_score,
+                                                float* out_approx, const masr_hotword_graph* hot_host, const int* slot_root,
+                                                void* stream) {
+    return launch_beam<BEAM_CHAR_LM, true, true>("masr_ctc_prefix_beam_lm_hot_pool", true,
+        {cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
+         state_i, state_f, 0, fresh, out_tok, tok_stride, out_n, out_score, out_approx}, lm_host, alpha, beta, stream,
+        hot_host, slot_root);
+}
+
+extern "C" int masr_ctc_prefix_beam_wordlm_hot(const int* cand_id, const float* cand_logp, const int* cand_cnt,
+                                               const float* blank_logp, int64_t bstride, const int* lens, int B, int beam_size,
+                                               int blank, const masr_word_lm_tables* lm_host, float alpha, float beta,
+                                               float* pool, int* trie_parent, int* trie_tok, int64_t trie_cap, int* out_tok,
+                                               int64_t tok_stride, int* out_n, float* out_score, float* out_approx,
+                                               const masr_hotword_graph* hot_host, const int* slot_root, void* stream) {
+    return launch_beam<BEAM_WORD_LM, false, true>("masr_ctc_prefix_beam_wordlm_hot", false,
+        {cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
+         nullptr, nullptr, 0, nullptr, out_tok, tok_stride, out_n, out_score, out_approx}, lm_host, alpha, beta, stream,
+        hot_host, slot_root);
+}
+
+extern "C" int masr_ctc_prefix_beam_wordlm_hot_stream(const int* cand_id, const float* cand_logp, const int* cand_cnt,
+                                                      const float* blank_logp, int64_t bstride, const int* lens, int B,
+                                                      int beam_size, int blank, const masr_word_lm_tables* lm_host, float alpha,
+                                                      float beta, float* pool, int* trie_parent, int* trie_tok, int64_t trie_cap,
+                                                      int* state_i, float* state_f, int resume, int* out_tok, int64_t tok_stride,
+                                                      int* out_n, float* out_score, float* out_approx,
+                                                      const masr_hotword_graph* hot_host, const int* slot_root, void* stream) {
+    return launch_beam<BEAM_WORD_LM, false, true>("masr_ctc_prefix_beam_wordlm_hot_stream", true,
+        {cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
+         state_i, state_f, resume, nullptr, out_tok, tok_stride, out_n, out_score, out_approx}, lm_host, alpha, beta, stream,
+        hot_host, slot_root);
+}
+
+extern "C" int masr_ctc_prefix_beam_wordlm_hot_pool(const int* cand_id, const float* cand_logp, const int* cand_cnt,
+                                                    const float* blank_logp, int64_t bstride, const int* lens, int B,
+                                                    int beam_size, int blank, const masr_word_lm_tables* lm_host, float alpha,
+                                                    float beta, float* pool, int* trie_parent, int* trie_tok, int64_t trie_cap,
+                                                    int* state_i, float* state_f, int* fresh, int* out_tok, int64_t tok_stride,
+                                                    int* out_n, float* out_score, float* out_approx,
+                                                    const masr_hotword_graph* hot_host, const int* slot_root, void* stream) {
+    return launch_beam<BEAM_WORD_LM, true, true>("masr_ctc_prefix_beam_wordlm_hot_pool", true,
+        {cand_id, cand_logp, cand_cnt, blank_logp, bstride, lens, B, beam_size, blank, pool, trie_parent, trie_tok, trie_cap,
+         state_i, state_f, 0, fresh, out_tok, tok_stride, out_n, out_score, out_approx}, lm_host, alpha, beta, stream,
+        hot_host, slot_root);
 }
 
 extern "C" int masr_ctc_prefix_beam_frames(const int* trie_parent, const int* trie_tok, int64_t trie_cap, const int* out_tok,

@@ -655,15 +655,18 @@ class ConformerEngine:
 
     # ---- CTC prefix beam search (optionally with a character or word LM) ---------------------------------
     def ctc_beam(self, enc: torch.Tensor, out_lens: Sequence[int], T: int, ws, beam_size: int = 300,
-                 cutoff_prob: float = 0.99, cutoff_top_n: int = 40, lm=None, alpha: float = 0.0, beta: float = 0.0):
+                 cutoff_prob: float = 0.99, cutoff_top_n: int = 40, lm=None, alpha: float = 0.0, beta: float = 0.0,
+                 hotwords=None):
         """`ctc_beam_search_decoding(probs, vocab, beam_size, cutoff_prob, cutoff_top_n, scorer, blank_id=0)` of the
         reference's external decoder (masr/decoders/swig_wrapper.py:35-64) for a whole batch on the GPU -> device tensors
         (tokens [B,T], count [B], log-score [B]).  ``lm`` (a masr_b200.lm.CharLM or WordLM, or None): shallow fusion with
         weight ``alpha`` and insertion bonus ``beta`` (a WordLM scores per word and constrains the words to its lexicon); the
         log-score is then the reference's approx_ctc (the fused score with the LM terms taken out again; the fused score is
-        in ws["beam_score"], and ln p_blank per row in ws["blank_lp"]).  Parity unpinned (DESIGN.md)."""
+        in ws["beam_score"], and ln p_blank per row in ws["blank_lp"]).  ``hotwords``: None or a masr_b200.hotwords.HotwordGraph
+        boosted inside the search; the hotword credit steers which prefix is reported, but neither the log-score nor
+        ws["beam_score"] includes it.  Parity unpinned (DESIGN.md)."""
         B, Tb = len(out_lens), max(1, T)
-        settings = (beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta)
+        settings = (beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta, hotwords)
         logits = self.ctc_logits(ws, enc.shape[0])
         if "beam" not in ws or not ws["beam"].fits(B, Tb, *settings):
             ws.pop("beam", None)                      # (the old buffers go back to the allocator before the new ones are taken)
@@ -688,22 +691,23 @@ class ConformerEngine:
 
     def transcribe_beam(self, waves: Sequence[np.ndarray], beam_size: int = 300, cutoff_prob: float = 0.99,
                         cutoff_top_n: int = 40, use_db_normalization: bool = True, target_db: float = -20.0, lm=None,
-                        alpha: float = 0.0, beta: float = 0.0, rates: Optional[Sequence[int]] = None, onsets: bool = False):
-        """Host waveforms -> (token ids per utterance, log-scores) with the GPU prefix beam search (``lm``: see ctc_beam;
-        ``rates``: see transcribe; ``onsets``: see beam_features)."""
+                        alpha: float = 0.0, beta: float = 0.0, rates: Optional[Sequence[int]] = None, onsets: bool = False,
+                        hotwords=None):
+        """Host waveforms -> (token ids per utterance, log-scores) with the GPU prefix beam search (``lm``, ``hotwords``:
+        see ctc_beam; ``rates``: see transcribe; ``onsets``: see beam_features)."""
         feats, frames, status = self.fbank(waves, use_db_normalization, target_db, rates=rates)
-        return self.beam_features(feats, frames, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta, onsets)
+        return self.beam_features(feats, frames, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta, onsets, hotwords)
 
     def transcribe_beam_pipelined(self, batches, beam_size: int = 300, cutoff_prob: float = 0.99, cutoff_top_n: int = 40,
                                   use_db_normalization: bool = True, target_db: float = -20.0, lm=None, alpha: float = 0.0,
-                                  beta: float = 0.0, with_rates: bool = False):
+                                  beta: float = 0.0, with_rates: bool = False, hotwords=None):
         """Generator over ``batches`` (iterable of lists of float32 waveforms; with ``with_rates``, of ``(waves, rates)``
         pairs, see transcribe) yielding ``transcribe_beam(batch)`` per batch, in order, one batch late.  The prefix beam
         search is one CTA per utterance — 32 of 132 SMs busy for milliseconds — so it runs on a SECOND stream, concurrently with the fbank / encoder / top-k kernels of the next batch on the idle SMs
         (two sets of candidate / trie / output buffers; the LM tables are shared read-only).  Same results as the blocking
         call."""
         dev = self.device
-        settings = (beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta)
+        settings = (beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta, hotwords)
         main = torch.cuda.current_stream(dev)
         if getattr(self, "_beam_stream", None) is None:
             self._beam_stream = torch.cuda.Stream(device=dev)
@@ -767,14 +771,14 @@ class ConformerEngine:
             yield finish(prev)
 
     def beam_features(self, feats, frames, beam_size: int = 300, cutoff_prob: float = 0.99, cutoff_top_n: int = 40, lm=None,
-                      alpha: float = 0.0, beta: float = 0.0, onsets: bool = False):
+                      alpha: float = 0.0, beta: float = 0.0, onsets: bool = False, hotwords=None):
         """-> (token ids per utterance, log-scores); ``onsets``: also the onset frame of every token per utterance
-        (BeamSearch.frames), as a third element."""
+        (BeamSearch.frames), as a third element; ``hotwords``: see ctc_beam."""
         B = feats.shape[0]
         enc, tl, T, ws = self.encode(feats, frames)
         if T == 0:
             return ([[] for _ in range(B)], [0.0] * B) + (([[] for _ in range(B)],) if onsets else ())
-        tok, n, sc = self.ctc_beam(enc, tl, T, ws, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta)
+        tok, n, sc = self.ctc_beam(enc, tl, T, ws, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta, hotwords)
         fr = ws["beam"].frames(self, B).cpu().numpy() if onsets else None
         tok, n, sc = tok.cpu().numpy(), n.cpu().numpy(), sc.cpu().numpy()
         self.d2h_bytes += tok.nbytes + n.nbytes + sc.nbytes + (0 if fr is None else fr.nbytes)
@@ -1247,12 +1251,15 @@ class StreamBeam(BeamSearch):
     stay on the device between chunks (the search's streaming form), so after every chunk the best prefix equals the
     whole-utterance search over all frames seen so far.  ``lm`` / ``alpha`` / ``beta``: shallow fusion of a character or
     word LM as in ConformerEngine.ctc_beam (each beam entry's LM window, and with a word LM its lexicon state, is part of
-    the device state); the score is then approx_ctc.
+    the device state); the score is then approx_ctc.  ``hotwords``: None or a masr_b200.hotwords.HotwordGraph boosted
+    inside the search (each beam entry's automaton state is part of the device state; scores exclude the credit).
     Parity unpinned (DESIGN.md)."""
 
     def __init__(self, eng: "ConformerEngine", beam_size: int = 300, cutoff_prob: float = 0.99, cutoff_top_n: int = 40,
-                 max_frames: int = 3000, max_chunk: int = 64, lm=None, alpha: float = 0.0, beta: float = 0.0):
-        super().__init__(eng.device, STREAM, 1, max_chunk, max_frames, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta)
+                 max_frames: int = 3000, max_chunk: int = 64, lm=None, alpha: float = 0.0, beta: float = 0.0,
+                 hotwords=None):
+        super().__init__(eng.device, STREAM, 1, max_chunk, max_frames, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta,
+                         hotwords)
         self.eng, self._own_lm = eng, lm                         # (the search itself holds the LM only weakly)
         self.max_chunk = int(max_chunk)
         self.lens = torch.zeros(1, device=eng.device, dtype=torch.int32)

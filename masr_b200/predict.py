@@ -8,6 +8,10 @@ ids + a score come back (the reference featurises on the CPU, copies features up
 [T,V] posterior down and decodes with numpy — predict.py:181-190, inference_predictor.py:59-64).
 
 Additive entry points (the reference API is single-utterance): ``predict_batch``.
+Hotwords (``decoder: ctc_beam_search`` only): ``MASRPredictor(..., hotwords=[...], hotword_score=1.5)`` boosts those words
+inside the GPU prefix beam search (masr_b200/hotwords.py) for every call; ``predict``, ``predict_batch`` and
+``predict_long`` take a per-call ``hotwords=`` that overrides the list (``[]``: none), and each slot of
+``create_stream_pool`` can have its own (``StreamPool.set_hotwords``).  Scores never include the hotword credit.
 Audio at other sample rates than 16 kHz is resampled on the GPU, as the reference's featurizer does
 (audio_featurizer.py:45-47), when the predictor is built with ``resample=True``; by default a rate mismatch raises.
 Out of the hot-path scope and therefore explicit errors here: punctuation (``use_pun``), inverse
@@ -69,6 +73,8 @@ def chunk_starts(num_frames: int, is_end: bool) -> List[int]:
 
 
 class MASRPredictor:
+    _hotwords = None                      # the predictor's HotwordGraph (None: no hotwords)
+
     def __init__(self,
                  configs=None,
                  model_tag='conformer_streaming_fbank_aishell',
@@ -76,9 +82,15 @@ class MASRPredictor:
                  use_pun=False,
                  pun_model_dir='models/pun_models/',
                  use_gpu=True,
-                 resample=False):
+                 resample=False,
+                 hotwords=None,
+                 hotword_score=1.5):
         """``resample``: accept audio at any sample rate and resample it to ``preprocess_conf.sample_rate`` on the GPU,
-        as the reference's featurizer does (audio_featurizer.py:45-47); False keeps a rate mismatch an error."""
+        as the reference's featurizer does (audio_featurizer.py:45-47); False keeps a rate mismatch an error.
+        ``hotwords``: strings the prefix beam search boosts by ``hotword_score`` per token of every whole hotword a
+        hypothesis contains (longest match; nested hotwords both count); None or ``[]``: no hotwords, the search as
+        without.  A ValueError for hotwords with ``decoder: ctc_greedy``, for a character outside the vocabulary, and for
+        an empty or over-32-token hotword.  The default score of 1.5 is untuned: pick it on your own data."""
         if not configs:
             raise Exception("masr_b200: model download (configs=None, model_tag=...) is not supported; "
                             "pass a YAML path or dict plus model_path")
@@ -117,6 +129,9 @@ class MASRPredictor:
             self.lm = self._load_lm(bc)
             if self.lm is not None:
                 self._beam_conf.update(lm=self.lm, alpha=float(bc.get('alpha', 0.0)), beta=float(bc.get('beta', 0.0)))
+        self._hotword_score = float(hotword_score)
+        self._hotword_graphs = {}
+        self._hotwords = self._graph(hotwords)
         if not os.path.exists(model_path):
             raise Exception("模型文件不存在，请检查{}是否存在！".format(model_path))
         from .squeezeformer import SqueezeformerEngine
@@ -170,6 +185,32 @@ class MASRPredictor:
         logger.info(f'language model: model path = {path}, {lm.describe()}')
         return lm
 
+    def _graph(self, hotwords):
+        """A list of hotwords -> its HotwordGraph (built and checked once per distinct list), None for None or ``[]``."""
+        from .hotwords import HotwordGraph, check_score, outside_lexicon
+        if hotwords is None or len(hotwords) == 0:
+            return None
+        if self._beam_conf is None:
+            raise ValueError("hotwords need the prefix beam search (decoder: ctc_beam_search), not ctc_greedy")
+        check_score(self._hotword_score)
+        key = tuple(hotwords)
+        g = self._hotword_graphs.get(key)
+        if g is None:
+            vocab = self._text_featurizer.vocab_list
+            g = HotwordGraph(hotwords, vocab, self._hotword_score)
+            if getattr(self.lm, "BEAM", "") == "masr_ctc_prefix_beam_wordlm":
+                missing = outside_lexicon(g, vocab, self.lm)
+                if missing:
+                    logger.warning(f"hotwords: the word LM's lexicon lacks {missing}: hotwords using them are never produced")
+            if len(self._hotword_graphs) >= 16:
+                self._hotword_graphs.pop(next(iter(self._hotword_graphs)))
+            self._hotword_graphs[key] = g
+        return g
+
+    def _call_graph(self, hotwords):
+        """The per-call ``hotwords=``: None keeps the predictor's list, a list (``[]`` included) replaces it."""
+        return self._hotwords if hotwords is None else self._graph(hotwords)
+
     def _check_rate(self, sr):
         if sr != self._sample_rate and not self._resample:
             raise Exception(f"masr_b200: resampling is outside the hot-path scope (got {sr} Hz, model expects "
@@ -192,27 +233,28 @@ class MASRPredictor:
             raise Exception("masr_b200: inverse text normalisation (is_itn) is outside the hot-path scope")
         return text
 
-    def predict(self, audio_data, use_pun=False, is_itn=False, sample_rate=16000, timestamps=False):
+    def predict(self, audio_data, use_pun=False, is_itn=False, sample_rate=16000, timestamps=False, hotwords=None):
         """Whole-utterance recognition (predict.py:167-192).  ``timestamps``: the result also carries ``'tokens'``
         (``[{'token', 'start', 'end'}]``, seconds) and, when the vocabulary has ``<space>``, ``'words'``
-        (masr_b200/timestamps.py)."""
-        r = self._recognise(*self._load_batch([audio_data], sample_rate), timestamps)[0]
+        (masr_b200/timestamps.py).  ``hotwords``: this call's list (None: the predictor's; ``[]``: none)."""
+        r = self._recognise(*self._load_batch([audio_data], sample_rate), timestamps, hotwords=self._call_graph(hotwords))[0]
         r['text'] = self._finish(r['text'], use_pun, is_itn)
         return r
 
-    def predict_batch(self, audio_list: Sequence, sample_rate=16000, timestamps=False):
+    def predict_batch(self, audio_list: Sequence, sample_rate=16000, timestamps=False, hotwords=None):
         """Additive: a list of utterances in one GPU pass; element i equals ``predict(audio_list[i])``.  With
-        ``resample=True`` the rows may have different rates (WAV files carry their own).  ``timestamps``: as in predict."""
-        return self._recognise(*self._load_batch(audio_list, sample_rate), timestamps)
+        ``resample=True`` the rows may have different rates (WAV files carry their own).  ``timestamps``, ``hotwords``: as
+        in predict."""
+        return self._recognise(*self._load_batch(audio_list, sample_rate), timestamps, hotwords=self._call_graph(hotwords))
 
-    def _recognise(self, waves, rates, timestamps=False, offsets=None):
+    def _recognise(self, waves, rates, timestamps=False, offsets=None, hotwords=None):
         """Waveforms -> ``[{'text', 'score'}]`` (+ token and word times, shifted by ``offsets[i]`` seconds)."""
         vocab = self._text_featurizer.vocab_list
         dt = ts.frame_seconds(self.predictor)
         offsets = offsets or [0.0] * len(waves)
         if self._beam_conf is not None:
             out = self.predictor.transcribe_beam(waves, use_db_normalization=self._use_db, target_db=self._target_db,
-                                                 rates=rates, onsets=timestamps, **self._beam_conf)
+                                                 rates=rates, onsets=timestamps, hotwords=hotwords, **self._beam_conf)
             res = [{'text': ids_to_text(t, vocab), 'score': s} for t, s in zip(out[0], out[1])]
             if timestamps:
                 for r, t, f, off in zip(res, out[0], out[2], offsets):
@@ -238,7 +280,7 @@ class MASRPredictor:
             loaded_b = (self._load_batch(audio_list, sample_rate) for audio_list in batches)
             for toks, scores in self.predictor.transcribe_beam_pipelined(loaded_b, use_db_normalization=self._use_db,
                                                                          target_db=self._target_db, with_rates=True,
-                                                                         **self._beam_conf):
+                                                                         hotwords=self._hotwords, **self._beam_conf):
                 yield [{'text': ids_to_text(t, vocab), 'score': s} for t, s in zip(toks, scores)]
             return
 
@@ -267,13 +309,14 @@ class MASRPredictor:
             self.vad_predictor = GpuSileroVAD(vad_model_path, device=self.predictor.device)
 
     def predict_long(self, audio_data, use_pun=False, is_itn=False, sample_rate=16000, vad_predictor=None, vad_model_path=None,
-                     timestamps=False):
+                     timestamps=False, hotwords=None):
         """Long-form recognition (predict.py:195-234): VAD segments -> recognise -> join with '，' and average the scores.
         All segments of the recording go through ONE batched GPU pass (``predict_batch``) instead of the reference's
         one-``predict``-per-segment loop; each segment's result equals ``predict(segment)`` (B=1 semantics).
         ``timestamps``: the result also carries ``'sentences'``, one ``{'text', 'score', 'start', 'end', 'tokens'}`` (+
         ``'words'``) per segment with non-empty text: the segment's bounds and its token times, in seconds of the
-        recording."""
+        recording.  ``hotwords``: as in predict, for every segment."""
+        graph = self._call_graph(hotwords)
         self.init_vad(vad_predictor, vad_model_path)
         samples, sr = load_audio(audio_data, sample_rate)
         self._check_rate(sr)
@@ -283,7 +326,7 @@ class MASRPredictor:
         stamps = self.vad_predictor.get_speech_timestamps(samples, sr)
         segs = [samples[t['start']:t['end']] for t in stamps]
         offsets = [t['start'] / sr for t in stamps]
-        results = self._recognise(*self._load_batch(segs, sr), timestamps, offsets) if segs else []
+        results = self._recognise(*self._load_batch(segs, sr), timestamps, offsets, graph) if segs else []
         texts, scores = '', []
         for r in results:
             if r['text'] != '':
@@ -352,7 +395,7 @@ class MASRPredictor:
                 # predict.py:320-322: beam_search_decoder.decode_chunk on this chunk's posteriors (state kept on the device)
                 if self._sbeam is None:
                     from .engine import StreamBeam
-                    self._sbeam = StreamBeam(eng, **self._beam_conf)
+                    self._sbeam = StreamBeam(eng, hotwords=self._hotwords, **self._beam_conf)
                 self._sbeam_result = self._sbeam.push(self._stream.last_logits, int(ids.shape[0]))
                 continue
             ids_h = ids.cpu().numpy()
@@ -386,7 +429,7 @@ class MASRPredictor:
         return ts.greedy_result(r, self._hist_ids, vocab, dt) if timestamps else r
 
     def create_stream_pool(self, n_slots: int, max_frames: int = 3000, vad_model_path=None, vad_options=None,
-                           timestamps=False):
+                           timestamps=False, max_hotword_nodes: int = 0):
         """Additive: a ``StreamPool`` of ``n_slots`` concurrent streams over this predictor's model, decoding as the YAML
         says — greedy, or the GPU prefix beam search with the character or word LM this predictor loaded (if any).  Each slot's
         ``push`` results equal ``predict_stream`` on that stream alone.  ``max_frames``: encoder frames one stream may reach
@@ -397,13 +440,22 @@ class MASRPredictor:
         fresh ``predict_stream`` (masr_b200/segment_pool.py), so a stream may run for any length.
 
         ``timestamps``: every result also carries ``'tokens'`` (+ ``'words'``) as ``predict_stream(..., timestamps=True)``,
-        timed since the slot's reset; with the VAD, segments and partials are timed since the slot's stream started."""
+        timed since the slot's reset; with the VAD, segments and partials are timed since the slot's stream started.
+
+        Hotwords: every slot boosts this predictor's list; ``max_hotword_nodes`` > 0 gives each slot room for its own list
+        of up to that many automaton nodes (a list of n hotwords of k characters takes at most n * k + 1), set with
+        ``set_hotwords(slot, hotwords)`` right after the slot's reset."""
         if not self.configs.streaming:
             raise Exception(f"不支持改该模型流式识别，当前模型：{self.configs.use_model}，参数streaming为：{self.configs.streaming}")
         from .stream_pool import StreamPool
+        beam = self._beam_conf
+        if beam is not None and (self._hotwords is not None or max_hotword_nodes > 0):
+            beam = dict(beam, hotwords=self._hotwords, max_hotword_nodes=int(max_hotword_nodes))
+        elif beam is None and max_hotword_nodes > 0:
+            raise ValueError("hotwords need the prefix beam search (decoder: ctc_beam_search), not ctc_greedy")
         pool = StreamPool(self.predictor, self._text_featurizer.vocab_list, n_slots, use_db_normalization=self._use_db,
-                          target_db=self._target_db, max_frames=max_frames, beam=self._beam_conf, resample=self._resample,
-                          timestamps=timestamps)
+                          target_db=self._target_db, max_frames=max_frames, beam=beam, resample=self._resample,
+                          timestamps=timestamps, hotword_score=self._hotword_score)
         if vad_model_path is None:
             return pool
         from .segment_pool import SegmentingStreamPool

@@ -167,6 +167,13 @@ class SegmentingStreamPool:
         """Start ``slot`` over: VAD state, recogniser stream and transcript."""
         self._clear([slot])
 
+    def set_hotwords(self, slot: int, hotwords):
+        """``StreamPool.set_hotwords`` for ``slot``'s stream: legal while the slot has received no audio since its reset.
+        The list holds for every utterance the VAD cuts from the stream (the per-utterance resets keep it)."""
+        if self.received[slot] != 0:
+            raise ValueError(f"slot {slot} has received audio since its reset: set its hotwords right after a reset")
+        self.pool.set_hotwords(slot, hotwords)
+
     def transcript(self, slot: int) -> dict:
         """The closed segments of the slot's stream joined as ``predict_long`` joins its segments: '，' between non-empty
         texts, the mean score rounded to 2 (0 without segments)."""

@@ -22,6 +22,7 @@ import torch
 from ._lib import EPI_BIAS, EPI_BIAS_GLU, EPI_RESIDUAL
 from .audio import pcm_bytes_to_float32, samples_to_float32
 from .beam import POOL, BeamSearch
+from .hotwords import HotwordBuffer, graph_or_none
 from .engine import ConformerEngine, _p, greedy_score, subsampled_len
 from .predict import CACHED_FEATURE_NUM, DECODING_WINDOW, FRAME_SHIFT, chunk_starts
 from .resample import MODEL_RATE, output_length
@@ -564,17 +565,30 @@ class PoolBeam(BeamSearch):
     prefix equals the whole-utterance search over its frames since the last ``reset`` — what ``predict_stream`` returns.
     The trie is sized by ``beam_size`` and the pool's frame capacity (at most ``beam_size`` new prefixes per frame), so
     no stream the pool accepts can overflow it.  ``lm`` / ``alpha`` / ``beta``: character- or word-LM shallow fusion as in
-    ``StreamBeam``; the reported score is then approx_ctc."""
+    ``StreamBeam``; the reported score is then approx_ctc.
+
+    Hotwords (``hotwords``: the pool default, a ``HotwordGraph`` or None; ``max_hotword_nodes``: the room per slot): one
+    device buffer (``hotwords.HotwordBuffer``) with a region of ``max(max_hotword_nodes, default nodes)`` nodes per slot and
+    one for the default, allocated here, so a slot's graph never moves while the slot is live and the captured step graph
+    stays valid.  ``set_hotwords`` points a slot at the default, at no hotwords or at its own list.  With neither a
+    default nor room per slot the pool searches without the hotword instantiations, exactly as before."""
 
     def __init__(self, pool, beam_size: int = 300, cutoff_prob: float = 0.99, cutoff_top_n: int = 40, lm=None,
-                 alpha: float = 0.0, beta: float = 0.0):
+                 alpha: float = 0.0, beta: float = 0.0, hotwords=None, max_hotword_nodes: int = 0):
         beam_size = int(beam_size)
         if not 1 <= beam_size <= 512:
             raise ValueError(f"beam_size={beam_size} out of range (1..512)")
         S, R = pool.S, pool.OUT_ROWS
         # beam frames one slot can reach: the pool's cap at its output rate (+1: the EfficientConformer halves an odd final chunk up)
         frames = pool.cap * R // CHUNK_OUT + 1
-        super().__init__(pool.eng.device, POOL, S, S * R, frames, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta)
+        buf, roots, self.default_hotwords = None, None, hotwords
+        if hotwords is not None or max_hotword_nodes > 0:
+            buf = HotwordBuffer(pool.eng.device, S + 1, max(int(max_hotword_nodes), 0 if hotwords is None else hotwords.nodes))
+            if hotwords is not None:
+                buf.put(S, hotwords)
+            roots = torch.full((S,), -1 if hotwords is None else buf.root(S), device=pool.eng.device, dtype=torch.int32)
+        super().__init__(pool.eng.device, POOL, S, S * R, frames, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta,
+                         buf, roots)
         # what the launches read from the pool (the pool holds this object: no reference back to it, so dropping a pool frees
         # its CUDA graph at once instead of in a later garbage collection, which may fall inside another pool's capture)
         self.eng, self.R, self.logits = pool.eng, R, pool.b["logits"]
@@ -587,6 +601,20 @@ class PoolBeam(BeamSearch):
         cap = self.trie_cap
         self.fresh[slot] = 1
         self.trie_par[slot * cap + cap // 5:(slot + 1) * cap].fill_(-1)
+
+    def set_hotwords(self, slot: int, graph, default: bool = False):
+        """Slot ``slot`` searches with ``graph`` (copied into its own region), with the pool default (``default``), or
+        without hotwords (graph None, not default).  Outside graph capture, while the slot has no frames since its reset."""
+        if self.hot is None:
+            raise ValueError("this pool was built without hotwords: create it with hotwords or max_hotword_nodes > 0")
+        if default:
+            root = -1 if self.default_hotwords is None else self.hot.root(self.slots)
+        elif graph is None:
+            root = -1
+        else:
+            self.hot.put(slot, graph)
+            root = self.hot.root(slot)
+        self.slot_root[slot] = root
 
     def launch(self):
         """The two launches of one pool step (device inputs only: safe to capture and replay)."""
@@ -634,7 +662,7 @@ class StreamPool:
 
     def __init__(self, eng: ConformerEngine, vocab: Sequence[str], n_slots: int, use_db_normalization: bool = True,
                  target_db: float = -20.0, max_frames: int = 3000, beam: Optional[dict] = None, use_graph: bool = True,
-                 resample: bool = False, timestamps: bool = False):
+                 resample: bool = False, timestamps: bool = False, hotword_score: float = 1.5):
         """``beam``: None decodes greedily (``ctc_greedy``); a dict ``{beam_size, cutoff_prob, cutoff_top_n, lm, alpha,
         beta}`` (``MASRPredictor``'s ``ctc_beam_search`` settings; ``lm`` a ``CharLM``, ``WordLM`` or None) runs the streaming prefix
         beam search of every slot on the GPU (``PoolBeam``), and every result is the beam's, as ``predict_stream`` with
@@ -643,7 +671,11 @@ class StreamPool:
         resample them on the GPU as ``predict_stream`` does; False makes such a push a per-slot error.  ``timestamps``:
         every result also carries ``'tokens'`` (+ ``'words'``) timed since the slot's reset, as ``predict_stream(...,
         timestamps=True)`` returns them, plus ``t0[slot]`` seconds (0 after a reset; a caller that cuts a longer stream
-        into utterances sets it to the utterance's start)."""
+        into utterances sets it to the utterance's start).
+
+        Hotwords (beam search only): ``beam`` may also carry ``hotwords`` (the pool default, a ``HotwordGraph``) and
+        ``max_hotword_nodes`` (automaton nodes each slot's own list may take; ``HotwordBuffer.bytes_per_node`` bytes of
+        device memory per node, per slot).  ``set_hotwords`` gives a slot its own list, scored ``hotword_score`` per token."""
         self.eng, self.vocab, self.S = eng, list(vocab), n_slots
         self.timestamps, self.dt, self.t0 = bool(timestamps), ts.frame_seconds(eng), [0.0] * n_slots
         self.resample = bool(resample)
@@ -654,6 +686,7 @@ class StreamPool:
         if beam is not None:
             self.beam = PoolBeam(self.pool, **beam)
             self.pool.beam = self.beam
+        self.hotword_score = hotword_score
         self.use_db, self.target_db = use_db_normalization, target_db
         self.remained: List[Optional[np.ndarray]] = [None] * n_slots
         dev = eng.device
@@ -720,6 +753,22 @@ class StreamPool:
         self.remained[slot] = None
         self.head[slot], self.count[slot], self.t0[slot] = 0, 0, 0.0
         self._reset_hist([slot])
+
+    def set_hotwords(self, slot: int, hotwords):
+        """The hotwords slot ``slot`` boosts from its next frames on: a list of strings (its own list, which must fit the
+        pool's ``max_hotword_nodes``), ``[]`` (none) or None (back to the pool default).  Legal only while the slot has had no
+        frames since its reset (a ValueError otherwise); the list stays with the slot across later resets until it is set
+        again.  Raises ValueError for a pool that decodes greedily or was built without hotwords."""
+        if self.beam is None:
+            raise ValueError("hotwords need the prefix beam search (decoder: ctc_beam_search)")
+        if not 0 <= slot < self.S:
+            raise ValueError(f"slot {slot} out of range (0..{self.S - 1})")
+        if self.pool.lens_host[slot] != 0:
+            raise ValueError(f"slot {slot} has decoded frames since its reset: set its hotwords right after a reset")
+        if hotwords is None:
+            self.beam.set_hotwords(slot, None, default=True)
+        else:
+            self.beam.set_hotwords(slot, graph_or_none(hotwords, self.vocab, self.hotword_score))
 
     def _dev_index(self, idx: np.ndarray) -> torch.Tensor:
         return torch.from_numpy(idx).to(self.eng.device, non_blocking=False)
