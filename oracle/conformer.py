@@ -139,7 +139,7 @@ def encode(sd, cfg: ConformerConfig, feats: torch.Tensor, taps: Optional[dict] =
     length): ``ConformerEncoder.forward(decoding_chunk_size=-1)`` -> [B,T,d] after ``after_norm``."""
     x = subsample(sd, cfg, feats)
     T = x.shape[1]
-    pos_emb = sinusoid_table(cfg)[None, :T]
+    pos_emb = sinusoid_table(cfg).to(x.dtype)[None, :T]      # (float32 table, widened for a float64 run)
     if taps is not None:
         taps["embed"] = x.clone()
     for i in range(cfg.blocks):

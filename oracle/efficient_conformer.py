@@ -95,7 +95,7 @@ def encoder_layer(sd, i, cfg: EfficientConfig, x, pos_emb):
 
 def encode(sd, cfg: EfficientConfig, feats: torch.Tensor, taps: Optional[dict] = None) -> torch.Tensor:
     x = oc.subsample(sd, cfg, feats)
-    pos_emb = oc.sinusoid_table(cfg)[None, :x.shape[1]]
+    pos_emb = oc.sinusoid_table(cfg).to(x.dtype)[None, :x.shape[1]]
     for i in range(cfg.blocks):
         x = encoder_layer(sd, i, cfg, x, pos_emb)
         if i == cfg.stride_layer:

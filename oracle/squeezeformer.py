@@ -131,7 +131,7 @@ def time_reduce(sd, cfg, x):
 def encode(sd, cfg: SqueezeformerConfig, feats: torch.Tensor, taps: Optional[dict] = None) -> torch.Tensor:
     x = subsample(sd, cfg, feats)
     T = x.shape[1]
-    pos_emb = oc.sinusoid_table(oc.ConformerConfig(d_model=cfg.d_model, max_len=cfg.max_len))[None, :T]
+    pos_emb = oc.sinusoid_table(oc.ConformerConfig(d_model=cfg.d_model, max_len=cfg.max_len)).to(x.dtype)[None, :T]
     x = _ln(sd, "encoder.preln", x)
     saved = None
     for i in range(cfg.blocks):
