@@ -649,6 +649,47 @@ int masr_ctc_prefix_beam_wordlm_hot_pool(const int* cand_id, const float* cand_l
                                          float* out_approx, const masr_hotword_graph* hot_host, const int* slot_root,
                                          void* stream);
 
+/* ---- N-best read-out ------------------------------------------------------------------------------------------------
+ * The reference decoder returns "a list of (log probability, sentence) tuples, sorted by probability, descending"
+ * (masr/decoders/swig_wrapper.py:58,61-64; MASR's wrapper keeps the first, beam_search_decoder.py:56,72,89-91).  These
+ * read the n best hypotheses of slots 0..B-1 out of the beam a streaming or pool search of the matching kind left in
+ * state_i / state_f (the same trie_parent / trie_tok / trie_cap, and with an LM the same tables, alpha and beta; with
+ * hotwords the same graph and slot_root).  The search's state is only read, so the read-out may follow any launch.
+ * Order: the search's own selection score after the read-out terms (the word LM's alpha lnP(last word | h) + beta, the
+ * hotwords' fin(s) - acc(s)), descending, ties to the lower beam rank, so hypothesis 0 is the prefix the search reported.
+ * Per slot b and hypothesis h < out_count[b] = min(n, live beam entries): tokens out_tok[(b*n + h) * tok_stride + p] for
+ * p < out_len[b*n + h], out_score[b*n + h] as the search's out_score (log P without an LM, the fused score with one;
+ * hotword credit taken out) and with an LM out_approx[b*n + h] as its out_approx (approx_ctc).  With an LM the list is
+ * ordered by the fused score, so the approx_ctc values need not decrease down it.  fresh (may be NULL): the pool form's
+ * flags; a slot whose flag is set has no beam yet and reports out_count[b] = 0, nothing else.  n in 1..512; a refused
+ * call writes nothing.  One CTA per slot. */
+int masr_ctc_prefix_beam_nbest(const int* trie_parent, const int* trie_tok, int64_t trie_cap, const int* state_i,
+                               const float* state_f, const int* fresh, int B, int n, int* out_tok, int64_t tok_stride,
+                               int* out_len, float* out_score, int* out_count, void* stream);
+int masr_ctc_prefix_beam_lm_nbest(const int* trie_parent, const int* trie_tok, int64_t trie_cap, const int* state_i,
+                                  const float* state_f, const int* fresh, int B, int n, const masr_lm_tables* lm_host,
+                                  float alpha, float beta, int* out_tok, int64_t tok_stride, int* out_len, float* out_score,
+                                  float* out_approx, int* out_count, void* stream);
+int masr_ctc_prefix_beam_wordlm_nbest(const int* trie_parent, const int* trie_tok, int64_t trie_cap, const int* state_i,
+                                      const float* state_f, const int* fresh, int B, int n, const masr_word_lm_tables* lm_host,
+                                      float alpha, float beta, int* out_tok, int64_t tok_stride, int* out_len,
+                                      float* out_score, float* out_approx, int* out_count, void* stream);
+int masr_ctc_prefix_beam_hot_nbest(const int* trie_parent, const int* trie_tok, int64_t trie_cap, const int* state_i,
+                                   const float* state_f, const int* fresh, int B, int n, int* out_tok, int64_t tok_stride,
+                                   int* out_len, float* out_score, int* out_count, const masr_hotword_graph* hot_host,
+                                   const int* slot_root, void* stream);
+int masr_ctc_prefix_beam_lm_hot_nbest(const int* trie_parent, const int* trie_tok, int64_t trie_cap, const int* state_i,
+                                      const float* state_f, const int* fresh, int B, int n, const masr_lm_tables* lm_host,
+                                      float alpha, float beta, int* out_tok, int64_t tok_stride, int* out_len,
+                                      float* out_score, float* out_approx, int* out_count, const masr_hotword_graph* hot_host,
+                                      const int* slot_root, void* stream);
+int masr_ctc_prefix_beam_wordlm_hot_nbest(const int* trie_parent, const int* trie_tok, int64_t trie_cap, const int* state_i,
+                                          const float* state_f, const int* fresh, int B, int n,
+                                          const masr_word_lm_tables* lm_host, float alpha, float beta, int* out_tok,
+                                          int64_t tok_stride, int* out_len, float* out_score, float* out_approx,
+                                          int* out_count, const masr_hotword_graph* hot_host, const int* slot_root,
+                                          void* stream);
+
 /* The silero VAD network (16 kHz branch of silero_vad.onnx, weights packed by masr_b200/silero.py) over one recording
  * of n_samples 16 kHz samples in windows of `window` samples (512, 1024 or 1536; the last window zero-padded),
  * T = window / 512 recurrent steps per window, N = ceil(n_samples / window) windows.

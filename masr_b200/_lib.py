@@ -158,6 +158,16 @@ SIGNATURES = {
                                                _vp, _i, _vp, _i64, _vp, _vp, _vp, _hgp, _vp, _vp],
     "masr_ctc_prefix_beam_wordlm_hot_pool": [_vp, _vp, _vp, _vp, _i64, _vp, _i, _i, _i, _wlmp, _f, _f, _vp, _vp, _vp, _i64, _vp,
                                              _vp, _vp, _vp, _i64, _vp, _vp, _vp, _hgp, _vp, _vp],
+    "masr_ctc_prefix_beam_nbest": [_vp, _vp, _i64, _vp, _vp, _vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp],
+    "masr_ctc_prefix_beam_lm_nbest": [_vp, _vp, _i64, _vp, _vp, _vp, _i, _i, _lmp, _f, _f, _vp, _i64, _vp, _vp, _vp, _vp,
+                                      _vp],
+    "masr_ctc_prefix_beam_wordlm_nbest": [_vp, _vp, _i64, _vp, _vp, _vp, _i, _i, _wlmp, _f, _f, _vp, _i64, _vp, _vp, _vp,
+                                          _vp, _vp],
+    "masr_ctc_prefix_beam_hot_nbest": [_vp, _vp, _i64, _vp, _vp, _vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _hgp, _vp, _vp],
+    "masr_ctc_prefix_beam_lm_hot_nbest": [_vp, _vp, _i64, _vp, _vp, _vp, _i, _i, _lmp, _f, _f, _vp, _i64, _vp, _vp, _vp,
+                                          _vp, _hgp, _vp, _vp],
+    "masr_ctc_prefix_beam_wordlm_hot_nbest": [_vp, _vp, _i64, _vp, _vp, _vp, _i, _i, _wlmp, _f, _f, _vp, _i64, _vp, _vp,
+                                              _vp, _vp, _hgp, _vp, _vp],
 }
 
 

@@ -8,12 +8,22 @@ from __future__ import annotations
 import ctypes as C
 import weakref
 
+import numpy as np
 import torch
 
 from ._lib import call
 
 BK_MAX = 40                                  # candidates per frame: the largest cutoff_top_n the top-k kernel takes
 ONE_SHOT, STREAM, POOL = "", "_stream", "_pool"      # the forms, named by their entry points' suffix
+
+
+def check_n_best(n_best, beam_size: int) -> int:
+    """``n_best`` as an int in 1..beam_size, else a ValueError."""
+    if isinstance(n_best, bool) or not isinstance(n_best, (int, np.integer)):
+        raise ValueError(f"n_best must be an integer, got {n_best!r}")
+    if not 1 <= int(n_best) <= int(beam_size):
+        raise ValueError(f"n_best={n_best} out of range (1..beam_size={beam_size})")
+    return int(n_best)
 
 
 class BeamSearch:
@@ -79,6 +89,7 @@ class BeamSearch:
         self.score, self.count = self.out[0], self.out[1].view(i32)
         self.fused = self.out[0] if lm is None else self.out[2]
         self.out_frame = None
+        self.nb_tok = None                                 # N-best buffers: allocated by the first ``nbest``
 
     @property
     def lm(self):
@@ -130,3 +141,35 @@ class BeamSearch:
                self.out_tok.data_ptr(), self.max_frames, self.count.data_ptr(), B, self.out_frame.data_ptr(),
                self.max_frames)
         return self.out_frame
+
+    def nbest(self, eng, B: int, n: int):
+        """The ``n`` best hypotheses of slots 0..B-1 from the beam the last ``search`` left (STREAM and POOL only) ->
+        device tensors (tokens [slots, n, max_frames], count [slots, n], score [slots, n], fused [slots, n], hypotheses
+        [slots]): hypothesis h of slot b, h < hypotheses[b], ranked as the search ranks its result, so h = 0 is its
+        ``out_tok`` / ``count`` / ``score`` / ``fused``; ``score`` is approx_ctc with an LM, and need not decrease down the
+        list then (the list is ordered by ``fused``).  A POOL slot that is still fresh reports 0.  One launch after ``search``, on the
+        same stream, never inside a graph capture: the buffers are allocated on first use (and again for a larger n)."""
+        if self.form == ONE_SHOT:
+            raise ValueError("the N-best read-out needs the beam the streaming or pool form keeps")
+        if not 1 <= int(n) <= self.beam:
+            raise ValueError(f"n={n} out of range (1..{self.beam})")
+        n = int(n)
+        if self.nb_tok is None or self.nb_tok.shape[1] < n:
+            dev = self.device
+            self.nb_tok = torch.zeros(self.slots, n, self.max_frames, device=dev, dtype=torch.int32)
+            self.nb_out = torch.zeros(3, self.slots, n, device=dev, dtype=torch.float32)
+            self.nb_n = torch.zeros(self.slots, device=dev, dtype=torch.int32)
+        tok, out = self.nb_tok.view(-1)[:self.slots * n * self.max_frames], self.nb_out.view(3, -1)[:, :self.slots * n]
+        score, count = out[0], out[1].view(torch.int32)
+        if self._lm is None:
+            fusion, scores = (), (score.data_ptr(),)
+        else:                        # as search: the fused score to out_score, approx_ctc to out_approx
+            fusion, scores = (C.byref(self.lm.tables(self.device)), self.alpha, self.beta), (out[2].data_ptr(), score.data_ptr())
+        hot = () if self.hot is None else (C.byref(self.hot.tables(self.device)), self.slot_root.data_ptr())
+        base = self.name[:-len(self.form)]
+        eng._k("beam_nbest", base + "_nbest", self.trie_par.data_ptr(), self.trie_tok.data_ptr(), self.trie_cap,
+               self.state_i.data_ptr(), self.state_f.data_ptr(), self.fresh.data_ptr() if self.form == POOL else None, B, n,
+               *fusion, tok.data_ptr(), self.max_frames, count.data_ptr(), *scores, self.nb_n.data_ptr(), *hot)
+        S = self.slots
+        fused = score if self._lm is None else out[2]
+        return (tok.view(S, n, self.max_frames), count.view(S, n), score.view(S, n), fused.view(S, n), self.nb_n)

@@ -266,6 +266,100 @@ __device__ __forceinline__ float hot_readout(const masr_hotword_graph& g, int s)
 constexpr int LM_STATE_INTS = 3 * BEAM_CAP + 2 + BEAM_CAP * LM_CTX / 2;   // + the windows, two ids per int
 constexpr int WLM_STATE_INTS = 3 * BEAM_CAP + 2 + BEAM_CAP * (WLM_CTX + 1);   // + the word windows and lexicon states
 
+// ---- the read-out after the last frame, shared by prefix_beam_kernel (the entry it reports) and prefix_nbest_kernel
+// (its N best entries), so that hypothesis 0 of the one is the other's result bit for bit ----
+
+// An entry's selection score at read-out: its score, plus (WORD) alpha lnP(last word | h) + beta for a non-empty entry
+// not ending in <space>, plus (HOT) the hotword read-out fin(s) - acc(s).  Computed on the side: the state never sees it.
+template <int MODE, bool HOT>
+__device__ __forceinline__ float readout_score(float score, int par, int last, int lex, const uint32_t* wctx, int hs,
+                                               int hroot, const LmSearch& lms, const HotArg<HOT>& hot) {
+    float a = score;
+    if constexpr (MODE == BEAM_WORD_LM) {
+        if (par >= 0 && last != lms.wlm.space) {
+            const int wid = lex > 0 ? __ldg(lms.wlm.lex_word + lex) : -1;
+            const float lnp = wlm_lnp(lms.wlm, wctx, wid < 0 ? WLM_OOV : (uint32_t)wid);
+            a = __fadd_rn(a, __fadd_rn(__fmul_rn(lms.alpha, lnp), lms.beta));
+        }
+    }
+    if constexpr (HOT) {
+        if (hroot >= 0) a = __fadd_rn(a, hot_readout(hot.g, hs));
+    }
+    return a;
+}
+
+// The hypothesis of trie node `node` whose selection score is `sel`: its tokens -> tok[0, len) (the walk stops at the root
+// or at a node past node_cap), *score = sel without the hotword credit (its tokens' deltas replayed, plus its read-out),
+// and (LM) *approx = approx_ctc: score - len * beta - alpha * lnP(sentence).  Returns len.  One thread.
+template <int MODE, bool HOT>
+__device__ __forceinline__ int readout_hyp(int node, float sel, const int* tpar, const int* ttok, int64_t node_cap, int* tok,
+                                           int hroot, const LmSearch& lms, const HotArg<HOT>& hot, float* score,
+                                           float* approx) {
+    float sc = sel;
+    int len = 0;
+    for (int x = node; x > 0 && x < node_cap; x = tpar[x]) ++len;
+    const int n = len;
+    int pos = len - 1;
+    for (int x = node; x > 0 && x < node_cap && pos >= 0; x = tpar[x]) tok[pos--] = ttok[x];
+    if constexpr (HOT) {                       // the score without credit: minus the replayed deltas and read-out
+        if (hroot >= 0) {
+            float cr = 0.f;
+            int s = hroot;
+            for (int p = 0; p < n; ++p) cr = __fadd_rn(cr, hot_step(hot.g, hroot, s, tok[p], &s));
+            sc = __fsub_rn(sc, __fadd_rn(cr, hot_readout(hot.g, s)));
+        }
+    }
+    *score = sc;
+    if constexpr (MODE == BEAM_WORD_LM) {
+        // approx_ctc: score' - len * beta - alpha * lnP(sentence) over the words split on <space> (a trailing partial
+        // word is one; a partial that is not a word end is out of vocabulary)
+        const masr_word_lm_tables& lm = lms.wlm;
+        const int n1 = lm.order - 1;
+        uint32_t win[WLM_CTX];
+#pragma unroll
+        for (int j = 0; j < WLM_CTX; ++j) win[j] = (uint32_t)lm.bos;
+        float s = 0.f;
+        int nw = 0, ln = 0;
+        for (int p = 0; p <= n; ++p) {
+            const int t = p < n ? tok[p] : lm.space;
+            if (t != lm.space) {
+                ln = ln >= 0 ? lex_child(lm, ln, t) : -1;
+                continue;
+            }
+            if (ln == 0) continue;                                  // (no letters since the last <space>)
+            const int wid = ln > 0 ? __ldg(lm.lex_word + ln) : -1;
+            const uint32_t w = wid < 0 ? WLM_OOV : (uint32_t)wid;
+            s = __fadd_rn(s, wlm_lnp(lm, win, w));
+            for (int j = 0; j + 1 < n1; ++j) win[j] = win[j + 1];
+            if (n1 > 0) win[n1 - 1] = w;
+            ++nw;
+            ln = 0;
+        }
+        if (nw == 0) s = wlm_lnp(lm, win, (uint32_t)lm.bos);
+        s = __fadd_rn(s, wlm_lnp(lm, win, (uint32_t)lm.eos));
+        *approx = __fsub_rn(__fsub_rn(sc, __fmul_rn((float)n, lms.beta)), __fmul_rn(lms.alpha, s));
+    }
+    if constexpr (MODE == BEAM_CHAR_LM) {
+        // approx_ctc: score - len * beta - alpha * lnP(sentence), sentence = <s>^(N-1) tokens </s> (<s>^N </s> if empty)
+        const masr_lm_tables& lm = lms.lm;
+        const int n1 = lm.order - 1;
+        uint16_t win[LM_CTX];
+#pragma unroll
+        for (int j = 0; j < LM_CTX; ++j) win[j] = (uint16_t)lm.bos;
+        float s = 0.f;
+        if (n == 0) s = lm_lnp(lm, win, (uint32_t)lm.bos);
+        for (int p = 0; p < n; ++p) {
+            const uint16_t w = lm_word(lm, tok[p]);
+            s = __fadd_rn(s, lm_lnp(lm, win, w));
+            for (int j = 0; j + 1 < n1; ++j) win[j] = win[j + 1];
+            if (n1 > 0) win[n1 - 1] = w;
+        }
+        s = __fadd_rn(s, lm_lnp(lm, win, (uint32_t)lm.eos));
+        *approx = __fsub_rn(__fsub_rn(sc, __fmul_rn((float)n, lms.beta)), __fmul_rn(lms.alpha, s));
+    }
+    return n;
+}
+
 // pool layout: [0, BEAM_CAP) existing prefixes (rank order), then BEAM_CAP + i*K + k children of (rank i, candidate k);
 // K = this frame's candidate count (usually a handful, cutoff_prob 0.99), so the pool the selection scans is 512 + beam*K
 // entries, not 512 + beam*40
@@ -704,28 +798,19 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
         }
         if (tid == 0) { st_i[3 * BEAM_CAP] = nbeam; st_i[3 * BEAM_CAP + 1] = nnodes; }
     }
-    // the entry to report: rank 0, or (WORD) the best after the read-out term, which is computed on the side (the state
-    // saved above never sees it): alpha lnP(last word | h) + beta for every non-empty entry not ending in <space>;
-    // (HOT) plus the hotword read-out fin(s) - acc(s)
+    // the entry to report: rank 0, or (WORD, HOT) the best after the read-out terms (readout_score), ties to the lower rank
     int best = 0;
     float best_sc = nbeam > 0 ? S.score[0] : -INFINITY;
     if constexpr (WORD || HOT) {
         float a = -INFINITY;
         int ai = 0x7fffffff;
         if (tid < nbeam) {
-            a = S.score[tid];
+            const uint32_t* wctx = nullptr;
+            int lex = 0, hs = -1;
+            if constexpr (WORD) { wctx = S.wctx[tid]; lex = S.lex[tid]; }
+            if constexpr (HOT) hs = S.hs[tid];
+            a = readout_score<MODE, HOT>(S.score[tid], S.par[tid], S.last[tid], lex, wctx, hs, hroot, lms, hot);
             ai = tid;
-            if constexpr (WORD) {
-                if (S.par[tid] >= 0 && S.last[tid] != lms.wlm.space) {
-                    const int st = S.lex[tid];
-                    const int wid = st > 0 ? __ldg(lms.wlm.lex_word + st) : -1;
-                    const float lnp = wlm_lnp(lms.wlm, S.wctx[tid], wid < 0 ? WLM_OOV : (uint32_t)wid);
-                    a = __fadd_rn(a, __fadd_rn(__fmul_rn(lms.alpha, lnp), lms.beta));
-                }
-            }
-            if constexpr (HOT) {
-                if (hroot >= 0) a = __fadd_rn(a, hot_readout(hot.g, S.hs[tid]));
-            }
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
@@ -746,81 +831,13 @@ __global__ void __launch_bounds__(BEAM_THREADS) prefix_beam_kernel(
     }
     if (tid == 0) {
         int n = 0;
-        float sc = -INFINITY;
-        if (nbeam > 0) {
-            sc = best_sc;
-            int node = S.node[best];
-            int len = 0;
-            for (int x = node; x > 0 && x < node_cap; x = tpar[x]) ++len;
-            n = len;
-            int pos = len - 1;
-            for (int x = node; x > 0 && x < node_cap && pos >= 0; x = tpar[x]) out_tok[(int64_t)b * tok_stride + pos--] = ttok[x];
-            if constexpr (HOT) {                   // the score without credit: minus the replayed deltas and read-out
-                if (hroot >= 0) {
-                    float cr = 0.f;
-                    int s = hroot;
-                    for (int p = 0; p < n; ++p) cr = __fadd_rn(cr, hot_step(hot.g, hroot, s, out_tok[(int64_t)b * tok_stride + p], &s));
-                    sc = __fsub_rn(sc, __fadd_rn(cr, hot_readout(hot.g, s)));
-                }
-            }
-        }
+        float sc = -INFINITY, apx = -INFINITY;
+        if (nbeam > 0)
+            n = readout_hyp<MODE, HOT>(S.node[best], best_sc, tpar, ttok, node_cap, out_tok + (int64_t)b * tok_stride, hroot,
+                                       lms, hot, &sc, &apx);
         out_n[b] = n;
         out_score[b] = sc;
-        if constexpr (WORD) {
-            // approx_ctc: score' - len * beta - alpha * lnP(sentence) over the words split on <space> (a trailing partial
-            // word is one; a partial that is not a word end is out of vocabulary)
-            float apx = sc;
-            if (nbeam > 0) {
-                const masr_word_lm_tables& lm = lms.wlm;
-                const int n1 = lm.order - 1;
-                uint32_t win[WLM_CTX];
-#pragma unroll
-                for (int j = 0; j < WLM_CTX; ++j) win[j] = (uint32_t)lm.bos;
-                float s = 0.f;
-                int nw = 0, ln = 0;
-                for (int p = 0; p <= n; ++p) {
-                    const int tok = p < n ? out_tok[(int64_t)b * tok_stride + p] : lm.space;
-                    if (tok != lm.space) {
-                        ln = ln >= 0 ? lex_child(lm, ln, tok) : -1;
-                        continue;
-                    }
-                    if (ln == 0) continue;                              // (no letters since the last <space>)
-                    const int wid = ln > 0 ? __ldg(lm.lex_word + ln) : -1;
-                    const uint32_t w = wid < 0 ? WLM_OOV : (uint32_t)wid;
-                    s = __fadd_rn(s, wlm_lnp(lm, win, w));
-                    for (int j = 0; j + 1 < n1; ++j) win[j] = win[j + 1];
-                    if (n1 > 0) win[n1 - 1] = w;
-                    ++nw;
-                    ln = 0;
-                }
-                if (nw == 0) s = wlm_lnp(lm, win, (uint32_t)lm.bos);
-                s = __fadd_rn(s, wlm_lnp(lm, win, (uint32_t)lm.eos));
-                apx = __fsub_rn(__fsub_rn(sc, __fmul_rn((float)n, lms.beta)), __fmul_rn(lms.alpha, s));
-            }
-            lms.out_approx[b] = apx;
-        }
-        if constexpr (CHAR) {
-            // approx_ctc: score - len * beta - alpha * lnP(sentence), sentence = <s>^(N-1) tokens </s> (<s>^N </s> if empty)
-            float apx = sc;
-            if (nbeam > 0) {
-                const masr_lm_tables& lm = lms.lm;
-                const int n1 = lm.order - 1;
-                uint16_t win[LM_CTX];
-#pragma unroll
-                for (int j = 0; j < LM_CTX; ++j) win[j] = (uint16_t)lm.bos;
-                float s = 0.f;
-                if (n == 0) s = lm_lnp(lm, win, (uint32_t)lm.bos);
-                for (int p = 0; p < n; ++p) {
-                    const uint16_t w = lm_word(lm, out_tok[(int64_t)b * tok_stride + p]);
-                    s = __fadd_rn(s, lm_lnp(lm, win, w));
-                    for (int j = 0; j + 1 < n1; ++j) win[j] = win[j + 1];
-                    if (n1 > 0) win[n1 - 1] = w;
-                }
-                s = __fadd_rn(s, lm_lnp(lm, win, (uint32_t)lm.eos));
-                apx = __fsub_rn(__fsub_rn(sc, __fmul_rn((float)n, lms.beta)), __fmul_rn(lms.alpha, s));
-            }
-            lms.out_approx[b] = apx;
-        }
+        if constexpr (LM) lms.out_approx[b] = apx;
     }
 }
 
@@ -844,6 +861,66 @@ __global__ void __launch_bounds__(32) prefix_frames_kernel(const int* __restrict
         if (node >= 0) node = trie_find(tpar + node_cap, tpar, ttok, hcap, node, out_tok[(int64_t)b * tok_stride + p]);
         out_frame[(int64_t)b * tok_stride_f + p] = node >= 0 ? tonset[node] : -1;
     }
+}
+
+// The N best hypotheses of each slot's saved beam (the streaming and pool forms' state_i / state_f and trie), one CTA per
+// slot and one thread per beam entry: each entry's selection score at read-out (readout_score), its rank in the total
+// order (selection score descending, then beam rank ascending) by counting, and the entries ranked below n read out
+// their hypothesis (readout_hyp) into row `rank`, so hypothesis 0 is the entry the search reported.  A slot whose
+// fresh[b] is set (pool forms) has no beam yet: it reports 0 hypotheses and nothing else is written.
+template <int MODE, bool HOT>
+__global__ void __launch_bounds__(BEAM_THREADS) prefix_nbest_kernel(
+    const int* __restrict__ trie_parent, const int* __restrict__ trie_tok, int64_t trie_cap, const int* __restrict__ state_i,
+    const float* __restrict__ state_f, const int* __restrict__ fresh, int n, const LmSearch lms, const HotArg<HOT> hot,
+    int* __restrict__ out_tok, int64_t tok_stride, int* __restrict__ out_len, float* __restrict__ out_score,
+    float* __restrict__ out_approx, int* __restrict__ out_count) {
+    constexpr bool WORD = MODE == BEAM_WORD_LM, CHAR = MODE == BEAM_CHAR_LM;
+    constexpr int ST_INTS = (WORD ? WLM_STATE_INTS : CHAR ? LM_STATE_INTS : 3 * BEAM_CAP + 2) + (HOT ? BEAM_CAP : 0);
+    __shared__ float s_sel[BEAM_CAP];
+    const int b = blockIdx.x, tid = threadIdx.x;
+    if (fresh && fresh[b]) {                                        // (uniform across the CTA)
+        if (tid == 0) out_count[b] = 0;
+        return;
+    }
+    const int* st_i = state_i + (int64_t)b * ST_INTS;
+    const float* st_f = state_f + (int64_t)b * (3 * BEAM_CAP);
+    const int nbeam = st_i[3 * BEAM_CAP];
+    const int64_t node_cap = trie_cap / 5;
+    int hroot = -1;
+    if constexpr (HOT) hroot = hot.slot_root[b];
+    float sel = -INFINITY;
+    if (tid < nbeam) {
+        uint32_t wctx[WLM_CTX > 0 ? WLM_CTX : 1];
+        int lex = 0, hs = -1;
+        if constexpr (WORD) {
+            const int* w = st_i + 3 * BEAM_CAP + 2 + tid * (WLM_CTX + 1);
+#pragma unroll
+            for (int j = 0; j < WLM_CTX; ++j) wctx[j] = (uint32_t)w[j];
+            lex = w[WLM_CTX];
+        }
+        if constexpr (HOT) hs = st_i[ST_INTS - BEAM_CAP + tid];
+        sel = readout_score<MODE, HOT>(st_f[2 * BEAM_CAP + tid], st_i[BEAM_CAP + tid], st_i[2 * BEAM_CAP + tid], lex, wctx, hs,
+                                       hroot, lms, hot);
+        s_sel[tid] = sel;
+    }
+    __syncthreads();
+    if (tid < nbeam) {
+        int rank = 0;                                               // entries before this one in the total order
+        for (int j = 0; j < nbeam; ++j) {
+            const float o = s_sel[j];
+            rank += (o > sel) | ((o == sel) & (j < tid));
+        }
+        if (rank < n) {
+            const int64_t h = (int64_t)b * n + rank;
+            float sc, apx = 0.f;
+            out_len[h] = readout_hyp<MODE, HOT>(st_i[tid], sel, trie_parent + (int64_t)b * trie_cap,
+                                                trie_tok + (int64_t)b * trie_cap, node_cap, out_tok + h * tok_stride, hroot,
+                                                lms, hot, &sc, &apx);
+            out_score[h] = sc;
+            if constexpr (WORD || CHAR) out_approx[h] = apx;
+        }
+    }
+    if (tid == 0) out_count[b] = min(n, nbeam);
 }
 
 }  // namespace masr
@@ -1227,4 +1304,101 @@ extern "C" int masr_ctc_prefix_beam_frames(const int* trie_parent, const int* tr
     prefix_frames_kernel<<<B, 32, 0, (cudaStream_t)stream>>>(trie_parent, trie_tok, trie_cap, out_tok, tok_stride, out_n,
                                                               out_frame, tok_stride_f);
     return check_launch("prefix_frames_kernel");
+}
+
+// ---- the six N-best read-outs: {no LM, character LM, word LM} x {without, with hotwords}, after a streaming or pool
+// search of the matching kind (its trie, state and, with hotwords, graph and slot roots).  `fresh` may be null (the
+// streaming form); B = 0 writes nothing.
+template <int MODE, bool HOT = false>
+static int launch_nbest(const char* what, const int* trie_parent, const int* trie_tok, int64_t trie_cap, const int* state_i,
+                        const float* state_f, const int* fresh, int B, int n,
+                        const std::conditional_t<MODE == BEAM_WORD_LM, masr_word_lm_tables, masr_lm_tables>* lm, float alpha,
+                        float beta, int* out_tok, int64_t tok_stride, int* out_len, float* out_score, float* out_approx,
+                        int* out_count, void* stream, const masr_hotword_graph* hot = nullptr, const int* slot_root = nullptr) {
+    constexpr bool LM = MODE != BEAM_PLAIN;
+    if (B == 0) return MASR_OK;
+    MASR_REQUIRE(trie_parent && trie_tok && state_i && state_f && out_tok && out_len && out_score && out_count &&
+                 (!LM || (lm && out_approx)), "%s: null pointer", what);
+    MASR_REQUIRE(B > 0 && trie_cap >= 5, "%s: B=%d, trie_cap=%lld out of range", what, B, (long long)trie_cap);
+    MASR_REQUIRE(n >= 1 && n <= BEAM_CAP, "%s: n=%d out of range (1..%d)", what, n, BEAM_CAP);
+    MASR_REQUIRE(tok_stride >= 0, "%s: tok_stride=%lld out of range", what, (long long)tok_stride);
+    LmSearch lms{};
+    if constexpr (LM) {
+        const int rc = check_tables(what, lm, -1);
+        if (rc) return rc;
+        if constexpr (MODE == BEAM_CHAR_LM) lms.lm = *lm;
+        else lms.wlm = *lm;
+    }
+    lms.alpha = alpha;
+    lms.beta = beta;
+    HotArg<HOT> ha{};
+    if constexpr (HOT) {
+        MASR_REQUIRE(hot && slot_root, "%s: null hotword graph or slot roots", what);
+        MASR_REQUIRE(hot->arc_off && hot->arc_tok && hot->arc_next && hot->fail && hot->tail && hot->leaf && hot->acc &&
+                     hot->ta_acc && hot->fin && hot->nodes >= 1, "%s: hotword graph not set", what);
+        ha.g = *hot;
+        ha.slot_root = slot_root;
+    }
+    prefix_nbest_kernel<MODE, HOT><<<B, BEAM_THREADS, 0, (cudaStream_t)stream>>>(
+        trie_parent, trie_tok, trie_cap, state_i, state_f, fresh, n, lms, ha, out_tok, tok_stride, out_len, out_score,
+        out_approx, out_count);
+    return check_launch(what);
+}
+
+extern "C" int masr_ctc_prefix_beam_nbest(const int* trie_parent, const int* trie_tok, int64_t trie_cap, const int* state_i,
+                                          const float* state_f, const int* fresh, int B, int n, int* out_tok,
+                                          int64_t tok_stride, int* out_len, float* out_score, int* out_count, void* stream) {
+    return launch_nbest<BEAM_PLAIN>("masr_ctc_prefix_beam_nbest", trie_parent, trie_tok, trie_cap, state_i, state_f, fresh, B,
+                                    n, nullptr, 0.f, 0.f, out_tok, tok_stride, out_len, out_score, nullptr, out_count, stream);
+}
+
+extern "C" int masr_ctc_prefix_beam_lm_nbest(const int* trie_parent, const int* trie_tok, int64_t trie_cap, const int* state_i,
+                                             const float* state_f, const int* fresh, int B, int n,
+                                             const masr_lm_tables* lm_host, float alpha, float beta, int* out_tok,
+                                             int64_t tok_stride, int* out_len, float* out_score, float* out_approx,
+                                             int* out_count, void* stream) {
+    return launch_nbest<BEAM_CHAR_LM>("masr_ctc_prefix_beam_lm_nbest", trie_parent, trie_tok, trie_cap, state_i, state_f,
+                                      fresh, B, n, lm_host, alpha, beta, out_tok, tok_stride, out_len, out_score, out_approx,
+                                      out_count, stream);
+}
+
+extern "C" int masr_ctc_prefix_beam_wordlm_nbest(const int* trie_parent, const int* trie_tok, int64_t trie_cap,
+                                                 const int* state_i, const float* state_f, const int* fresh, int B, int n,
+                                                 const masr_word_lm_tables* lm_host, float alpha, float beta, int* out_tok,
+                                                 int64_t tok_stride, int* out_len, float* out_score, float* out_approx,
+                                                 int* out_count, void* stream) {
+    return launch_nbest<BEAM_WORD_LM>("masr_ctc_prefix_beam_wordlm_nbest", trie_parent, trie_tok, trie_cap, state_i, state_f,
+                                      fresh, B, n, lm_host, alpha, beta, out_tok, tok_stride, out_len, out_score, out_approx,
+                                      out_count, stream);
+}
+
+extern "C" int masr_ctc_prefix_beam_hot_nbest(const int* trie_parent, const int* trie_tok, int64_t trie_cap, const int* state_i,
+                                              const float* state_f, const int* fresh, int B, int n, int* out_tok,
+                                              int64_t tok_stride, int* out_len, float* out_score, int* out_count,
+                                              const masr_hotword_graph* hot_host, const int* slot_root, void* stream) {
+    return launch_nbest<BEAM_PLAIN, true>("masr_ctc_prefix_beam_hot_nbest", trie_parent, trie_tok, trie_cap, state_i, state_f,
+                                          fresh, B, n, nullptr, 0.f, 0.f, out_tok, tok_stride, out_len, out_score, nullptr,
+                                          out_count, stream, hot_host, slot_root);
+}
+
+extern "C" int masr_ctc_prefix_beam_lm_hot_nbest(const int* trie_parent, const int* trie_tok, int64_t trie_cap,
+                                                 const int* state_i, const float* state_f, const int* fresh, int B, int n,
+                                                 const masr_lm_tables* lm_host, float alpha, float beta, int* out_tok,
+                                                 int64_t tok_stride, int* out_len, float* out_score, float* out_approx,
+                                                 int* out_count, const masr_hotword_graph* hot_host, const int* slot_root,
+                                                 void* stream) {
+    return launch_nbest<BEAM_CHAR_LM, true>("masr_ctc_prefix_beam_lm_hot_nbest", trie_parent, trie_tok, trie_cap, state_i,
+                                            state_f, fresh, B, n, lm_host, alpha, beta, out_tok, tok_stride, out_len,
+                                            out_score, out_approx, out_count, stream, hot_host, slot_root);
+}
+
+extern "C" int masr_ctc_prefix_beam_wordlm_hot_nbest(const int* trie_parent, const int* trie_tok, int64_t trie_cap,
+                                                     const int* state_i, const float* state_f, const int* fresh, int B, int n,
+                                                     const masr_word_lm_tables* lm_host, float alpha, float beta,
+                                                     int* out_tok, int64_t tok_stride, int* out_len, float* out_score,
+                                                     float* out_approx, int* out_count, const masr_hotword_graph* hot_host,
+                                                     const int* slot_root, void* stream) {
+    return launch_nbest<BEAM_WORD_LM, true>("masr_ctc_prefix_beam_wordlm_hot_nbest", trie_parent, trie_tok, trie_cap, state_i,
+                                            state_f, fresh, B, n, lm_host, alpha, beta, out_tok, tok_stride, out_len,
+                                            out_score, out_approx, out_count, stream, hot_host, slot_root);
 }

@@ -656,7 +656,7 @@ class ConformerEngine:
     # ---- CTC prefix beam search (optionally with a character or word LM) ---------------------------------
     def ctc_beam(self, enc: torch.Tensor, out_lens: Sequence[int], T: int, ws, beam_size: int = 300,
                  cutoff_prob: float = 0.99, cutoff_top_n: int = 40, lm=None, alpha: float = 0.0, beta: float = 0.0,
-                 hotwords=None):
+                 hotwords=None, n_best=None):
         """`ctc_beam_search_decoding(probs, vocab, beam_size, cutoff_prob, cutoff_top_n, scorer, blank_id=0)` of the
         reference's external decoder (masr/decoders/swig_wrapper.py:35-64) for a whole batch on the GPU -> device tensors
         (tokens [B,T], count [B], log-score [B]).  ``lm`` (a masr_b200.lm.CharLM or WordLM, or None): shallow fusion with
@@ -664,13 +664,16 @@ class ConformerEngine:
         log-score is then the reference's approx_ctc (the fused score with the LM terms taken out again; the fused score is
         in ws["beam_score"], and ln p_blank per row in ws["blank_lp"]).  ``hotwords``: None or a masr_b200.hotwords.HotwordGraph
         boosted inside the search; the hotword credit steers which prefix is reported, but neither the log-score nor
-        ws["beam_score"] includes it.  Parity unpinned (DESIGN.md)."""
+        ws["beam_score"] includes it.  ``n_best`` > 1: the search runs in its streaming form from the root (resume = 0,
+        bit for bit the one-shot search) so that its final beam stays on the device for ``ws["beam"].nbest``.
+        Parity unpinned (DESIGN.md)."""
         B, Tb = len(out_lens), max(1, T)
         settings = (beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta, hotwords)
+        form = STREAM if n_best is not None and n_best > 1 else ONE_SHOT
         logits = self.ctc_logits(ws, enc.shape[0])
-        if "beam" not in ws or not ws["beam"].fits(B, Tb, *settings):
+        if "beam" not in ws or ws["beam"].form != form or not ws["beam"].fits(B, Tb, *settings):
             ws.pop("beam", None)                      # (the old buffers go back to the allocator before the new ones are taken)
-            ws["beam"] = BeamSearch(self.device, ONE_SHOT, B, B * Tb, Tb, *settings)
+            ws["beam"] = BeamSearch(self.device, form, B, B * Tb, Tb, *settings)
         bs = ws["beam"]
         ws["beam_score"], ws["blank_lp"] = bs.fused, bs.blank_lp
         bs.topk(self, logits, self.Vpad, B * T)
@@ -692,11 +695,12 @@ class ConformerEngine:
     def transcribe_beam(self, waves: Sequence[np.ndarray], beam_size: int = 300, cutoff_prob: float = 0.99,
                         cutoff_top_n: int = 40, use_db_normalization: bool = True, target_db: float = -20.0, lm=None,
                         alpha: float = 0.0, beta: float = 0.0, rates: Optional[Sequence[int]] = None, onsets: bool = False,
-                        hotwords=None):
+                        hotwords=None, n_best=None):
         """Host waveforms -> (token ids per utterance, log-scores) with the GPU prefix beam search (``lm``, ``hotwords``:
-        see ctc_beam; ``rates``: see transcribe; ``onsets``: see beam_features)."""
+        see ctc_beam; ``rates``: see transcribe; ``onsets``, ``n_best``: see beam_features)."""
         feats, frames, status = self.fbank(waves, use_db_normalization, target_db, rates=rates)
-        return self.beam_features(feats, frames, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta, onsets, hotwords)
+        return self.beam_features(feats, frames, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta, onsets, hotwords,
+                                  n_best)
 
     def transcribe_beam_pipelined(self, batches, beam_size: int = 300, cutoff_prob: float = 0.99, cutoff_top_n: int = 40,
                                   use_db_normalization: bool = True, target_db: float = -20.0, lm=None, alpha: float = 0.0,
@@ -771,19 +775,23 @@ class ConformerEngine:
             yield finish(prev)
 
     def beam_features(self, feats, frames, beam_size: int = 300, cutoff_prob: float = 0.99, cutoff_top_n: int = 40, lm=None,
-                      alpha: float = 0.0, beta: float = 0.0, onsets: bool = False, hotwords=None):
+                      alpha: float = 0.0, beta: float = 0.0, onsets: bool = False, hotwords=None, n_best=None):
         """-> (token ids per utterance, log-scores); ``onsets``: also the onset frame of every token per utterance
-        (BeamSearch.frames), as a third element; ``hotwords``: see ctc_beam."""
+        (BeamSearch.frames), as a third element; ``hotwords``: see ctc_beam; ``n_best`` (1..beam_size): also, last, the
+        ``n_best`` best (token ids, log-score) of every utterance, best first, entry 0 its reported result (nbest_lists)."""
         B = feats.shape[0]
         enc, tl, T, ws = self.encode(feats, frames)
         if T == 0:
-            return ([[] for _ in range(B)], [0.0] * B) + (([[] for _ in range(B)],) if onsets else ())
-        tok, n, sc = self.ctc_beam(enc, tl, T, ws, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta, hotwords)
+            toks, scores = [[] for _ in range(B)], [0.0] * B
+            return (toks, scores) + (([[] for _ in range(B)],) if onsets else ()) + (
+                (nbest_lists(None, self, B, n_best, toks, scores),) if n_best is not None else ())
+        tok, n, sc = self.ctc_beam(enc, tl, T, ws, beam_size, cutoff_prob, cutoff_top_n, lm, alpha, beta, hotwords, n_best)
         fr = ws["beam"].frames(self, B).cpu().numpy() if onsets else None
         tok, n, sc = tok.cpu().numpy(), n.cpu().numpy(), sc.cpu().numpy()
         self.d2h_bytes += tok.nbytes + n.nbytes + sc.nbytes + (0 if fr is None else fr.nbytes)
         out = [tok[b, :n[b]].tolist() for b in range(B)], [float(s) for s in sc]
-        return out + (([fr[b, :n[b]].tolist() for b in range(B)],) if onsets else ())
+        out = out + (([fr[b, :n[b]].tolist() for b in range(B)],) if onsets else ())
+        return out + ((nbest_lists(ws["beam"], self, B, n_best, out[0], out[1]),) if n_best is not None else ())
 
     # ---- public batched entry points -----------------------------------------------------------
     def transcribe(self, waves: Sequence[np.ndarray], use_db_normalization: bool = True, target_db: float = -20.0,
@@ -1269,9 +1277,10 @@ class StreamBeam(BeamSearch):
         """``reset_decoder`` (beam_search_decoder.py:93-96)."""
         self.seen = 0
 
-    def push(self, logits: torch.Tensor, rows: int):
+    def push(self, logits: torch.Tensor, rows: int, n_best=None):
         """CTC-head logits [>= rows, ld] of the new chunk's frames -> (token ids of the best prefix so far, its log score);
-        ``onsets()`` reads out the frames of those tokens."""
+        ``onsets()`` reads out the frames of those tokens.  ``n_best``: also, third, the ``n_best`` best (token ids,
+        log score) so far, best first, entry 0 the first two (nbest_lists)."""
         if rows > self.max_chunk:
             raise ValueError(f"a chunk has at most {self.max_chunk} frames")
         if self.seen + rows > self.max_frames:
@@ -1285,13 +1294,35 @@ class StreamBeam(BeamSearch):
         n = int(oh[1].view(torch.int32).item())
         toks = self.out_tok[0, :n].cpu().tolist() if n else []
         self.eng.d2h_bytes += 8 + 4 * n
-        return toks, float(oh[0].item())
+        if n_best is None:
+            return toks, float(oh[0].item())
+        return toks, float(oh[0].item()), nbest_lists(self, self.eng, 1, n_best, [toks], [float(oh[0].item())])[0]
 
     def onsets(self) -> List[int]:
         """The onset frame (since the last ``reset``) of every token of the best prefix the last ``push`` reported."""
         n = int(self.count[0].item())
         self.eng.d2h_bytes += 4 * n
         return self.frames(self.eng, 1)[0, :n].cpu().tolist() if n else []
+
+
+def nbest_lists(bs, eng, B: int, n_best: int, toks, scores):
+    """The ``n_best`` best hypotheses of slots 0..B-1 of the STREAM / POOL search ``bs`` after its last search -> per slot
+    a list of (token ids, log score), best first, at most ``n_best`` long: ``BeamSearch.nbest``, one launch, then the
+    counts and the tokens copied to the host.  Entry 0 is always (toks[b], scores[b]), the slot's reported result: the
+    read-out's hypothesis 0 is that bit for bit, and a slot with no hypothesis (no frames searched) gets just it.
+    n_best = 1 (or ``bs`` None) launches nothing."""
+    if n_best == 1 or bs is None:
+        return [[(list(toks[b]), scores[b])] for b in range(B)]
+    tok, cnt, sc, _, nh = bs.nbest(eng, B, n_best)
+    nh, cnt, sc = nh[:B].cpu().numpy(), cnt[:B].cpu().numpy(), sc[:B].cpu().numpy()
+    L = int(cnt.max()) if cnt.size else 0
+    tk = tok[:B, :, :L].cpu().numpy()
+    eng.d2h_bytes += nh.nbytes + cnt.nbytes + sc.nbytes + tk.nbytes
+    out = []
+    for b in range(B):
+        lst = [(tk[b, h, :cnt[b, h]].tolist(), float(sc[b, h])) for h in range(int(nh[b]))]
+        out.append(lst if lst else [(list(toks[b]), scores[b])])
+    return out
 
 
 def greedy_score(psum: np.float32, pcount: int) -> float:

@@ -12,6 +12,9 @@ Hotwords (``decoder: ctc_beam_search`` only): ``MASRPredictor(..., hotwords=[...
 inside the GPU prefix beam search (masr_b200/hotwords.py) for every call; ``predict``, ``predict_batch`` and
 ``predict_long`` take a per-call ``hotwords=`` that overrides the list (``[]``: none), and each slot of
 ``create_stream_pool`` can have its own (``StreamPool.set_hotwords``).  Scores never include the hotword credit.
+N-best (``decoder: ctc_beam_search`` only): ``predict``, ``predict_batch`` and ``predict_stream`` take ``n_best=``, and
+``create_stream_pool`` takes it for every slot; the result then also carries ``'n_best'``, the best hypotheses of the
+search as ``[{'text', 'score'}, ...]``, best first, entry 0 the result's own text and score.
 Audio at other sample rates than 16 kHz is resampled on the GPU, as the reference's featurizer does
 (audio_featurizer.py:45-47), when the predictor is built with ``resample=True``; by default a rate mismatch raises.
 Out of the hot-path scope and therefore explicit errors here: punctuation (``use_pun``), inverse
@@ -31,7 +34,8 @@ from . import SUPPORT_MODEL
 from .audio import load_audio, pcm_bytes_to_float32, samples_to_float32
 from .engine import ConformerEngine, EfficientConformerEngine, greedy_score, subsampled_len
 from .resample import MODEL_RATE, needs_resampling
-from .text import TextFeaturizer, ids_to_text
+from .beam import check_n_best
+from .text import TextFeaturizer, ids_to_text, nbest_dicts
 from . import timestamps as ts
 
 logger = logging.getLogger(__name__)
@@ -211,6 +215,14 @@ class MASRPredictor:
         """The per-call ``hotwords=``: None keeps the predictor's list, a list (``[]`` included) replaces it."""
         return self._hotwords if hotwords is None else self._graph(hotwords)
 
+    def _n_best(self, n_best):
+        """The per-call ``n_best``: None, or an int in 1..beam_size (a ValueError otherwise, and for greedy decoding)."""
+        if n_best is None:
+            return None
+        if self._beam_conf is None:
+            raise ValueError("n_best needs the prefix beam search (decoder: ctc_beam_search), not ctc_greedy")
+        return check_n_best(n_best, self._beam_conf['beam_size'])
+
     def _check_rate(self, sr):
         if sr != self._sample_rate and not self._resample:
             raise Exception(f"masr_b200: resampling is outside the hot-path scope (got {sr} Hz, model expects "
@@ -233,32 +245,45 @@ class MASRPredictor:
             raise Exception("masr_b200: inverse text normalisation (is_itn) is outside the hot-path scope")
         return text
 
-    def predict(self, audio_data, use_pun=False, is_itn=False, sample_rate=16000, timestamps=False, hotwords=None):
+    def predict(self, audio_data, use_pun=False, is_itn=False, sample_rate=16000, timestamps=False, hotwords=None,
+                n_best=None):
         """Whole-utterance recognition (predict.py:167-192).  ``timestamps``: the result also carries ``'tokens'``
         (``[{'token', 'start', 'end'}]``, seconds) and, when the vocabulary has ``<space>``, ``'words'``
-        (masr_b200/timestamps.py).  ``hotwords``: this call's list (None: the predictor's; ``[]``: none)."""
-        r = self._recognise(*self._load_batch([audio_data], sample_rate), timestamps, hotwords=self._call_graph(hotwords))[0]
+        (masr_b200/timestamps.py).  ``hotwords``: this call's list (None: the predictor's; ``[]``: none).
+        ``n_best`` (1..beam_size): the result also carries ``'n_best'``, at most ``n_best`` hypotheses ``{'text',
+        'score'}`` in the order the search ranks them, entry 0 the result itself.  Their scores are what ``'score'`` is:
+        the log probability, or approx_ctc with an LM (the ranking is by the fused score then, so those need not
+        decrease down the list).  Timestamps are only for the result itself."""
+        n_best = self._n_best(n_best)
+        r = self._recognise(*self._load_batch([audio_data], sample_rate), timestamps, hotwords=self._call_graph(hotwords),
+                            n_best=n_best)[0]
         r['text'] = self._finish(r['text'], use_pun, is_itn)
         return r
 
-    def predict_batch(self, audio_list: Sequence, sample_rate=16000, timestamps=False, hotwords=None):
+    def predict_batch(self, audio_list: Sequence, sample_rate=16000, timestamps=False, hotwords=None, n_best=None):
         """Additive: a list of utterances in one GPU pass; element i equals ``predict(audio_list[i])``.  With
-        ``resample=True`` the rows may have different rates (WAV files carry their own).  ``timestamps``, ``hotwords``: as
-        in predict."""
-        return self._recognise(*self._load_batch(audio_list, sample_rate), timestamps, hotwords=self._call_graph(hotwords))
+        ``resample=True`` the rows may have different rates (WAV files carry their own).  ``timestamps``, ``hotwords``,
+        ``n_best``: as in predict."""
+        n_best = self._n_best(n_best)
+        return self._recognise(*self._load_batch(audio_list, sample_rate), timestamps, hotwords=self._call_graph(hotwords),
+                               n_best=n_best)
 
-    def _recognise(self, waves, rates, timestamps=False, offsets=None, hotwords=None):
-        """Waveforms -> ``[{'text', 'score'}]`` (+ token and word times, shifted by ``offsets[i]`` seconds)."""
+    def _recognise(self, waves, rates, timestamps=False, offsets=None, hotwords=None, n_best=None):
+        """Waveforms -> ``[{'text', 'score'}]`` (+ token and word times, shifted by ``offsets[i]`` seconds; + ``'n_best'``)."""
         vocab = self._text_featurizer.vocab_list
         dt = ts.frame_seconds(self.predictor)
         offsets = offsets or [0.0] * len(waves)
         if self._beam_conf is not None:
             out = self.predictor.transcribe_beam(waves, use_db_normalization=self._use_db, target_db=self._target_db,
-                                                 rates=rates, onsets=timestamps, hotwords=hotwords, **self._beam_conf)
+                                                 rates=rates, onsets=timestamps, hotwords=hotwords, n_best=n_best,
+                                                 **self._beam_conf)
             res = [{'text': ids_to_text(t, vocab), 'score': s} for t, s in zip(out[0], out[1])]
             if timestamps:
                 for r, t, f, off in zip(res, out[0], out[2], offsets):
                     ts.beam_result(r, t, f, vocab, dt, off)
+            if n_best is not None:
+                for r, hyps in zip(res, out[-1]):
+                    r['n_best'] = nbest_dicts(hyps, vocab)
             return res
         g = self.predictor.transcribe(waves, self._use_db, self._target_db, return_frames=timestamps, rates=rates)
         self._raise_status(g.status)
@@ -345,10 +370,11 @@ class MASRPredictor:
 
     # ---------------------------------------------------------------------------------------------
     def predict_stream(self, audio_data, is_end=False, use_pun=False, is_itn=False, channels=1, samp_width=2,
-                       sample_rate=16000, timestamps=False):
+                       sample_rate=16000, timestamps=False, n_best=None):
         """Streaming recognition, one push of audio per call (predict.py:237-343).  Returns ``None``
         while fewer than 67 feature frames are buffered, else the running ``{'text','score'}``; ``timestamps``: with
-        ``'tokens'`` (+ ``'words'``) as in predict, timed since the last ``reset_stream``."""
+        ``'tokens'`` (+ ``'words'``) as in predict, timed since the last ``reset_stream``; ``n_best``: with ``'n_best'`` as
+        in predict, over the frames seen so far."""
         if not self.configs.streaming:
             raise Exception(
                 f"不支持改该模型流式识别，当前模型：{self.configs.use_model}，参数streaming为：{self.configs.streaming}")
@@ -361,6 +387,7 @@ class MASRPredictor:
         else:
             raise Exception(f'不支持该数据类型，当前数据类型为：{type(audio_data)}')
         self._check_rate(sample_rate)
+        n_best = self._n_best(n_best)
         self.remained_wav = new if self.remained_wav is None else np.concatenate([self.remained_wav, new])
         if sample_rate != self._sample_rate:
             # predict.py:267-274: the buffer (the carried-over tail, already at 16 kHz, plus the new chunk) is labelled with
@@ -396,7 +423,9 @@ class MASRPredictor:
                 if self._sbeam is None:
                     from .engine import StreamBeam
                     self._sbeam = StreamBeam(eng, hotwords=self._hotwords, **self._beam_conf)
-                self._sbeam_result = self._sbeam.push(self._stream.last_logits, int(ids.shape[0]))
+                rows = int(ids.shape[0])
+                self._sbeam_result = self._sbeam.push(self._stream.last_logits, rows) if n_best is None else \
+                    self._sbeam.push(self._stream.last_logits, rows, n_best=n_best)
                 continue
             ids_h = ids.cpu().numpy()
             mp_h = maxp.cpu().numpy()
@@ -405,11 +434,16 @@ class MASRPredictor:
         self.cached_feat = self.cached_feat[end - CACHED_FEATURE_NUM:]
         vocab, dt = self._text_featurizer.vocab_list, ts.frame_seconds(eng)
         if self._beam_conf is not None:
-            toks, score = self._sbeam_result
+            toks, score = self._sbeam_result[:2]
             if is_itn:
                 raise Exception("masr_b200: inverse text normalisation (is_itn) is outside the hot-path scope")
             r = {'text': ids_to_text(toks, vocab), 'score': score}
-            return ts.beam_result(r, toks, self._sbeam.onsets() if toks else [], vocab, dt) if timestamps else r
+            if timestamps:
+                ts.beam_result(r, toks, self._sbeam.onsets() if toks else [], vocab, dt)
+            if n_best is not None:
+                hyps = self._sbeam_result[2] if len(self._sbeam_result) > 2 else [(toks, score)]
+                r['n_best'] = nbest_dicts(hyps[:n_best], vocab)
+            return r
         # greedy_decoder_chunk re-collapses the whole history (ctc_greedy_decoder.py:81-88)
         toks, prev = [], None
         for i in self._hist_ids:
@@ -429,7 +463,7 @@ class MASRPredictor:
         return ts.greedy_result(r, self._hist_ids, vocab, dt) if timestamps else r
 
     def create_stream_pool(self, n_slots: int, max_frames: int = 3000, vad_model_path=None, vad_options=None,
-                           timestamps=False, max_hotword_nodes: int = 0):
+                           timestamps=False, max_hotword_nodes: int = 0, n_best=None):
         """Additive: a ``StreamPool`` of ``n_slots`` concurrent streams over this predictor's model, decoding as the YAML
         says — greedy, or the GPU prefix beam search with the character or word LM this predictor loaded (if any).  Each slot's
         ``push`` results equal ``predict_stream`` on that stream alone.  ``max_frames``: encoder frames one stream may reach
@@ -444,10 +478,13 @@ class MASRPredictor:
 
         Hotwords: every slot boosts this predictor's list; ``max_hotword_nodes`` > 0 gives each slot room for its own list
         of up to that many automaton nodes (a list of n hotwords of k characters takes at most n * k + 1), set with
-        ``set_hotwords(slot, hotwords)`` right after the slot's reset."""
+        ``set_hotwords(slot, hotwords)`` right after the slot's reset.
+
+        ``n_best``: every result (with the VAD, every segment and partial) also carries ``'n_best'`` as in predict."""
         if not self.configs.streaming:
             raise Exception(f"不支持改该模型流式识别，当前模型：{self.configs.use_model}，参数streaming为：{self.configs.streaming}")
         from .stream_pool import StreamPool
+        n_best = self._n_best(n_best)
         beam = self._beam_conf
         if beam is not None and (self._hotwords is not None or max_hotword_nodes > 0):
             beam = dict(beam, hotwords=self._hotwords, max_hotword_nodes=int(max_hotword_nodes))
@@ -455,7 +492,7 @@ class MASRPredictor:
             raise ValueError("hotwords need the prefix beam search (decoder: ctc_beam_search), not ctc_greedy")
         pool = StreamPool(self.predictor, self._text_featurizer.vocab_list, n_slots, use_db_normalization=self._use_db,
                           target_db=self._target_db, max_frames=max_frames, beam=beam, resample=self._resample,
-                          timestamps=timestamps, hotword_score=self._hotword_score)
+                          timestamps=timestamps, hotword_score=self._hotword_score, n_best=n_best)
         if vad_model_path is None:
             return pool
         from .segment_pool import SegmentingStreamPool

@@ -128,7 +128,8 @@ class SegmentingStreamPool:
     ``push(audio, is_end=False)`` -> per pushed slot ``{'segments': [{'start', 'end', 'text', 'score'}, ...] (closed
     during this push), 'partial': {'start', 'text', 'score'} | None (the open segment's latest result), 'speech': bool}``.
     With a pool made with ``timestamps=True`` segments and partials also carry ``'tokens'`` (+ ``'words'``), timed in
-    seconds since the slot's stream started.
+    seconds since the slot's stream started, and with a pool made with ``n_best`` they carry ``'n_best'`` (the
+    segment's or partial's best hypotheses, ``[{'text', 'score'}, ...]``, entry 0 its own text and score).
     ``is_end`` (one bool or ``{slot: bool}``) ends a slot's stream: its open segment closes at the last received sample and
     the slot starts a new stream (with an empty transcript) on its next push.  ``transcript(slot)`` joins the closed
     segments as ``predict_long`` does.  Per-slot errors (undecodable input, a rate other than 16 kHz, a failure of the slot's recognition) fail only
@@ -250,13 +251,15 @@ class SegmentingStreamPool:
                         if self.pool.timestamps:
                             rec.update({k: v for k, v in got.items() if k in ("tokens", "words")} if got is not None
                                        else {"tokens": []})
+                        if self.pool.n_best is not None:
+                            rec["n_best"] = got["n_best"] if got is not None else [{"text": "", "score": 0.0}]
                         self.closed[s].append(rec)
                         seg_out[s].append(rec)
                         self.partial[s] = None
                         self.pool.reset_stream(s)
                     elif got is not None:
                         self.partial[s] = {"start": self.planners[s].open, "text": got["text"], "score": got["score"]}
-                        self.partial[s].update({k: got[k] for k in ("tokens", "words") if k in got})
+                        self.partial[s].update({k: got[k] for k in ("tokens", "words", "n_best") if k in got})
         for s in failed:                              # the slot's stream is abandoned: start it over
             self._clear([s])
         out: Dict[int, dict] = {}

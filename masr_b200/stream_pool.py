@@ -21,12 +21,12 @@ import torch
 
 from ._lib import EPI_BIAS, EPI_BIAS_GLU, EPI_RESIDUAL
 from .audio import pcm_bytes_to_float32, samples_to_float32
-from .beam import POOL, BeamSearch
+from .beam import POOL, BeamSearch, check_n_best
 from .hotwords import HotwordBuffer, graph_or_none
-from .engine import ConformerEngine, _p, greedy_score, subsampled_len
+from .engine import ConformerEngine, _p, greedy_score, nbest_lists, subsampled_len
 from .predict import CACHED_FEATURE_NUM, DECODING_WINDOW, FRAME_SHIFT, chunk_starts
 from .resample import MODEL_RATE, output_length
-from .text import ids_to_text
+from .text import ids_to_text, nbest_dicts
 from . import timestamps as ts
 
 CHUNK_FRAMES = DECODING_WINDOW          # 67 feature frames -> 16 encoder frames
@@ -621,11 +621,14 @@ class PoolBeam(BeamSearch):
         self.topk(self.eng, self.logits, self.eng.Vpad, self.slots * self.R)
         self.search(self.eng, self.lens, self.slots, self.R)
 
-    def results(self, slots: Sequence[int], frames: Sequence[int], onsets: bool = False) -> Dict[int, tuple]:
+    def results(self, slots: Sequence[int], frames: Sequence[int], onsets: bool = False,
+                n_best: Optional[int] = None) -> Dict[int, tuple]:
         """slot -> (token ids of its best prefix, score) after the last step: one D2H copy of every slot's count and score,
         then one of the token rows spanning `slots`.  ``frames[slot]``: the slot's encoder frames since its reset; a slot
         without any gets ([], 0.0), as ``predict_stream`` does.  ``onsets``: each with a third element, the tokens' onset
-        frames since the slot's reset (one read-out launch here, outside the step graph, and one more copy)."""
+        frames since the slot's reset (one read-out launch here, outside the step graph, and one more copy).  ``n_best``
+        (1..beam_size): each with a last element, the slot's ``n_best`` best (token ids, score), best first, entry 0 the
+        first two (``engine.nbest_lists``: one read-out launch here, outside the step graph; none for n_best = 1)."""
         slots = list(slots)
         if not slots:
             return {}
@@ -647,6 +650,11 @@ class PoolBeam(BeamSearch):
                 out[s] = (toks[s - lo, :n[s]].tolist() if n[s] else [], float(score[s]))
             if onsets:
                 out[s] += (fr[s - lo, :len(out[s][0])].tolist() if out[s][0] else [],)
+        if n_best is not None:
+            nb = nbest_lists(self if had else None, eng, hi, n_best, [out.get(s, ([], 0.0))[0] for s in range(hi)],
+                             [out.get(s, ([], 0.0))[1] for s in range(hi)])
+            for s in slots:
+                out[s] += (nb[s] if frames[s] > 0 else [([], 0.0)],)
         return out
 
 
@@ -662,7 +670,7 @@ class StreamPool:
 
     def __init__(self, eng: ConformerEngine, vocab: Sequence[str], n_slots: int, use_db_normalization: bool = True,
                  target_db: float = -20.0, max_frames: int = 3000, beam: Optional[dict] = None, use_graph: bool = True,
-                 resample: bool = False, timestamps: bool = False, hotword_score: float = 1.5):
+                 resample: bool = False, timestamps: bool = False, hotword_score: float = 1.5, n_best: Optional[int] = None):
         """``beam``: None decodes greedily (``ctc_greedy``); a dict ``{beam_size, cutoff_prob, cutoff_top_n, lm, alpha,
         beta}`` (``MASRPredictor``'s ``ctc_beam_search`` settings; ``lm`` a ``CharLM``, ``WordLM`` or None) runs the streaming prefix
         beam search of every slot on the GPU (``PoolBeam``), and every result is the beam's, as ``predict_stream`` with
@@ -675,7 +683,16 @@ class StreamPool:
 
         Hotwords (beam search only): ``beam`` may also carry ``hotwords`` (the pool default, a ``HotwordGraph``) and
         ``max_hotword_nodes`` (automaton nodes each slot's own list may take; ``HotwordBuffer.bytes_per_node`` bytes of
-        device memory per node, per slot).  ``set_hotwords`` gives a slot its own list, scored ``hotword_score`` per token."""
+        device memory per node, per slot).  ``set_hotwords`` gives a slot its own list, scored ``hotword_score`` per token.
+
+        ``n_best`` (beam search only, 1..beam_size): every result also carries ``'n_best'``, the slot's ``n_best`` best
+        hypotheses so far as ``[{'text', 'score'}, ...]``, best first, entry 0 the result's own text and score (one
+        read-out launch per push, outside the step graph; scores as ``'score'``: approx_ctc with an LM, so they need not
+        decrease down the list)."""
+        if n_best is not None:
+            if beam is None:
+                raise ValueError("n_best needs the prefix beam search (decoder: ctc_beam_search)")
+            check_n_best(n_best, beam.get("beam_size", 300))
         self.eng, self.vocab, self.S = eng, list(vocab), n_slots
         self.timestamps, self.dt, self.t0 = bool(timestamps), ts.frame_seconds(eng), [0.0] * n_slots
         self.resample = bool(resample)
@@ -687,6 +704,7 @@ class StreamPool:
             self.beam = PoolBeam(self.pool, **beam)
             self.pool.beam = self.beam
         self.hotword_score = hotword_score
+        self.n_best = None if n_best is None else int(n_best)
         self.use_db, self.target_db = use_db_normalization, target_db
         self.remained: List[Optional[np.ndarray]] = [None] * n_slots
         dev = eng.device
@@ -910,8 +928,8 @@ class StreamPool:
                 ids, maxp, tout = self.pool.step(batch, nfr)
                 if self.beam is None:                # (the beam's state stays on the device: no copy per round)
                     self._fold(ids.cpu().numpy(), maxp.cpu().numpy(), tout)
-            beam_out = self.beam.results([s for s in live if pending[s]], self.pool.lens_host, self.timestamps) \
-                if self.beam is not None else None
+            beam_out = self.beam.results([s for s in live if pending[s]], self.pool.lens_host, self.timestamps,
+                                         self.n_best) if self.beam is not None else None
             for s in live:
                 if not pending[s]:
                     out[s] = None
@@ -924,6 +942,8 @@ class StreamPool:
                     out[s] = {"text": ids_to_text(toks, self.vocab), "score": score}
                     if self.timestamps:
                         ts.beam_result(out[s], toks, beam_out[s][2], self.vocab, self.dt, self.t0[s])
+                    if self.n_best is not None:
+                        out[s]["n_best"] = nbest_dicts(beam_out[s][-1], self.vocab)
                 else:
                     out[s] = {"text": ids_to_text(self.toks[s], self.vocab), "score": greedy_score(self.acc[s], int(self.nprob[s]))}
                     if self.timestamps:

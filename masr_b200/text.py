@@ -32,3 +32,8 @@ class TextFeaturizer:
 def ids_to_text(ids: Sequence[int], vocabulary: Sequence[str]) -> str:
     """ctc_greedy_decoder.py:26,31."""
     return "".join(vocabulary[i] for i in ids).replace("<space>", " ")
+
+
+def nbest_dicts(hyps, vocabulary: Sequence[str]) -> List[dict]:
+    """[(token ids, score)], best first -> the ``'n_best'`` entries [{'text', 'score'}] of a result."""
+    return [{"text": ids_to_text(t, vocabulary), "score": float(s)} for t, s in hyps]
